@@ -88,9 +88,9 @@ enum mmmot_weight_id {
   MMMOT_W_NE_W1T = 129, MMMOT_W_NE_B1 = 130, MMMOT_W_NE_G1W = 131, MMMOT_W_NE_G1B = 132,
   MMMOT_W_NE_W2T = 133, MMMOT_W_NE_B2 = 134, MMMOT_W_NE_G2W = 135, MMMOT_W_NE_G2B = 136,
   MMMOT_W_NE_W3 = 137, MMMOT_W_NE_B3 = 138,
-  /* ---- tensor-core operands: the same matrices split into FP16 hi/lo and pre-tiled in the UMMA
+  /* ---- tensor-core operands: the same matrices split into FP16 hi/lo and pre-tiled in the wgmma
      canonical K-major core-matrix layout  [k chunk 32][m tile 128][hi|lo][k group 4][m group 16][8][8]
-     (zero padded to multiples of 128 rows / 32 k); see csrc/gemm_tc.cuh.  VGG layer 0 (fp32 NCHW crops) uses
+     (zero padded to multiples of 128 rows / 32 k); see weights.py::pack_tc.  VGG layer 0 (fp32 NCHW crops) uses
      the K order k = ci*9 + (ky*3+kx); layers 1..12 (packed FP16 NHWC activations) use k = (ky*3+kx)*Cin + ci. */
   MMMOT_W_VGG_WP0 = 139,          /* .. +12 */
   MMMOT_W_PN_WP1 = 152,           /* .. +4 : PointNet trunk layers 1..5 */
@@ -295,7 +295,7 @@ int mmmot_set_kseg(int chunks);
  *   bit 6 (64)   64-channel layers on the channel-major kernel instead of the pixel-major one
  *   bit 7 (128)  pixel-major epilogue with 16-byte stores instead of whole 32-byte sectors
  *   bit 8 (256)  pixel-major kernel without halo boxes (nine boxes per channel chunk)
- *   bit 9 (512)  no fused max-pool in the pixel-major epilogue
+ *   bit 9 (512)  no fused max-pool in the conv epilogues (separate max-pool kernel)
  *   bit 14 (16384) first VGG layer with a separate im2col pre-pass instead of in-kernel operand producers */
 int mmmot_set_debug(int flags);
 
@@ -318,6 +318,30 @@ int mmmot_debug_linear_planar(const void* Wp, float wp_scale, const float* bias,
 int mmmot_debug_conv_planar(const void* Wp, float wp_scale, const float* bias, const void* Xhi, void* Yhi,
                             int n_img, int H, int W, int C, int M, float* kseg_scratch /* fp32 [n*H*W][M] or NULL */,
                             void* stream);
+
+/* Test hooks of the VGG trunk's convolutions, run through the same launch code as mmmot_appearance_fwd.
+ * conv_plan: the launch plan of one 3x3 conv layer (n_img x H x W, C -> M channels), computed on the host without any
+ *   CUDA call, under the current mmmot_set_debug / mmmot_set_kseg state.  want_pool: the caller takes a fused 2x2
+ *   max-pool; use_kseg: the caller provides K-segment scratch.  plan[8] (host) = {pixel-major kernel, halo boxes,
+ *   fused pool, box x, box y, box images, K segments, column tiles}.
+ * conv_layer: 3x3 pad 1 + bias + ReLU on NHWC planes X[2][n][H][W][C] (x_plane apart) -> Y[2][n][H][W][M] (y_plane
+ *   apart), or, when *did_pool (host) comes back 1, the 2x2 max-pooled map Y[2][n][H/2][W/2][M] (y_plane_pooled apart;
+ *   y_plane_pooled > 0 and did_pool != NULL ask for the fused pool).  Wpx (or NULL): compact N = 64 tiles of a 64-output
+ *   layer (weights.py::pack_px).  pool_sum (or NULL): [n][M] per-image sums of the pooled map in 2^-32 fixed point,
+ *   accumulated (the caller zeroes it), filled only when the channel-major kernel fuses the pool.  kseg_scratch (or NULL):
+ *   fp32 [column tiles * 256][M].  status: a status word (bit 0 = FP16 range).  plan (host, or NULL): as conv_plan.
+ * vgg_conv0: the first VGG layer, fp32 NCHW crops [n][3][H][W] -> Y[2][n][H][W][64] (y_plane apart), bias + ReLU.
+ *   wt [27][64] fp32 (k = (ky*3+kx)*3 + ci, debug bit 5), Wp / Wpx packed tiles with k = ci*9 + ky*3 + kx, cols
+ *   [2][n*H*W][32] FP16 scratch of the im2col variant.  variant (host, or NULL) receives 0 = taps generated in the
+ *   contraction kernel, 1 = im2col + matrix contraction, 2 = FP32 FFMA. */
+int mmmot_debug_conv_plan(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg, int* plan);
+int mmmot_debug_conv_layer(const void* Wp, const void* Wpx, float wp_scale, const float* bias, const void* Xhi, long x_plane,
+                           int n_img, int H, int W, int C, int M, void* Yhi, long y_plane, long y_plane_pooled,
+                           int* did_pool, unsigned long long* pool_sum, float* kseg_scratch, int* status, int* plan,
+                           void* stream);
+int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const float* wt, const float* bias, const void* Wp,
+                          float wp_scale, const void* Wpx, void* Yhi, long y_plane, void* cols, int* status, int* variant,
+                          void* stream);
 
 /* Per-launch timing of the hot kernels with CUDA events on the launching stream; used by bench.py's roofline
  * figures.  Every timed launch carries a tag = (stage, layer) — mmmot_timing_tag_count() tags, named by

@@ -58,6 +58,10 @@ SIGNATURES = {
     "mmmot_debug_linear": (_i, [_vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mmmot_debug_linear_planar": (_i, [_vp, _f, _vp, _vp, _vp, _i, _i, _l, _vp]),
     "mmmot_debug_conv_planar": (_i, [_vp, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "mmmot_debug_conv_plan": (_i, [_i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(_i)]),
+    "mmmot_debug_conv_layer": (_i, [_vp, _vp, _f, _vp, _vp, _l, _i, _i, _i, _i, _i, _vp, _l, _l, ctypes.POINTER(_i), _vp, _vp,
+                                    _vp, ctypes.POINTER(_i), _vp]),
+    "mmmot_debug_vgg_conv0": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _vp, _vp, _l, _vp, _vp, ctypes.POINTER(_i), _vp]),
     "mmmot_timing_enable": (_i, [_i]),
     "mmmot_timing_tag_count": (_i, []),
     "mmmot_timing_tag_name": (ctypes.c_char_p, [_i]),

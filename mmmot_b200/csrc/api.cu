@@ -230,3 +230,33 @@ extern "C" int mmmot_debug_conv_planar(const void* Wp, float wp_scale, const flo
   return gemm_tma_launch_conv(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, (long)n_img * H * W * C, n_img, H, W, C,
                               (__half*)Yhi, (long)n_img * H * W * M, (cudaStream_t)stream, kseg_scratch);
 }
+
+static void conv_plan_words(const ConvPlan& c, int* plan) {
+  const int v[8] = {c.px, c.halo, c.pool, c.bx, c.by, c.bi, c.ksegs, c.num_tiles};
+  for (int i = 0; i < 8; i++) plan[i] = v[i];
+}
+
+// The launch plan gemm_tma_launch_conv takes for one VGG layer, computed on the host without any CUDA call.
+extern "C" int mmmot_debug_conv_plan(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg, int* plan) {
+  if (!plan || n_img <= 0 || H <= 0 || W <= 0 || C <= 0 || C % tc::BK || M <= 0) return MMMOT_E_ARG;
+  conv_plan_words(conv_plan(M, false, n_img, H, W, C, want_pool != 0, use_kseg != 0, mm_debug_flags(), mm_kseg_chunks()),
+                  plan);
+  return 0;
+}
+
+// One VGG conv layer (3x3 pad 1 + bias + ReLU) through gemm_tma_launch_conv with the arguments mmmot_appearance_fwd
+// passes it.
+extern "C" int mmmot_debug_conv_layer(const void* Wp, const void* Wpx, float wp_scale, const float* bias, const void* Xhi,
+                                      long x_plane, int n_img, int H, int W, int C, int M, void* Yhi, long y_plane,
+                                      long y_plane_pooled, int* did_pool, unsigned long long* pool_sum, float* kseg_scratch,
+                                      int* status, int* plan, void* stream) {
+  if (!Wp || !bias || !Xhi || !Yhi || n_img <= 0 || H <= 0 || W <= 0 || M <= 0) return MMMOT_E_ARG;
+  GemmP p = gemm_defaults();
+  p.bias = bias; p.M = M; p.relu = 1;
+  ConvPlan c;
+  const int rc = gemm_tma_launch_conv(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, x_plane, n_img, H, W, C,
+                                      (__half*)Yhi, y_plane, (cudaStream_t)stream, kseg_scratch, y_plane_pooled, did_pool,
+                                      status, pool_sum, (const uint4*)Wpx, &c);
+  if (plan && rc != MMMOT_E_ARG) conv_plan_words(c, plan);
+  return rc;
+}

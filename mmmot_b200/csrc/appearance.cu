@@ -266,7 +266,51 @@ __global__ void __launch_bounds__(128) skip_head_kernel(
   feats[(((long)pair * 3 + 0) * 512 + head * 128 + t) * L + l] = o;
 }
 
+// First VGG layer (3 -> 64, bias + ReLU): fp32 NCHW crops -> FP16 hi/lo NHWC planes Y[2][n][H][W][64], y_plane apart.
+//   FFMA (debug bit 32): conv0_packed_kernel on wt [(ky*3+kx)*3 + ci][64]
+//   GEN27: taps generated by the contraction kernel's producers (needs the compact Wpx, H*W % 256 == 0, W <= 512)
+//   otherwise (or debug bit 16384): im2col27_kernel into cols [2][n*H*W][32] + the matrix contraction on Wp (and Wpx)
+// variant (optional) receives 0 = GEN27, 1 = im2col + matrix, 2 = FFMA.
+static int vgg_conv0_launch(const float* crops, int n_img, int H, int W, const float* wt, const float* bias, const uint4* Wp,
+                            float wp_scale, const uint4* Wpx, __half* Y, long y_plane, __half* cols, int* status,
+                            int* variant, cudaStream_t st) {
+  const long n_pix = (long)n_img * H * W;
+  const int dbg = mm_debug_flags();
+  if (dbg & 32) {   // A/B: direct FP32 FFMA first layer
+    if (variant) *variant = 2;
+    if (!wt || (W & 1)) return MMMOT_E_ARG;
+    conv0_packed_kernel<<<mm_cdiv(n_pix / 2, 64), 256, 0, st>>>(crops, wt, bias, n_pix / 2, H, W, Y, y_plane, status);
+    MM_LAUNCH_CHECK();
+  } else if (Wpx && !(dbg & 16384) && ((long)H * W) % 256 == 0 && W <= 512) {
+    // taps generated inside the contraction kernel (no im2col matrix in HBM)
+    if (variant) *variant = 0;
+    MM_TRY(gemm_tma_px_launch_gen27(crops, n_img, H, W, Wpx, wp_scale, bias, Y, y_plane, status, st));
+  } else {
+    if (variant) *variant = 1;
+    if (!Wp || !cols) return MMMOT_E_ARG;
+    if (n_pix >= (1L << 31)) return MMMOT_E_SHAPE;
+    im2col27_kernel<<<mm_cdiv(n_pix, 256), 256, 0, st>>>(crops, n_pix, H, W, cols, n_pix * 32, status);
+    MM_LAUNCH_CHECK();
+    GemmP p = gemm_defaults();
+    p.bias = bias; p.M = 64; p.K = 32; p.relu = 1;
+    p.S = (int)n_pix; p.tiles_per_group = mm_cdiv(n_pix, tc::BN); p.num_tiles = p.tiles_per_group;
+    p.Y = reinterpret_cast<float*>(Y); p.y_ms = 64;
+    MM_TRY(gemm_tma_launch_mat(p, Wp, wp_scale, cols, n_pix * 32, n_pix, 32, tma::OUT_PLANAR, y_plane, st, nullptr, status,
+                               nullptr, Wpx));
+  }
+  return 0;
+}
+
 }  // namespace
+
+// Test hook: the first VGG layer exactly as mmmot_appearance_fwd runs it (vgg_conv0_launch).
+extern "C" int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const float* wt, const float* bias,
+                                     const void* Wp, float wp_scale, const void* Wpx, void* Yhi, long y_plane, void* cols,
+                                     int* status, int* variant, void* stream) {
+  if (!crops || !bias || !Yhi || n_img <= 0 || H <= 0 || W <= 0) return MMMOT_E_ARG;
+  return vgg_conv0_launch(crops, n_img, H, W, wt, bias, (const uint4*)Wp, wp_scale, (const uint4*)Wpx, (__half*)Yhi, y_plane,
+                          (__half*)cols, status, variant, (cudaStream_t)stream);
+}
 
 int mm_launch_skip_heads(const mmmot_weights* wts, float* const* pooled, int n_img, int L, float* feats, cudaStream_t st);
 
@@ -317,29 +361,11 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
       if (timed) mm_timing_begin(st, MM_T_VGG0 + i, 2.0 * cout * 9.0 * cin * (double)n_img * h * w,
                                  4.0 * (double)n_img * h * w * (cin + (i == 1 ? cout / 4.0 : cout)));
       if (i == 0) {
-        const long n_pix = (long)n_img * h * w;
-        if (mm_debug_flags() & 32) {   // A/B: direct FP32 FFMA first layer
-          conv0_packed_kernel<<<mm_cdiv(n_pix / 2, 64), 256, 0, st>>>(crops, wts->w[MMMOT_W_VGG_WT0], wts->w[MMMOT_W_VGG_B0],
-                                                                     n_pix / 2, h, w, hb[which], plane_out, status);
-          MM_LAUNCH_CHECK();
-        } else if (wts->w[MMMOT_W_VGG_WPX0] && !(mm_debug_flags() & 16384) && ((long)h * w) % 256 == 0 && w <= 512) {
-          // taps generated inside the contraction kernel (no im2col matrix in HBM)
-          MM_TRY(gemm_tma_px_launch_gen27(crops, n_img, h, w, (const uint4*)wts->w[MMMOT_W_VGG_WPX0],
-                                          wts->tc_scale[MMMOT_W_VGG_WP0], wts->w[MMMOT_W_VGG_B0], hb[which], plane_out,
-                                          status, st));
-        } else {
-          if (n_pix >= (1L << 31)) return MMMOT_E_SHAPE;
-          __half* cols = hb[which ^ 1];   // [2][pixels][32] taps, dead once the contraction has run
-          im2col27_kernel<<<mm_cdiv(n_pix, 256), 256, 0, st>>>(crops, n_pix, h, w, cols, n_pix * 32, status);
-          MM_LAUNCH_CHECK();
-          GemmP p = gemm_defaults();
-          p.bias = wts->w[MMMOT_W_VGG_B0]; p.M = cout; p.K = 32; p.relu = 1;
-          p.S = (int)n_pix; p.tiles_per_group = mm_cdiv(n_pix, tc::BN); p.num_tiles = p.tiles_per_group;
-          p.Y = reinterpret_cast<float*>(hb[which]); p.y_ms = cout;
-          MM_TRY(gemm_tma_launch_mat(p, (const uint4*)wts->w[MMMOT_W_VGG_WP0], wts->tc_scale[MMMOT_W_VGG_WP0], cols,
-                                     n_pix * 32, n_pix, 32, tma::OUT_PLANAR, plane_out, st, nullptr, status, nullptr,
-                                     (const uint4*)wts->w[MMMOT_W_VGG_WPX0]));
-        }
+        // im2col taps (if that variant runs) in the other activation buffer, dead once the contraction has run
+        MM_TRY(vgg_conv0_launch(crops, n_img, h, w, wts->w[MMMOT_W_VGG_WT0], wts->w[MMMOT_W_VGG_B0],
+                                (const uint4*)wts->w[MMMOT_W_VGG_WP0], wts->tc_scale[MMMOT_W_VGG_WP0],
+                                (const uint4*)wts->w[MMMOT_W_VGG_WPX0], hb[which], plane_out, hb[which ^ 1], status,
+                                nullptr, st));
       } else {
         GemmP p = gemm_defaults();
         p.bias = wts->w[MMMOT_W_VGG_B0 + i];

@@ -695,63 +695,90 @@ static int gemm_tma_launch_mat(const GemmP& g, const uint4* Wp, float out_scale,
   return 0;
 }
 
+// Waste of a box: padded / real pixels of the tile grid it induces.
+static inline double conv_box_waste(int n_img, int H, int W, int bx, int by, int bi) {
+  return (double)mm_cdiv(W, bx) * bx / W * mm_cdiv(H, by) * by / H * mm_cdiv(n_img, bi) * bi / n_img;
+}
+
+// Launch plan of a 3x3 convolution (gemm_tma_launch_conv).  Pure host logic, no CUDA call, so that tests can query
+// the decision the launcher takes (mmmot_debug_conv_plan) on a machine without a GPU.
+struct ConvPlan {
+  int px;                  // pixel-major kernel (gemm_tma_px.cuh) instead of the channel-major one
+  int halo;                // pixel-major: vertical taps from one (by + 2)-row halo box
+  int pool;                // 2x2 max-pool fused into the epilogue
+  int bx, by, bi;          // box of 256 pixels (powers of two)
+  int ksegs, kc_per_seg;   // K accumulated in ksegs passes of kc_per_seg 32-wide chunks
+  int tiles_x, tiles_y, num_tiles;   // column tiles (boxes); the channel-major kernel runs ceil(M/128) row tiles of each
+};
+// want_pool: the caller takes a fused pooled map; use_kseg: the caller provides K-segment scratch.
+// dbg / seg_chunks: mmmot_set_debug / mmmot_set_kseg state.
+static inline ConvPlan conv_plan(int M, bool part, int n_img, int H, int W, int C, bool want_pool, bool use_kseg, int dbg,
+                                 int seg_chunks) {
+  ConvPlan c;
+  memset(&c, 0, sizeof(c));
+  // box of 256 pixels = bx * by * bi (powers of two): the shape with the least padding waste, widest first
+  c.bx = 1; c.by = 1; c.bi = 256;
+  double best = 1e30;
+  for (int cx = 256; cx >= 1; cx >>= 1)
+    for (int cy = 256 / cx; cy >= 1; cy >>= 1) {
+      const int ci = 256 / (cx * cy);
+      const double waste = conv_box_waste(n_img, H, W, cx, cy, ci);
+      if (waste < best - 1e-9) { best = waste; c.bx = cx; c.by = cy; c.bi = ci; }
+    }
+  const int kchunks = 9 * C / tc::BK;
+  // 64-channel outputs run on the pixel-major kernel (gemm_tma_px.cuh); it prefers a 16 x 16 single-image box
+  // (vertical taps from one halo box, 2x2 pooling windows inside a warp) when that wastes no more than the best box
+  c.px = M == 64 && !part && !(dbg & 64) && !(use_kseg && seg_chunks > 0 && kchunks > seg_chunks);
+  if (c.px && conv_box_waste(1, H, W, 16, 16, 1) <= best + 1e-9) { c.bx = 16; c.by = 16; c.bi = 1; }
+  if (c.px) {
+    c.halo = (c.bi == 1 && c.bx >= 8 && c.bx * (c.by + 2) * 64 <= tma::PX_X_PLANE && !(dbg & 256)) ? 1 : 0;
+    c.pool = want_pool && c.bx >= 2 && c.bx <= 16 && c.by >= 2 && !(H & 1) && !(W & 1) && !(dbg & 512);
+  } else {
+    // channel-major kernel: the 2x2 max-pool (and SkipPool's per-image sums) fused into the epilogue when every pooling
+    // window lies inside one thread's chunks: box rows of <= 32 pixels, an even number of box rows per 128-column half
+    c.pool = want_pool && c.bx >= 2 && c.bx <= 32 && c.by >= 2 && !(H & 1) && !(W & 1) && !(dbg & 512);
+  }
+  c.ksegs = 1; c.kc_per_seg = kchunks;
+  if (use_kseg && seg_chunks > 0 && kchunks > seg_chunks) {
+    c.ksegs = (kchunks + seg_chunks - 1) / seg_chunks;
+    c.kc_per_seg = (kchunks + c.ksegs - 1) / c.ksegs;
+  }
+  c.tiles_x = mm_cdiv(W, c.bx); c.tiles_y = mm_cdiv(H, c.by);
+  c.num_tiles = c.tiles_x * c.tiles_y * mm_cdiv(n_img, c.bi);
+  return c;
+}
+
 // 3x3 / pad 1 convolution on planar FP16 NHWC activations; output planar FP16 NHWC (ReLU via g.relu).
 // acc_scratch (fp32 [tiles*256][M], tiles = ceil(W/bx)*ceil(H/by)*ceil(n/bi) <= padded pixel count) enables K-segmentation: chains longer than mmmot_set_kseg() chunks of 32 are
 // accumulated in several passes and summed in fp32 RN, which bounds the tensor core's round-toward-zero
 // accumulation error (DESIGN.md §4.2).  nullptr = single pass.
+// pool_sum is filled only by the channel-major kernel's fused pool; plan (optional) receives the plan taken.
 static int gemm_tma_launch_conv(const GemmP& g0, const uint4* Wp, float out_scale, const __half* Xhi, long x_plane,
                                 int n_img, int H, int W, int C, __half* Yhi, long y_plane, cudaStream_t st,
                                 float* acc_scratch = nullptr, long y_plane_pooled = 0, int* did_pool = nullptr,
-                                int* status = nullptr, unsigned long long* pool_sum = nullptr, const uint4* Wpx = nullptr) {
+                                int* status = nullptr, unsigned long long* pool_sum = nullptr, const uint4* Wpx = nullptr,
+                                ConvPlan* plan = nullptr) {
   if (did_pool) *did_pool = 0;
   if (!Wp || C % tc::BK) return MMMOT_E_ARG;
+  const ConvPlan c = conv_plan(g0.M, g0.part != nullptr, n_img, H, W, C, y_plane_pooled > 0 && did_pool,
+                               acc_scratch != nullptr, mm_debug_flags(), mm_kseg_chunks());
+  if (plan) *plan = c;
   int sms = 0;
   MM_TRY(mm_sm_count(&sms));
   static std::atomic<unsigned long long> attr{0};
   MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel, tma::T_SMEM_BYTES, attr));
-  // box of 256 pixels = bx * by * bi (powers of two): the shape with the least padding waste, widest first
-  int bx = 1, by = 1, bi = 256;
-  {
-    double best = 1e30;
-    for (int cx = 256; cx >= 1; cx >>= 1)
-      for (int cy = 256 / cx; cy >= 1; cy >>= 1) {
-        const int ci = 256 / (cx * cy);
-        const double waste = (double)mm_cdiv(W, cx) * cx / W * mm_cdiv(H, cy) * cy / H * mm_cdiv(n_img, ci) * ci / n_img;
-        if (waste < best - 1e-9) { best = waste; bx = cx; by = cy; bi = ci; }
-      }
-  }
-  // 64-channel outputs run on the pixel-major kernel (gemm_tma_px.cuh); it prefers a 16 x 16 single-image box
-  // (vertical taps from one halo box, 2x2 pooling windows inside a warp) when that wastes no more than the best box
-  const int seg_chunks = mm_kseg_chunks();   // 0 = single pass
-  const int dbg = mm_debug_flags();
-  const bool px = g0.M == 64 && !g0.part && !(dbg & 64) && !(acc_scratch && seg_chunks > 0 && 9 * C / tc::BK > seg_chunks);
-  if (px) {
-    const double best = (double)mm_cdiv(W, bx) * bx / W * mm_cdiv(H, by) * by / H * mm_cdiv(n_img, bi) * bi / n_img;
-    const double w16 = (double)mm_cdiv(W, 16) * 16 / W * mm_cdiv(H, 16) * 16 / H;
-    if (w16 <= best + 1e-9) { bx = 16; by = 16; bi = 1; }
-  }
   tma::TmaP P;
   memset(&P, 0, sizeof(P));
   GemmP g = g0;
   g.K = 9 * C;
-  P.conv = 1; P.bx = bx; P.by = by; P.bi = bi;
-  if (px) {
-    P.halo = (bi == 1 && bx >= 8 && bx * (by + 2) * 64 <= tma::PX_X_PLANE && !(dbg & 256)) ? 1 : 0;
-    if (y_plane_pooled > 0 && did_pool && bx >= 2 && bx <= 16 && by >= 2 && !(H & 1) && !(W & 1) && !(dbg & 512)) {
-      P.pool = 1;
-      *did_pool = 1;
-    }
-  }
-  // channel-major kernel: the 2x2 max-pool (and SkipPool's per-image sums) fused into the epilogue when every pooling
-  // window lies inside one thread's chunks: box rows of <= 32 pixels, an even number of box rows per 128-column half
-  if (!px && y_plane_pooled > 0 && did_pool && bx >= 2 && bx <= 32 && by >= 2 && !(H & 1) && !(W & 1) && !(dbg & 512)) {
-    P.pool = 1;
-    P.pool_sum = pool_sum;
-    *did_pool = 1;
-  }
-  P.tiles_x = mm_cdiv(W, bx); P.tiles_y = mm_cdiv(H, by);
+  P.conv = 1; P.bx = c.bx; P.by = c.by; P.bi = c.bi;
+  P.halo = c.halo;
+  P.pool = c.pool;
+  if (c.pool) *did_pool = 1;
+  if (c.pool && !c.px) P.pool_sum = pool_sum;
+  P.tiles_x = c.tiles_x; P.tiles_y = c.tiles_y;
   P.n_img = n_img; P.H = H; P.W = W; P.C = C;
-  g.num_tiles = P.tiles_x * P.tiles_y * mm_cdiv(n_img, bi);
+  g.num_tiles = c.num_tiles;
   g.tile_tab = nullptr;
   g.Y = reinterpret_cast<float*>(Yhi);
   g.y_ms = g.M;
@@ -764,17 +791,13 @@ static int gemm_tma_launch_conv(const GemmP& g0, const uint4* Wp, float out_scal
   P.t.dbg = mm_debug_flags();
   P.plane_elems = P.pool ? y_plane_pooled : y_plane;
   P.status = status;
-  P.ksegs = 1; P.kc_per_seg = P.t.k_chunks;
-  if (acc_scratch && seg_chunks > 0 && P.t.k_chunks > seg_chunks) {
-    P.ksegs = (P.t.k_chunks + seg_chunks - 1) / seg_chunks;
-    P.kc_per_seg = (P.t.k_chunks + P.ksegs - 1) / P.ksegs;
-    P.acc_scratch = acc_scratch;
-  }
+  P.ksegs = c.ksegs; P.kc_per_seg = c.kc_per_seg;
+  if (c.ksegs > 1) P.acc_scratch = acc_scratch;
   alignas(64) CUtensorMap mh, ml;
-  const int box_y = P.halo ? by + 2 : by;
-  MM_TRY(tma::make_map_4d(&mh, Xhi, n_img, H, W, C, bx, box_y, bi));
-  MM_TRY(tma::make_map_4d(&ml, Xhi + x_plane, n_img, H, W, C, bx, box_y, bi));
-  if (px) {
+  const int box_y = P.halo ? c.by + 2 : c.by;
+  MM_TRY(tma::make_map_4d(&mh, Xhi, n_img, H, W, C, c.bx, box_y, c.bi));
+  MM_TRY(tma::make_map_4d(&ml, Xhi + x_plane, n_img, H, W, C, c.bx, box_y, c.bi));
+  if (c.px) {
     if (Wpx) { P.t.Wp = Wpx; P.wcompact = 1; }
     return gemm_tma_px_launch(P, mh, ml, sms, st);
   }

@@ -68,8 +68,9 @@ def pack_tc(wt):
 def pack_px(packed_u8, M, K):
     """The compact N = 64 form of a pack_tc() result for the pixel-major kernel (64-output layers): rows 0..63 only,
     [k chunk][k group 4][hi rows | lo rows][row group 8][8 rows][8 k] fp16 = 8 KB per k chunk.  One bulk copy per chunk,
-    and per k group the 64 hi rows followed by the 64 lo rows form ONE 128-row K-major operand, so X_hi * W_hi and
-    X_hi * W_lo are a single N = 128 MMA (csrc/gemm_tma_px.cuh)."""
+    and per k group the 64 hi rows are followed by the 64 lo rows (one copy for both).  The pixel-major kernel
+    (csrc/gemm_tma_px.cuh) issues X_hi * W_hi and X_hi * W_lo as two m64n64 wgmmas whose B descriptors start at the
+    hi rows and 8 row groups later at the lo rows."""
     assert M == 64
     kc = (K + 31) // 32
     t = packed_u8.view(torch.int16).view(kc, 1, 2, 4, 16, 8, 8)          # kc, mt, hl, kg, mg, r, e
