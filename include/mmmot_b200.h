@@ -296,6 +296,9 @@ int mmmot_set_kseg(int chunks);
  *   bit 7 (128)  pixel-major epilogue with 16-byte stores instead of whole 32-byte sectors
  *   bit 8 (256)  pixel-major kernel without halo boxes (nine boxes per channel chunk)
  *   bit 9 (512)  no fused max-pool in the conv epilogues (separate max-pool kernel)
+ *   bit 10 (1024) generated-operand engine (csrc/gemm_gen.cuh): producers without the software pipeline, every GEN
+ *   bit 12 (4096) generated-operand engine: GEN_NORM producers with the software pipeline (prefetching variant)
+ *   bit 13 (8192) PointNet layers 3, 4 through norm_split + the TMA-fed kernel instead of GEN_NORM producers
  *   bit 14 (16384) first VGG layer with a separate im2col pre-pass instead of in-kernel operand producers */
 int mmmot_set_debug(int flags);
 
@@ -304,11 +307,41 @@ int mmmot_set_debug(int flags);
 int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scale, const float* bias, const float* X,
                        float* Y, int M, int K, int S, int engine, void* stream);
 
-/* Test hook of the generated-operand tensor-core engine (csrc/gemm_gen.cuh, GroupNorm+ReLU producer): with X [S][K] and
- * Y [S][M] fp32 channels-last, Y = relu(X*sc + sh) W^T + bias, sc/sh [K] per input channel (K a multiple of 32,
- * <= 512).  Wp = packed FP16 hi/lo tiles of W [M][K]. */
-int mmmot_debug_linear_gen(const void* Wp, float wp_scale, const float* bias, const float* X, const float* sc,
-                           const float* sh, float* Y, int M, int K, int S, void* stream);
+/* Test hooks of the generated-operand tensor-core engine (csrc/gemm_gen.cuh), run through the same launch code as the
+ * affinity, PointNet and fusion stages.  gen: 0-2 = pairwise multiply / |minus| / minus (MMMOT_AFF_*), 3 = GroupNorm +
+ * ReLU of an fp32 source (GEN_NORM), 4 = an fp32 source as it is (GEN_COPY).
+ * gen_prefetch: 1 if the launch takes the software-pipelined (prefetching) producers, else 0, under the current
+ *   mmmot_set_debug state; computed on the host without any CUDA call.  m: detections of a pairwise launch.
+ * gen: Y[row][y_ms] (fp32 channels-last, first M channels written, or NULL) = op(x) W^T + bias (+ ReLU if relu), Wp =
+ *   packed FP16 hi/lo tiles of W [M][K] (weights.py::pack_tc).  Columns (operand rows):
+ *     uniform tiling (tile_tab NULL): `groups` groups of S columns, 256-column tiles; column s of group g reads source
+ *       row g*x_gs + s (pairwise: s = i*m + j of the group's feature stack) and writes row g*y_gs + s;
+ *     tile table (GEN_NORM / GEN_COPY only; x_gs, y_gs ignored): tile_tab int4 [num_tiles] {group, first absolute row,
+ *       length <= 256, 0}.
+ *   Source: pairwise src = feature stacks fcl [groups][Lf][K] with rows [0, n) objects, [n, n + m) detections, Lf = n + m;
+ *   GEN_NORM / GEN_COPY src = fp32 rows of ld_src floats (multiple of 8, >= K; the first K are read), GEN_NORM
+ *   x = relu(src*gsc[g][k] + gsh[g][k]) with gsc/gsh [groups][K], K <= 512.  part (or NULL): double2
+ *   [num_tiles*2][M] = (sum, sum of squares) of each tile's column half (tile*2 + half).  prefetched (host, or NULL):
+ *   the variant taken, as gen_prefetch. */
+int mmmot_debug_gen_prefetch(int gen, int m);
+int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_scale, const float* bias, int relu, const float* src,
+                    int ld_src, const float* gsc, const float* gsh, int n, int m, int Lf, int S, int groups, long x_gs,
+                    long y_gs, const void* tile_tab, int num_tiles, float* Y, long y_ms, void* part, int* prefetched,
+                    void* stream);
+
+/* Test hook of PointNet's tensor-core trunk over ragged detections (csrc/pointnet.cu).  From the CSR offsets det_split
+ * [pairs*L + 1] (device; h_det_split the same on the host) it builds, as mmmot_pointnet_fwd does: tiles int4 [n_tiles]
+ * {pair, first point, length <= 256, 0}, cnt [pairs] points per pair, gstart [pairs + 1] first tile of each pair, seg
+ * [P] detection of each point, ctab int4 [2*n_tiles] chunk descriptors ((first detection << 1) | chunk complete and
+ * inside one detection, per 32-column chunk of each tile half).  *n_tiles (host, or NULL) = tile count;
+ * MMMOT_E_WORKSPACE if it exceeds max_tiles.  If Wp is not NULL it then runs one matrix-mode contraction on those tables
+ * as the trunk issues it: X = FP16 planes [2][P][K] (Xhi), Y [P][M] fp32 (or NULL), part [n_tiles*2][M] double2 (or
+ * NULL), addend [det][ld_add] per-detection addend (or NULL), segsum (or NULL): [det][M] sums over each detection's
+ * points of relu(y*sc[pair][co] + sh[pair][co]) in 2^-32 fixed point, accumulated (the caller zeroes it). */
+int mmmot_debug_pn_contraction(const int* det_split, const int* h_det_split, int pairs, int L, long max_tiles, void* tiles,
+                               int* cnt, int* gstart, int* seg, void* ctab, long* n_tiles, const void* Wp, float wp_scale,
+                               const float* bias, int M, int K, const void* Xhi, float* Y, void* part, const float* addend,
+                               int ld_add, unsigned long long* segsum, const float* sc, const float* sh, void* stream);
 
 /* Test hooks of the TMA-fed tensor-core engine: operands are two FP16 planes (hi, lo), channels-last.
  * linear: Y[rows][M] fp32 = X W^T + bias, X planes [2][rows][K].  conv: 3x3 pad 1 + bias + ReLU on NHWC planes

@@ -194,17 +194,41 @@ extern "C" int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scal
   return gemm_simt_launch<XM_DIRECT>(p, st);
 }
 
-// Generated-operand tensor-core engine (gemm_gen.cuh, GEN_NORM): Y[S][M] = relu(X[S][K]*sc + sh) W^T + bias with X, Y
-// fp32 channels-last, sc/sh [K].
-extern "C" int mmmot_debug_linear_gen(const void* Wp, float wp_scale, const float* bias, const float* X, const float* sc,
-                                      const float* sh, float* Y, int M, int K, int S, void* stream) {
-  if (!Wp || !X || !Y || !sc || !sh || M <= 0 || K <= 0 || S <= 0) return MMMOT_E_ARG;
+// The producer variant gemm_gen_launch takes (1 = prefetching), computed on the host without any CUDA call.
+extern "C" int mmmot_debug_gen_prefetch(int gen, int m) {
+  if (gen < gen::GEN_PAIR_MUL || gen > gen::GEN_COPY) return MMMOT_E_ARG;
+  return gen_prefetch(gen, m, mm_debug_flags()) ? 1 : 0;
+}
+
+// One contraction of the generated-operand tensor-core engine (gemm_gen.cuh) through gemm_gen_launch, with the
+// arguments the affinity, PointNet and fusion stages pass it.
+extern "C" int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_scale, const float* bias, int relu,
+                               const float* src, int ld_src, const float* gsc, const float* gsh, int n, int m, int Lf, int S,
+                               int groups, long x_gs, long y_gs, const void* tile_tab, int num_tiles, float* Y, long y_ms,
+                               void* part, int* prefetched, void* stream) {
+  if (M <= 0 || K <= 0) return MMMOT_E_ARG;
   GemmP p = gemm_defaults();
-  p.bias = bias; p.M = M; p.K = K;
-  p.S = S; p.tiles_per_group = mm_cdiv(S, tc::BN); p.num_tiles = p.tiles_per_group;
-  p.x_gs = S;
-  p.Y = Y; p.y_gs = S; p.y_ms = M;
-  return gemm_gen_launch<gen::GEN_NORM>(p, (const uint4*)Wp, wp_scale, X, K, sc, sh, 0, 0, 0, (cudaStream_t)stream);
+  p.bias = bias; p.M = M; p.K = K; p.relu = relu;
+  if (tile_tab) {
+    if (num_tiles <= 0) return MMMOT_E_ARG;
+    p.tile_tab = (const int4*)tile_tab; p.num_tiles = num_tiles;
+  } else {
+    if (S <= 0 || groups <= 0) return MMMOT_E_ARG;
+    p.S = S; p.tiles_per_group = mm_cdiv(S, tc::BN); p.num_tiles = p.tiles_per_group * groups;
+    p.x_gs = x_gs; p.y_gs = y_gs;
+  }
+  p.Y = Y; p.y_ms = y_ms;
+  p.part = (double2*)part;
+  const uint4* w = (const uint4*)Wp;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (gen) {
+    case gen::GEN_PAIR_MUL: return gemm_gen_launch<gen::GEN_PAIR_MUL>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_PAIR_ABS: return gemm_gen_launch<gen::GEN_PAIR_ABS>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_PAIR_SUB: return gemm_gen_launch<gen::GEN_PAIR_SUB>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_NORM: return gemm_gen_launch<gen::GEN_NORM>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_COPY: return gemm_gen_launch<gen::GEN_COPY>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
+    default: return MMMOT_E_ARG;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -342,7 +342,7 @@ static __global__ void __launch_bounds__(G_THREADS, 1) gemm_gen_kernel(const Gen
 }  // namespace gen
 
 // Host launcher.  g: M, K (multiple of 32, <= 512 for GEN_NORM), bias, S / tiles_per_group / num_tiles (uniform column
-// tiling, 256 columns per tile) or tile_tab (GEN_NORM: ragged groups, absolute rows), x_gs (NORM: source rows per group), Y / y_gs / y_ms = fp32 channels-last output (or
+// tiling, 256 columns per tile) or tile_tab (GEN_NORM, GEN_COPY: ragged groups, absolute rows), x_gs (NORM: source rows per group), Y / y_gs / y_ms = fp32 channels-last output (or
 // null), part = two GroupNorm partials per tile (stats_reduce(..., mult = 2)).  Wp = weights packed by
 // weights.py::pack_tc.  PAIR: src = fcl [G][Lf][K]; NORM: src = [G*x_gs][ld_src] fp32, gsc/gsh [G][K].
 template <int GEN, bool PAIRED>
@@ -374,11 +374,24 @@ static int gemm_gen_launch_t(const GemmP& g, const uint4* Wp, float out_scale, c
   return 0;
 }
 
+// Producer variant gemm_gen_launch takes: the software-pipelined (prefetching, PAIRED) producers or the plain ones.
+// Pure host logic, no CUDA call, so that tests can query it without a GPU (mmmot_debug_gen_prefetch).
+// dbg: mmmot_set_debug state; bit 10 (1024) producers without the software pipeline (A/B runs), bit 12 (4096) GEN_NORM
+// with it.  GEN_PAIR_* pipeline only at m == 128 (two whole rows per tile, see gemm_gen_kernel).
+static inline bool gen_prefetch(int GEN, int m, int dbg) {
+  if (dbg & 1024) return false;
+  if (GEN == gen::GEN_NORM) return (dbg & 4096) != 0;
+  if (GEN == gen::GEN_COPY) return true;
+  return m == 128;
+}
+
+// prefetched (host, or NULL) receives the variant taken (gen_prefetch)
 template <int GEN>
 static int gemm_gen_launch(const GemmP& g, const uint4* Wp, float out_scale, const float* src, int ld_src,
-                           const float* gsc, const float* gsh, int n, int m, int Lf, cudaStream_t st) {
-  // debug bit 10 (1024): producers without the software pipeline (A/B runs)
-  const bool pipe = !(mm_debug_flags() & 1024) && (GEN == gen::GEN_NORM ? (mm_debug_flags() & 4096) != 0 : GEN == gen::GEN_COPY ? true : m == 128);
+                           const float* gsc, const float* gsh, int n, int m, int Lf, cudaStream_t st,
+                           int* prefetched = nullptr) {
+  const bool pipe = gen_prefetch(GEN, m, mm_debug_flags());
+  if (prefetched) *prefetched = pipe ? 1 : 0;
   if (pipe) return gemm_gen_launch_t<GEN, true>(g, Wp, out_scale, src, ld_src, gsc, gsh, n, m, Lf, st);
   return gemm_gen_launch_t<GEN, false>(g, Wp, out_scale, src, ld_src, gsc, gsh, n, m, Lf, st);
 }

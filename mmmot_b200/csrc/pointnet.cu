@@ -225,6 +225,31 @@ PnWs carve(MmArena& a, int pairs, int L, long P, long max_tiles, bool use_tc) {
   return w;
 }
 
+// Column tiles of at most tw points over each pair's point range (tiles never straddle two pairs: one pair = one
+// GroupNorm domain).  The host needs only this count for its launch geometry.
+long pn_tile_count(const int* h_det_split, int pairs, int L, int tw) {
+  long n = 0;
+  for (int p = 0; p < pairs; p++) n += mm_cdiv((long)h_det_split[(p + 1) * L] - h_det_split[p * L], tw);
+  return n;
+}
+
+// The tables of the ragged per-pair point ranges, built on the device from the CSR offsets det_split [pairs*L + 1]:
+// tiles [n_tiles] {pair, first point, length <= tw, 0}, cnt [pairs] points per pair, gstart [pairs + 1] first tile of
+// each pair, seg [P] detection of each point and, if ctab is set, the chunk descriptors of the tensor-core epilogue
+// (tma::seg_chunk_tab_kernel, [2*n_tiles]).
+int pn_tables(const int* det_split, int pairs, int L, long P, int tw, long n_tiles, int* cnt, int* gstart, int4* tiles,
+              int* seg, int4* ctab, cudaStream_t st) {
+  pn_tiles_kernel<<<1, 256, 0, st>>>(det_split, pairs, L, tw, cnt, gstart, tiles);
+  MM_LAUNCH_CHECK();
+  point_segment_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(det_split, pairs * L, P, seg);
+  MM_LAUNCH_CHECK();
+  if (ctab) {
+    tma::seg_chunk_tab_kernel<<<mm_cdiv(n_tiles * 2, 128), 128, 0, st>>>(tiles, (int)n_tiles, seg, ctab);
+    MM_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
 }  // namespace
 
 // engine choice from the per-pair shape only (see appearance.cu)
@@ -275,23 +300,14 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
   // column tiles never straddle two frame-pairs (one pair = one GroupNorm domain)
   const bool use_tc = !train && pointnet_use_tc(L);
   const int TNW = use_tc ? tc::BN : 128;
-  long n_tiles = 0;   // the host needs only the COUNT (launch geometry); the table itself is built on the device
-  for (int p = 0; p < pairs; p++) n_tiles += mm_cdiv((long)h_det_split[(p + 1) * L] - h_det_split[p * L], TNW);
+  const long n_tiles = pn_tile_count(h_det_split, pairs, L, TNW);
   const long max_tiles = P / 128 + 2 * pairs + 2;   // also bounds 2 partials per 256-wide tile
   MmArena ar(workspace, workspace_bytes);
   PnWs w = carve(ar, pairs, L, P, max_tiles, use_tc);
   if (!ar.ok() || n_tiles > max_tiles) return MMMOT_E_WORKSPACE;
-  pn_tiles_kernel<<<1, 256, 0, st>>>(det_split, pairs, L, TNW, w.cnt, w.gstart, w.tiles);
-  MM_LAUNCH_CHECK();
-
   transpose_points_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(points, w.xt, P);
   MM_LAUNCH_CHECK();
-  point_segment_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(det_split, ndet, P, w.seg);
-  MM_LAUNCH_CHECK();
-  if (use_tc) {
-    tma::seg_chunk_tab_kernel<<<mm_cdiv(n_tiles * 2, 128), 128, 0, st>>>(w.tiles, (int)n_tiles, w.seg, w.ctab);
-    MM_LAUNCH_CHECK();
-  }
+  MM_TRY(pn_tables(det_split, pairs, L, P, TNW, n_tiles, w.cnt, w.gstart, w.tiles, w.seg, use_tc ? w.ctab : nullptr, st));
 
   const int cin[5] = {3, 64, 64, 64, 128}, cout[5] = {64, 64, 64, 128, 1024};
   const bool timed = mm_timing_on();
@@ -476,4 +492,37 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
     MM_LAUNCH_CHECK();
   }
   return 0;
+}
+
+// PointNet's tables over ragged per-pair point ranges (pn_tables, 256-point tiles as on the tensor-core path), then
+// optionally one matrix-mode contraction on them exactly as pointnet_impl issues it: FP16 planes X[2][P][K], tile
+// table, and per launch Y / part (statistics), addend (head) or segsum (second passes).
+extern "C" int mmmot_debug_pn_contraction(const int* det_split, const int* h_det_split, int pairs, int L, long max_tiles,
+                                          void* tiles, int* cnt, int* gstart, int* seg, void* ctab, long* n_tiles,
+                                          const void* Wp, float wp_scale, const float* bias, int M, int K, const void* Xhi,
+                                          float* Y, void* part, const float* addend, int ld_add,
+                                          unsigned long long* segsum, const float* sc, const float* sh, void* stream) {
+  if (!det_split || !h_det_split || pairs <= 0 || L <= 0 || !tiles || !cnt || !gstart || !seg || !ctab) return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ndet = pairs * L;
+  const long P = h_det_split[ndet];
+  if (h_det_split[0] != 0 || P <= 0) return MMMOT_E_SHAPE;
+  for (int d = 0; d < ndet; d++)
+    if (h_det_split[d + 1] <= h_det_split[d]) return MMMOT_E_SHAPE;
+  const long nt = pn_tile_count(h_det_split, pairs, L, tc::BN);
+  if (n_tiles) *n_tiles = nt;
+  if (nt > max_tiles) return MMMOT_E_WORKSPACE;
+  MM_TRY(pn_tables(det_split, pairs, L, P, tc::BN, nt, cnt, gstart, (int4*)tiles, seg, (int4*)ctab, st));
+  if (!Wp) return 0;
+  if (!Xhi) return MMMOT_E_ARG;
+  GemmP p = gemm_defaults();
+  p.bias = bias; p.M = M; p.K = K;
+  p.tile_tab = (const int4*)tiles; p.num_tiles = (int)nt;
+  p.Y = Y; p.y_ms = M;
+  p.part = (double2*)part;
+  p.addend = addend; p.ld_add = ld_add;
+  p.sc = sc; p.sh = sh;
+  if (addend || segsum) p.seg = seg;
+  return gemm_tma_launch_mat(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, P * K, P, K, tc::OUT_CL, 0, st, segsum, nullptr,
+                             (const int4*)ctab);
 }
