@@ -8,11 +8,11 @@
 //   * 3x3 convolution: 4-D map [img][H][W][C], box (32, bx, by, bi) with bx*by*bi = 256; the 9 taps are the
 //     same box at shifted (x, y) coordinates and the zero padding is TMA's out-of-bounds fill — no im2col,
 //     no boundary code, no index arithmetic on the SMs.
-// CTA (288 threads, persistent, one per SM): warps 0-7 are two consumer warpgroups (warpgroup h issues the wgmma
+// CTA (384 threads, persistent, one per SM): warps 0-7 are two consumer warpgroups (warpgroup h issues the wgmma
 // chains of the tile's 128 rows x column half h, then runs the epilogue of that half: warp q of it owns rows
-// 32q..32q+31), warp 8 is the loader (weights by cp.async.bulk, operand boxes by TMA).  The accumulator image of a
-// finished tile (128 x 256 fp32) overlays stages 0-1 of the ring, so the loader starts the next tile once the
-// epilogue has read it.  Conv outputs are transposed through a per-warp smem scratch so each lane stores 64
+// 32q..32q+31), warp 8 is the loader (weights by cp.async.bulk, operand boxes by TMA; warps 9-11 only complete its
+// warpgroup).  Ring of 4 x 48 KB stages; the accumulator image of a finished tile (128 x 256 fp32) overlays the
+// first 128 KB of it, so the loader starts the next tile once the epilogue has read it.  Conv outputs are transposed through a per-warp smem scratch so each lane stores 64
 // contiguous bytes (32 channels of one pixel) per plane.
 #pragma once
 #include <cuda.h>
@@ -29,7 +29,14 @@ constexpr int T_EPI_WARPS = 8, T_LOAD_WARP = 8;   // warps 9-11 only complete th
 constexpr int T_CONS_REGS = 232, T_LOAD_REGS = 40;
 static_assert(256 * T_CONS_REGS + 128 * T_LOAD_REGS <= launch_regs(T_THREADS) * T_THREADS, "register split exceeds the CTA's pool");
 constexpr int T_EPI_SCRATCH = 32 * 80;   // per epilogue warp: 32 pixels x (64 B of channels + 16 B pad)
-constexpr size_t T_SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 + 256 + T_EPI_WARPS * T_EPI_SCRATCH;
+// ring stage = one k chunk: the tile's weight block (hi | lo, 16 KB) and the operand box (hi, lo planes, 2 x 16 KB).
+// Four such stages fill the shared memory three 64 KB stages would (tc::STAGE_BYTES has room for a second weight
+// block this kernel never loads), so the loader runs one chunk further ahead of the MMAs.
+constexpr int T_STAGES = 4;
+constexpr int T_STAGE_BYTES = A_SUB + 2 * B_HALF;
+constexpr size_t T_SMEM_BYTES = (size_t)T_STAGES * T_STAGE_BYTES + 1024 + 256 + T_EPI_WARPS * T_EPI_SCRATCH;
+static_assert(T_SMEM_BYTES <= 227 * 1024, "gemm_tma_kernel exceeds the 227 KB of shared memory per block");
+static_assert(T_STAGES * T_STAGE_BYTES >= 128 * BN * 4, "the accumulator image must fit in the ring it overlays");
 
 enum { OUT_PLANAR = 3 };   // two FP16 planes Y_hi[row][y_ms], Y_lo = Y_hi + plane_elems (channels-last)
 
@@ -137,12 +144,12 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t bar0 = base + STAGES * STAGE_BYTES;
+  const uint32_t bar0 = base + T_STAGES * T_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
-  const uint32_t free_bar = bar0 + 8u * (2 * STAGES);   // the epilogue has read the accumulator image
-  float* img = reinterpret_cast<float*>(sm);              // accumulator image [128][BN] fp32 over stages 0-1
-  uint8_t* epi_scratch = sm + STAGES * STAGE_BYTES + 256;
+  auto empty_bar = [&](int s) { return bar0 + 8u * (T_STAGES + s); };
+  const uint32_t free_bar = bar0 + 8u * (2 * T_STAGES);   // the epilogue has read the accumulator image
+  float* img = reinterpret_cast<float*>(sm);              // accumulator image [128][BN] fp32 over the ring's first 128 KB
+  uint8_t* epi_scratch = sm + T_STAGES * T_STAGE_BYTES + 256;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mgroups = P.t.m_tiles;
@@ -152,7 +159,7 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
   const int cchunks = P.conv ? P.C / BK : KC;
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; s++) {
+    for (int s = 0; s < T_STAGES; s++) {
       mbar_init(full_bar(s), 1);              // the loader's single expect_tx arrive (weights + 2 operand boxes)
       mbar_init(empty_bar(s), T_EPI_WARPS);   // one arrive per consumer warp once its wgmmas have read the stage
     }
@@ -181,11 +188,7 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
     uint32_t wcount = 0;   // (tile, segment) work items processed by this CTA
     uint32_t it = 0;       // k chunks consumed (ring position)
     float acc[2][64];      // rows 64 mb + fragment row, columns 128 half + fragment column
-#pragma unroll
-    for (int mb = 0; mb < 2; mb++)
-#pragma unroll
-      for (int i = 0; i < 64; i++) acc[mb][i] = 0.f;
-    float amax = 0.f;      // largest magnitude converted to FP16 by this thread (range guard)
+    float amax = 0.f;     // largest magnitude converted to FP16 by this thread (range guard)
     __half* yh = reinterpret_cast<__half*>(p.Y);
     __half* scr = reinterpret_cast<__half*>(epi_scratch + warp * T_EPI_SCRATCH);
     // final conv values x[j] (pixel column col0+j, channel cb+lane) -> FP16 hi/lo NHWC planes.  The 32x32 block is
@@ -293,11 +296,17 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
       if (P.conv) conv_origin(nt, i0, y0, x0); else tile_cols(nt, g, c0, len);
       for (int seg = 0; seg < P.ksegs; seg++, wcount++) {
       // ---- main loop: this warpgroup's 128 rows x 128 columns (column half `half`), two m64n128 wgmma chains ----
+      // The first wgmma of each chain ignores the accumulators (scale_d = 0); clearing them here rather than once per
+      // CTA leaves them dead from the image dump to the next item, so the epilogue has their registers (no spills).
+#pragma unroll
+      for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+        for (int i = 0; i < 64; i++) acc[mb][i] = 0.f;
       const int kc_lo = seg * P.kc_per_seg, kc_hi = min(KC, kc_lo + P.kc_per_seg);
       for (int kc = kc_lo; kc < kc_hi; kc++, it++) {
-        const int s = it % STAGES;
-        mbar_wait(full_bar(s), (it / STAGES) & 1);
-        const uint32_t sa = base + s * STAGE_BYTES, sb = sa + 2 * A_SUB + half * (128 / 8) * 512;
+        const int s = it % T_STAGES;
+        mbar_wait(full_bar(s), (it / T_STAGES) & 1);
+        const uint32_t sa = base + s * T_STAGE_BYTES, sb = sa + A_SUB + half * (128 / 8) * 512;
         if (!(P.t.dbg & 8)) {
           wgmma_fence();
 #pragma unroll
@@ -315,14 +324,14 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
           wgmma_commit();
         }
         wgmma_wait<1>();   // the previous chunk's wgmmas are done: release its stage
-        if (kc > kc_lo) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar((it - 1) % STAGES)); }
+        if (kc > kc_lo) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar((it - 1) % T_STAGES)); }
       }
       wgmma_wait<0>();
       fence_acc(acc[0]);
       fence_acc(acc[1]);
       __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar((it - 1) % STAGES));
-      bar_sync(7, T_EPI_WARPS * 32);   // both warpgroups are past their wgmmas: stages 0-1 may be overwritten
+      if (lane == 0) mbar_arrive(empty_bar((it - 1) % T_STAGES));
+      bar_sync(7, T_EPI_WARPS * 32);   // both warpgroups are past their wgmmas: the image may overwrite the ring
       acc_dump(acc[0], img, BN, 0, half * 128);
       acc_dump(acc[1], img, BN, 64, half * 128);
       bar_sync(7, T_EPI_WARPS * 32);
@@ -534,12 +543,12 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
             if (wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);
             wcount++;
           }
-          const int s = it % STAGES;
-          mbar_wait(empty_bar(s), ((it / STAGES) & 1) ^ 1);
+          const int s = it % T_STAGES;
+          mbar_wait(empty_bar(s), ((it / T_STAGES) & 1) ^ 1);
           const uint32_t abytes = (uint32_t)A_SUB;
           const bool skipA = P.t.dbg & 2, skipB = P.t.dbg & 4;     // profiling experiments only
           mbar_expect_tx(full_bar(s), (skipA ? 0u : abytes) + (skipB ? 0u : 2u * B_HALF));
-          const uint32_t sa = base + s * STAGE_BYTES, sb = sa + 2 * A_SUB;
+          const uint32_t sa = base + s * T_STAGE_BYTES, sb = sa + A_SUB;
           const uint8_t* src = reinterpret_cast<const uint8_t*>(P.t.Wp) + ((size_t)kc * P.t.m_tiles + mt0) * A_SUB;
           if (!skipA) bulk_g2s(sa, src, abytes, full_bar(s));
           if (skipB) continue;
