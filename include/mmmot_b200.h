@@ -312,6 +312,8 @@ int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scale, const fl
  * ReLU of an fp32 source (GEN_NORM), 4 = an fp32 source as it is (GEN_COPY).
  * gen_prefetch: 1 if the launch takes the software-pipelined (prefetching) producers, else 0, under the current
  *   mmmot_set_debug state; computed on the host without any CUDA call.  m: detections of a pairwise launch.
+ * gen_staged: 1 if that variant stages the pairwise sources in shared memory by TMA (GEN_PAIR_* at m == 128 without
+ *   bit 10), else 0; computed on the host like gen_prefetch.
  * gen: Y[row][y_ms] (fp32 channels-last, first M channels written, or NULL) = op(x) W^T + bias (+ ReLU if relu), Wp =
  *   packed FP16 hi/lo tiles of W [M][K] (weights.py::pack_tc).  Columns (operand rows):
  *     uniform tiling (tile_tab NULL): `groups` groups of S columns, 256-column tiles; column s of group g reads source
@@ -324,6 +326,7 @@ int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scale, const fl
  *   [num_tiles*2][M] = (sum, sum of squares) of each tile's column half (tile*2 + half).  prefetched (host, or NULL):
  *   the variant taken, as gen_prefetch. */
 int mmmot_debug_gen_prefetch(int gen, int m);
+int mmmot_debug_gen_staged(int gen, int m);
 int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_scale, const float* bias, int relu, const float* src,
                     int ld_src, const float* gsc, const float* gsh, int n, int m, int Lf, int S, int groups, long x_gs,
                     long y_gs, const void* tile_tab, int num_tiles, float* Y, long y_ms, void* part, int* prefetched,

@@ -200,6 +200,12 @@ extern "C" int mmmot_debug_gen_prefetch(int gen, int m) {
   return gen_prefetch(gen, m, mm_debug_flags()) ? 1 : 0;
 }
 
+// Whether that variant stages the pairwise sources in shared memory by TMA (1) or not, on the host, no CUDA call.
+extern "C" int mmmot_debug_gen_staged(int gen, int m) {
+  if (gen < gen::GEN_PAIR_MUL || gen > gen::GEN_COPY) return MMMOT_E_ARG;
+  return gen_staged(gen, m, mm_debug_flags()) ? 1 : 0;
+}
+
 // One contraction of the generated-operand tensor-core engine (gemm_gen.cuh) through gemm_gen_launch, with the
 // arguments the affinity, PointNet and fusion stages pass it.
 extern "C" int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_scale, const float* bias, int relu,

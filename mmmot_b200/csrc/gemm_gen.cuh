@@ -16,8 +16,9 @@
 //
 // CTA (512 threads, persistent, one per SM): warps 0-7 are two consumer warpgroups (warpgroup h issues the wgmma chains
 // of the tile's 128 rows x column half h and runs that half's epilogue), warps 8-15 operand producers; the first
-// producer thread also fetches each chunk's pre-tiled FP16 hi/lo weight block (cp.async.bulk).  One mbarrier per
-// stage collects that expect_tx and the eight producer warps' arrivals.  The consumers hold 128 accumulator registers
+// producer thread also fetches each chunk's pre-tiled FP16 hi/lo weight block (cp.async.bulk) and, for the pairwise
+// producers at m == 128, the chunk's fp32 sources (TMA, see gemm_gen_kernel).  One mbarrier per stage collects the
+// weight expect_tx and the eight producer warps' arrivals.  The consumers hold 128 accumulator registers
 // each and take registers from the producers (setmaxnreg).  The accumulator image of a finished tile overlays
 // stages 0-1 of the ring, so the producers start the next tile once the epilogue has read it.
 #pragma once
@@ -33,8 +34,15 @@ constexpr int G_EPI_WARPS = 8, G_PROD_WARP0 = 8, G_PROD_WARPS = 8;
 constexpr int G_THREADS = (G_PROD_WARP0 + G_PROD_WARPS) * 32;   // 512
 constexpr int G_CONS_REGS = 176, G_PROD_REGS = 80;
 static_assert(256 * G_CONS_REGS + 256 * G_PROD_REGS <= launch_regs(G_THREADS) * G_THREADS, "register split exceeds the CTA's pool");
-constexpr size_t G_SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 + 256;
+// Staged pairwise sources (PAIRED GEN_PAIR_*): per stage, the chunk's [128 detections x 32 channels] fp32 box in the
+// stage's otherwise unused 16 KB slot at A_SUB (128-byte swizzle), and the two object rows [2 x 32] fp32 beside the
+// barriers (G_OBJ_BYTES per stage).
+constexpr int G_DET_BYTES = 128 * BK * 4, G_OBJ_BYTES = 2 * BK * 4;
+static_assert(G_DET_BYTES == A_SUB && A_SUB % 1024 == 0, "the detection box fills the stage's free 1024-aligned slot");
+constexpr int G_SRC_AHEAD = STAGES - 1;   // chunks whose sources are in flight while the producers convert one
+constexpr size_t G_SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 + 256 + STAGES * G_OBJ_BYTES;
 constexpr int G_MAX_K = 512;   // producer-side GroupNorm affine staged in shared memory
+__host__ __device__ constexpr bool staged(int GEN, bool PAIRED) { return PAIRED && GEN <= GEN_PAIR_SUB; }
 
 struct GenP {
   TcP t;               // .g: M, K, bias, S (columns per group), tiles_per_group, num_tiles, Y / y_gs / y_ms (fp32
@@ -58,12 +66,15 @@ __device__ __forceinline__ void ld_global_256(const float* p, float (&v)[8]) {
                : "l"(p));
 }
 
-// PAIRED: software-pipelined producers (the next chunk's source vectors are loaded before the current chunk is
-// converted).  GEN_PAIR_*: only for m == 128, where a 256-column tile is two whole rows i and the thread's four items are
-// {row i0, row i0 + 1} x {j = cb, j = cb + 64}: 2 + 2 source vectors instead of 4 + 4, which leaves the registers.
-// GEN_NORM: any shape; the GroupNorm affine is then re-read from shared memory per pair of items.
+// PAIRED: pipelined producers.  GEN_PAIR_*: only for m == 128, where a 256-column tile is two whole object rows i0,
+// i0 + 1 against all 128 detections and the thread's four items are {row i0, row i0 + 1} x {j = cb, j = cb + 64}.  The
+// chunk's sources (the detection box and the two object rows, map_det / map_obj) are staged in shared memory by TMA,
+// G_SRC_AHEAD chunks ahead of the conversion; the producers hold no prefetch in registers.
+// GEN_NORM, GEN_COPY: the next chunk's source vectors are loaded into registers before the current chunk is converted
+// (any shape; GEN_NORM then re-reads the GroupNorm affine from shared memory per pair of items).
 template <int GEN, bool PAIRED>
-static __global__ void __launch_bounds__(G_THREADS, 1) gemm_gen_kernel(const GenP P) {
+static __global__ void __launch_bounds__(G_THREADS, 1)
+gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const __grid_constant__ CUtensorMap map_obj) {
   const GemmP& p = P.t.g;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(16) float s_gsc[GEN == GEN_NORM ? G_MAX_K : 4], s_gsh[GEN == GEN_NORM ? G_MAX_K : 4];
@@ -74,6 +85,11 @@ static __global__ void __launch_bounds__(G_THREADS, 1) gemm_gen_kernel(const Gen
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
   const uint32_t free_bar = bar0 + 8u * (2 * STAGES);   // the epilogue has read the accumulator image
+  // staged sources: src_full(s) collects the TMA bytes of stage s's sources, src_empty(s) one arrive per producer warp
+  // once it has converted them
+  auto src_full = [&](int s) { return bar0 + 8u * (2 * STAGES + 1 + s); };
+  auto src_empty = [&](int s) { return bar0 + 8u * (3 * STAGES + 1 + s); };
+  const uint32_t obj0 = bar0 + 256;                       // object rows, G_OBJ_BYTES per stage
   float* img = reinterpret_cast<float*>(sm);              // accumulator image [128][BN] fp32 over stages 0-1
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -85,6 +101,10 @@ static __global__ void __launch_bounds__(G_THREADS, 1) gemm_gen_kernel(const Gen
     for (int s = 0; s < STAGES; s++) {
       mbar_init(full_bar(s), 1 + G_PROD_WARPS);   // weight expect_tx arrive + one arrive per producer warp
       mbar_init(empty_bar(s), G_EPI_WARPS);       // one arrive per consumer warp once its wgmmas have read the stage
+      if (staged(GEN, PAIRED)) {
+        mbar_init(src_full(s), 1);
+        mbar_init(src_empty(s), G_PROD_WARPS);
+      }
     }
     mbar_init(free_bar, G_EPI_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -106,15 +126,22 @@ static __global__ void __launch_bounds__(G_THREADS, 1) gemm_gen_kernel(const Gen
     const int q = warp & 3, half = warp >> 2;
     uint32_t it = 0;
     float acc[2][64];      // rows 64 mb + fragment row, columns 128 half + fragment column
+    auto clear_acc = [&]() {
 #pragma unroll
-    for (int mb = 0; mb < 2; mb++)
+      for (int mb = 0; mb < 2; mb++)
 #pragma unroll
-      for (int i = 0; i < 64; i++) acc[mb][i] = 0.f;
+        for (int i = 0; i < 64; i++) acc[mb][i] = 0.f;
+    };
+    if (!staged(GEN, PAIRED)) clear_acc();
     for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       const int mg = (int)(t % mgroups);
       const int nt = (int)(t / mgroups);
       int g, c0, len;
       tile_cols(nt, g, c0, len);
+      // The first wgmma of each chain ignores the accumulators (scale_d = 0).  Staged pairwise variant: clearing them
+      // here rather than once per CTA leaves them dead from the image dump to the next tile, so the epilogue has their
+      // registers (no spills).
+      if (staged(GEN, PAIRED)) clear_acc();
       for (int kc = 0; kc < KC; kc++, it++) {
         const int s = it % STAGES;
         mbar_wait(full_bar(s), (it / STAGES) & 1);
@@ -202,10 +229,12 @@ static __global__ void __launch_bounds__(G_THREADS, 1) gemm_gen_kernel(const Gen
     // and written as one 16-byte piece per plane of the canonical K-major layout:
     //   byte offset = kg * B_LBO + (column / 8) * 128 + (column % 8) * 16
     // (a quarter warp = one kg, eight consecutive columns -> 128 contiguous bytes: conflict-free).
-    // The 256-bit source loads of chunk c+1 are issued before chunk c is converted (two register sets, ping-pong), so
-    // the L2 transfer of one chunk overlaps the conversion of the previous one; the generic pairwise variant (8 source
-    // vectors per chunk) has no registers for that and only overlaps its loads with the wait for the ring slot.
-    constexpr bool PREFETCH = PAIRED;
+    // PAIRED GEN_NORM / GEN_COPY: the 256-bit source loads of chunk c+1 are issued before chunk c is converted (two
+    // register sets, ping-pong), so the L2 transfer of one chunk overlaps the conversion of the previous one; the generic
+    // pairwise variant (8 source vectors per chunk) has no registers for that and only overlaps its loads with the wait
+    // for the ring slot.  PAIRED GEN_PAIR_*: the sources come through shared memory (STAGED, below).
+    constexpr bool STAGED = staged(GEN, PAIRED);
+    constexpr bool PREFETCH = PAIRED && !STAGED;
     constexpr bool ROWS = GEN == GEN_NORM || GEN == GEN_COPY;      // the operand is a function of one fp32 source row
     constexpr int NA = (ROWS || !PAIRED) ? 4 : 2;                  // source vectors of 8 floats per chunk: a / y ...
     constexpr int NB = ROWS ? 0 : (PAIRED ? 2 : 4);                // ... and b
@@ -317,7 +346,78 @@ static __global__ void __launch_bounds__(G_THREADS, 1) gemm_gen_kernel(const Gen
         if (lane == 0) mbar_arrive(full_bar(s));
         it++;
       };
-      if (PREFETCH) {
+      if (STAGED) {
+        // Per chunk, the first producer thread loads the detection box [128 rows x 32 channels] (rows g*Lf + n ..,
+        // 128-byte swizzle: 16-byte unit u of box row j at unit u ^ (j & 7)) into the stage's free slot at A_SUB and the
+        // two object rows i0, i0 + 1 into the stage's object area, G_SRC_AHEAD chunks ahead.  The slot of chunk c + 2
+        // was last read by chunk c - 1, so the refill waits only for every producer warp to be done with that one.
+        // A quarter warp's eight detections j = cb + 64 b share a k group and have eight different j & 7: its 16-byte
+        // reads hit eight different bank groups.
+        const bool gen_ops = !(P.t.dbg & 4);
+        const int row_det = g * P.Lf + P.n, row_obj = g * P.Lf + c0 / P.m;
+        auto issue = [&](uint32_t pos, int kc) {
+          const int s = pos % STAGES;
+          mbar_wait(src_empty(s), ((pos / STAGES) & 1) ^ 1u);
+          mbar_expect_tx(src_full(s), G_DET_BYTES + G_OBJ_BYTES);
+          tma::tma_load_2d(base + s * STAGE_BYTES + A_SUB, &map_det, kc * BK, row_det, src_full(s));
+          tma::tma_load_2d(obj0 + s * G_OBJ_BYTES, &map_obj, kc * BK, row_obj, src_full(s));
+        };
+        if (pt == 0 && gen_ops)
+          for (int kc = 0; kc < KC && kc < G_SRC_AHEAD; kc++) issue(it + kc, kc);
+        const uint32_t u0 = (uint32_t)(((2 * kg) ^ (cb & 7)) * 16), u1 = (uint32_t)(((2 * kg + 1) ^ (cb & 7)) * 16);
+        for (int kc = 0; kc < KC; kc++) {
+          const int s = it % STAGES;
+          mbar_wait(empty_bar(s), ((it / STAGES) & 1) ^ 1u);
+          if (pt == 0) {   // the chunk's weight block
+            if (P.t.dbg & 2) {
+              mbar_arrive(full_bar(s));
+            } else {
+              mbar_expect_tx(full_bar(s), A_SUB);
+              bulk_g2s(base + s * STAGE_BYTES, reinterpret_cast<const uint8_t*>(P.t.Wp) + ((size_t)kc * P.t.m_tiles + mg) * A_SUB,
+                       A_SUB, full_bar(s));
+            }
+          }
+          if (gen_ops) {
+            uint8_t* bh = sm + s * STAGE_BYTES + 2 * A_SUB + off0;
+            const uint32_t db = base + s * STAGE_BYTES + A_SUB + (uint32_t)cb * 128u, ob = obj0 + s * G_OBJ_BYTES + kg * 32;
+            mbar_wait(src_full(s), (it / STAGES) & 1);
+            float4 d[2][2];   // detections j = cb, cb + 64: channels kg*8 .. kg*8 + 7
+            lds128(db + u0, d[0][0]); lds128(db + u1, d[0][1]);
+            lds128(db + 64 * 128 + u0, d[1][0]); lds128(db + 64 * 128 + u1, d[1][1]);
+#pragma unroll
+            for (int a = 0; a < 2; a++) {
+              float4 o[2];    // object row i0 + a (every lane of a k group reads the same 32 bytes: a broadcast)
+              lds128(ob + a * BK * 4, o[0]); lds128(ob + a * BK * 4 + 16, o[1]);
+              const float av[8] = {o[0].x, o[0].y, o[0].z, o[0].w, o[1].x, o[1].y, o[1].z, o[1].w};
+#pragma unroll
+              for (int b = 0; b < 2; b++) {
+                const int r = 2 * a + b;
+                const float bv[8] = {d[b][0].x, d[b][0].y, d[b][0].z, d[b][0].w, d[b][1].x, d[b][1].y, d[b][1].z, d[b][1].w};
+                float x[8];
+#pragma unroll
+                for (int e = 0; e < 8; e++) {
+                  if (GEN == GEN_PAIR_MUL) x[e] = av[e] * bv[e];
+                  else if (GEN == GEN_PAIR_ABS) x[e] = fabsf(av[e] - bv[e]) * 0.5f;
+                  else x[e] = (av[e] - bv[e]) * 0.5f;
+                }
+                uint32_t h[4], l[4];
+#pragma unroll
+                for (int q = 0; q < 4; q++) split_f16x2(x[2 * q], x[2 * q + 1], h[q], l[q]);
+                if (!((okmask >> r) & 1u)) { h[0] = h[1] = h[2] = h[3] = 0u; l[0] = l[1] = l[2] = l[3] = 0u; }
+                *reinterpret_cast<uint4*>(bh + r * 1024) = make_uint4(h[0], h[1], h[2], h[3]);
+                *reinterpret_cast<uint4*>(bh + B_HALF + r * 1024) = make_uint4(l[0], l[1], l[2], l[3]);
+              }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(src_empty(s));   // this warp is done with the stage's sources
+          }
+          fence_async_smem();   // generic-proxy writes -> visible to the tensor core (async proxy)
+          __syncwarp();
+          if (lane == 0) mbar_arrive(full_bar(s));
+          if (pt == 0 && gen_ops && kc + G_SRC_AHEAD < KC) issue(it + G_SRC_AHEAD, kc + G_SRC_AHEAD);
+          it++;
+        }
+      } else if (PREFETCH) {
         Raw R0, R1;
         load(R0, 0);
         for (int kc = 0; kc < KC; kc += 2) {
@@ -367,9 +467,19 @@ static int gemm_gen_launch_t(const GemmP& g, const uint4* Wp, float out_scale, c
   P.t.dbg = mm_debug_flags();
   P.src = src; P.ld_src = ld_src; P.gsc = gsc; P.gsh = gsh;
   P.n = n; P.m = m; P.Lf = Lf;
+  alignas(64) CUtensorMap map_det, map_obj;
+  memset(&map_det, 0, sizeof(map_det));
+  memset(&map_obj, 0, sizeof(map_obj));
+  if (gen::staged(GEN, PAIRED)) {
+    // two whole object rows per tile against all m = 128 detections; maps over the feature stacks [G * Lf][K]
+    if (m != 128 || Lf != n + m || g.tile_tab || g.tiles_per_group <= 0) return MMMOT_E_ARG;
+    const long rows = (long)(g.num_tiles / g.tiles_per_group) * Lf;
+    MM_TRY(tma::make_map_2d_f32(&map_det, src, rows, g.K, 128, CU_TENSOR_MAP_SWIZZLE_128B));
+    MM_TRY(tma::make_map_2d_f32(&map_obj, src, rows, g.K, 2, CU_TENSOR_MAP_SWIZZLE_NONE));
+  }
   const long total = (long)g.num_tiles * P.t.m_tiles;
   const int grid = (int)(total < sms ? total : sms);
-  gen::gemm_gen_kernel<GEN, PAIRED><<<grid, gen::G_THREADS, gen::G_SMEM_BYTES, st>>>(P);
+  gen::gemm_gen_kernel<GEN, PAIRED><<<grid, gen::G_THREADS, gen::G_SMEM_BYTES, st>>>(P, map_det, map_obj);
   MM_LAUNCH_CHECK();
   return 0;
 }
@@ -383,6 +493,12 @@ static inline bool gen_prefetch(int GEN, int m, int dbg) {
   if (GEN == gen::GEN_NORM) return (dbg & 4096) != 0;
   if (GEN == gen::GEN_COPY) return true;
   return m == 128;
+}
+
+// Whether that variant stages the pairwise sources in shared memory by TMA (the pipelined GEN_PAIR_* producers).  Pure
+// host logic, like gen_prefetch (mmmot_debug_gen_staged).
+static inline bool gen_staged(int GEN, int m, int dbg) {
+  return GEN <= gen::GEN_PAIR_SUB && gen_prefetch(GEN, m, dbg);
 }
 
 // prefetched (host, or NULL) receives the variant taken (gen_prefetch)

@@ -596,6 +596,19 @@ static inline int make_map_2d(CUtensorMap* m, const void* basep, long rows, int 
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
 }
+// fp32 [rows][C] matrix (row stride C elements), box 32 x box_rows: 128-byte box rows, so SWIZZLE_128B is allowed
+static inline int make_map_2d_f32(CUtensorMap* m, const void* basep, long rows, int C, int box_rows,
+                                  CUtensorMapSwizzle swizzle) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return MMMOT_E_ARG;
+  cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)C * 4};
+  cuuint32_t box[2] = {32, (cuuint32_t)box_rows}, es[2] = {1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(basep), dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
+}
 // fp16 NHWC [n_img][H][W][C], box (32, bx, by, bi)
 static inline int make_map_4d(CUtensorMap* m, const void* basep, int n_img, int H, int W, int C, int bx, int by,
                               int bi) {
