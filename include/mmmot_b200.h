@@ -290,7 +290,8 @@ int mmmot_set_kseg(int chunks);
  * the other bits select an alternative implementation of the same arithmetic.  Default 0.
  *   bit 0 (1)    skip epilogue work          bit 1 (2)   skip weight loads
  *   bit 2 (4)    skip operand loads          bit 3 (8)   skip MMA issue
- *   bit 4 (16)   unused
+ *   bit 4 (16)   PointNet's layer-5 and head GroupNorm statistics by a statistics-only pass of the contraction itself
+ *                instead of from the input's moments (mmmot_debug_pn_stats)
  *   bit 5 (32)   first VGG layer as the direct FP32 FFMA kernel instead of im2col + tensor cores
  *   bit 6 (64)   64-channel layers on the channel-major kernel instead of the pixel-major one
  *   bit 7 (128)  pixel-major epilogue with 16-byte stores instead of whole 32-byte sectors
@@ -345,6 +346,21 @@ int mmmot_debug_pn_contraction(const int* det_split, const int* h_det_split, int
                                int* cnt, int* gstart, int* seg, void* ctab, long* n_tiles, const void* Wp, float wp_scale,
                                const float* bias, int M, int K, const void* Xhi, float* Y, void* part, const float* addend,
                                int ld_add, unsigned long long* segsum, const float* sc, const float* sh, void* stream);
+
+/* Test hook of the GroupNorm statistics of PointNet's two widest tensor-core layers (csrc/pointnet.cu), computed as
+ * mmmot_pointnet_fwd computes them under the current mmmot_set_debug bits: y = x Wt + bias (+ addend[det]) over the
+ * FP16 planes X [2][P][K] (Xhi) of the ragged detections det_split [pairs*L + 1] (device; h_det_split on the host);
+ * K = 128 (layer 5, no addend) or 64 (head); M <= 1024, a multiple of 64; addend [det][M] or NULL.  Default: from the
+ * input's moments, Wt [K][M] fp32 (Wp ignored); bit 4: a statistics-only contraction with the packed tiles Wp / wp_scale
+ * (Wt ignored).  Then GroupNorm(M, M) per pair: sc / sh [pairs][M] (gamma, beta [M]).  Optional copies out: stats
+ * [pairs][M][2] (sum y, sum y^2) fp64; default path only: mom [pairs][K*K + K] = (sum x x^T row-major, sum x) fp64 and,
+ * for K = 64, detsum [det][64] = per-detection sums of x in 2^-32 fixed point.  workspace: the tensor-core PointNet
+ * workspace, mmmot_pointnet_workspace(pairs, L, P) bytes with L >= 16 or under mmmot_set_engine(2) (otherwise that
+ * function sizes the FP32 path's smaller layout and this hook returns MMMOT_E_WORKSPACE). */
+int mmmot_debug_pn_stats(const int* det_split, const int* h_det_split, int pairs, int L, const void* Xhi, int K,
+                         const float* Wt, const void* Wp, float wp_scale, const float* bias, int M, const float* addend,
+                         const float* gamma, const float* beta, float* sc, float* sh, double* stats, double* mom,
+                         unsigned long long* detsum, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Test hooks of the TMA-fed tensor-core engine: operands are two FP16 planes (hi, lo), channels-last.
  * linear: Y[rows][M] fp32 = X W^T + bias, X planes [2][rows][K].  conv: 3x3 pad 1 + bias + ReLU on NHWC planes

@@ -90,7 +90,8 @@ const char* const kTagNames[MM_T_COUNT] = {
     "pointnet.l5_128to1024_stats", "pointnet.l5_128to1024_segsum", "pointnet.head_64to512_stats",
     "pointnet.head_64to512_segsum",
     "affinity.l1_pair_512to1024", "affinity.newend_means", "affinity.l2_512to512", "affinity.l3_512to128",
-    "affinity.logit", "lp.assign"};
+    "affinity.logit", "lp.assign", "pointnet.moments_128", "pointnet.moments_64",
+    "pointnet.moments_finalize"};
 }  // namespace
 
 bool mm_timing_on() { return g_timing; }

@@ -41,7 +41,9 @@ enum {
   MM_T_PN_HEADA = 21, MM_T_PN_HEADB = 22,    // head 64 -> 512, two passes
   MM_T_AFF_L1 = 23, MM_T_AFF_MEAN = 24, MM_T_AFF_L2 = 25, MM_T_AFF_L3 = 26, MM_T_AFF_LOGIT = 27,
   MM_T_LP = 28,
-  MM_T_COUNT = 29
+  MM_T_PN_MOM128 = 29, MM_T_PN_MOM64 = 30,   // input moments of layer 5 and of the head (their GroupNorm statistics)
+  MM_T_PN_MOMFIN = 31,                       // their slice tables, fixed-order reductions and fp64 statistics
+  MM_T_COUNT = 32
 };
 bool mm_timing_on();
 void mm_timing_begin(cudaStream_t st, int tag, double flop, double bytes);

@@ -6,6 +6,8 @@
 //   * the 1088-wide head conv splits into a 64-wide per-point part plus a per-detection
 //     addend  Wh[:,64:] * mean_det(x5)  (1088 -> 64 MACs per point per output channel).
 // Per-detection pooling is a MEAN (SURVEY F5).  One frame-pair = one GroupNorm domain.
+#include <algorithm>
+#include <atomic>
 #include <vector>
 
 #include "norm_ops.cuh"
@@ -183,14 +185,286 @@ __global__ void pn_tiles_kernel(const int* __restrict__ split, int pairs, int L,
   }
 }
 
+// ---------------- GroupNorm statistics of the two widest layers from the moments of their input ----------------
+// GroupNorm(C, C) over a pair's n points of y = W x + b (+ a[det]) needs, per output channel, only the mean and the
+// variance of y, and both follow from the input's moments: S1 = sum x, S2 = sum x x^T (C x C) and, with an addend,
+// the per-detection sums of x.  Building them costs C^2 MACs per point instead of the layer's C x M (M = 8C here).
+namespace pnm {
+constexpr int KC = 32;        // points per pipeline stage
+constexpr int NSTG = 4;       // pipeline stages
+constexpr int SLICE = 32;     // tiles (of 256 points) per CTA
+
+template <int C> __host__ __device__ constexpr int threads() { return (C / 32) * (C / 32) * 32; }   // one warp per 32 x 32 block of S2
+template <int C> __host__ __device__ constexpr size_t ring_bytes() { return (size_t)NSTG * 2 * KC * (C + 8) * sizeof(__half); }
+// ring + the fp64 accumulators of S2 (32 per thread, kept in shared memory: in registers they would spill)
+template <int C> constexpr size_t smem_bytes() { return ring_bytes<C>() + 32 * sizeof(double) * threads<C>(); }
+constexpr long part_doubles(long max_tiles, int pairs) { return (max_tiles / SLICE + pairs) * (128L * 128 + 128); }
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// Moments of the FP16 hi/lo planes X [2][P][C] (x = hi + lo), one CTA per slice: slice j of pair p is the pair's tiles
+// gstart[p] + j*SLICE .. (at most SLICE, never past the pair), a contiguous range of its points; sstart [pairs + 1] =
+// first slice of each pair.  part[slice][C*C + C] (fp64) = S2 row-major, then S1, over the slice's points.
+// S2 ~ XhT Xh + XhT Xl + XlT Xh on mma.sync (points are the K dimension, so both operands are read transposed from the
+// channels-last rows with ldmatrix.trans); the fp32 accumulators restart at every 256-point tile and are added into
+// fp64 ones, so no fp32 chain spans more than one tile.  S1 in fp64 (x = hi + lo is exact in fp32).
+// DET: also detsum[det][C] += the detection's sums of x in 2^-32 fixed point (integer adds: order-independent).
+// Every partial depends only on the pair's data, never on the grid or on the rest of the batch.
+template <int C, bool DET>
+__global__ void __launch_bounds__(threads<C>(), 1)
+pn_moments_kernel(const __half* __restrict__ X, long P, const int4* __restrict__ tiles, const int* __restrict__ gstart,
+                  const int* __restrict__ sstart, int pairs, const int* __restrict__ seg, double* __restrict__ part,
+                  unsigned long long* __restrict__ detsum) {
+  constexpr int NT = threads<C>(), LD = C + 8, PLANE = KC * LD, STAGE = 2 * PLANE;   // smem rows padded: no conflicts
+  constexpr int Q = NT / C, R = KC / Q;     // per-channel sums: thread (c, q) takes rows [q R, q R + R) of each stage
+  constexpr int CH = C / 8;                  // 16-byte chunks per row
+  extern __shared__ __align__(16) __half sm[];
+  const int s = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int lo = 0, hi = pairs;                    // the pair: sstart[lo] <= s < sstart[lo + 1]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (sstart[mid] <= s) lo = mid; else hi = mid;
+  }
+  const int t0 = gstart[lo] + (s - sstart[lo]) * SLICE, t1 = min(t0 + SLICE, gstart[lo + 1]);
+  const long r0 = tiles[t0].y;
+  const int n = (int)(tiles[t1 - 1].y + tiles[t1 - 1].z - r0);
+  const int nst = (n + KC - 1) / KC;
+  const uint32_t sbase = tc::smem_u32(sm);
+
+  auto load = [&](int k) {
+    const uint32_t dst0 = sbase + (uint32_t)((k % NSTG) * STAGE * 2);
+#pragma unroll
+    for (int i = tid; i < 2 * KC * CH; i += NT) {
+      const int pl = i / (KC * CH), row = (i / CH) % KC, ch = i % CH;
+      const int r = k * KC + row;
+      const __half* src = r < n ? X + pl * P * C + (r0 + r) * C + ch * 8 : X;
+      cp_async16(dst0 + (uint32_t)((pl * PLANE + row * LD + ch * 8) * 2), src, r < n ? 16 : 0);   // zero-fills the tail
+    }
+  };
+
+  const int wi = warp / (C / 32), wj = warp % (C / 32);
+  float acc[2][4][4];
+  double* acc64 = reinterpret_cast<double*>(reinterpret_cast<char*>(sm) + ring_bytes<C>()) + tid;   // [32][NT]
+#pragma unroll
+  for (int a = 0; a < 2; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) { acc[a][b][e] = 0.f; acc64[((a * 4 + b) * 4 + e) * NT] = 0.0; }
+  const int c = tid % C, q = tid / C;
+  double s1 = 0.0;
+  int dcur = -1;
+  long long run = 0;
+
+#pragma unroll
+  for (int k = 0; k < NSTG - 1; k++) {
+    if (k < nst) load(k);
+    cp_commit();
+  }
+  for (int k = 0; k < nst; k++) {
+    cp_wait<NSTG - 2>();
+    __syncthreads();                         // stage k landed for all; stage k - 1's buffer is free
+    if (k + NSTG - 1 < nst) load(k + NSTG - 1);
+    cp_commit();
+    const uint32_t st_hi = sbase + (uint32_t)((k % NSTG) * STAGE * 2), st_lo = st_hi + PLANE * 2;
+#pragma unroll
+    for (int ks = 0; ks < KC / 16; ks++) {
+      uint32_t ah[2][4], al[2][4];
+      const int ka = ks * 16 + (lane & 7) + ((lane >> 4) & 1) * 8;
+#pragma unroll
+      for (int mt = 0; mt < 2; mt++) {
+        const uint32_t off = (uint32_t)((ka * LD + wi * 32 + mt * 16 + ((lane >> 3) & 1) * 8) * 2);
+        ldsm_x4_t(st_hi + off, ah[mt]);
+        ldsm_x4_t(st_lo + off, al[mt]);
+      }
+      const int kb = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+      for (int np = 0; np < 2; np++) {
+        uint32_t bh[4], bl[4];
+        const uint32_t off = (uint32_t)((kb * LD + wj * 32 + np * 16 + ((lane >> 4) & 1) * 8) * 2);
+        ldsm_x4_t(st_hi + off, bh);
+        ldsm_x4_t(st_lo + off, bl);
+#pragma unroll
+        for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+          for (int h = 0; h < 2; h++) {
+            float (&d)[4] = acc[mt][np * 2 + h];
+            mma16816(d, ah[mt], bh[2 * h], bh[2 * h + 1]);
+            mma16816(d, ah[mt], bl[2 * h], bl[2 * h + 1]);
+            mma16816(d, al[mt], bh[2 * h], bh[2 * h + 1]);
+          }
+      }
+    }
+    {
+      const __half* xs = sm + (k % NSTG) * STAGE + q * R * LD + c;
+#pragma unroll 4
+      for (int rr = 0; rr < R; rr++) {
+        const int r = k * KC + q * R + rr;
+        if (r >= n) break;
+        const float x = __half2float(xs[rr * LD]) + __half2float(xs[PLANE + rr * LD]);
+        s1 += (double)x;
+        if (DET) {
+          const int d = seg[r0 + r];
+          if (d != dcur) {
+            if (dcur >= 0) atomicAdd(detsum + (long)dcur * C + c, (unsigned long long)run);
+            dcur = d;
+            run = 0;
+          }
+          run += __float2ll_rn(x * 4294967296.f);
+        }
+      }
+    }
+    if ((k & 7) == 7 || k == nst - 1) {      // end of a 256-point tile
+#pragma unroll
+      for (int a = 0; a < 2; a++)
+#pragma unroll
+        for (int b = 0; b < 4; b++)
+#pragma unroll
+          for (int e = 0; e < 4; e++) { acc64[((a * 4 + b) * 4 + e) * NT] += (double)acc[a][b][e]; acc[a][b][e] = 0.f; }
+    }
+  }
+  if (DET && dcur >= 0) atomicAdd(detsum + (long)dcur * C + c, (unsigned long long)run);
+
+  double* out = part + (long)s * (C * C + C);
+#pragma unroll
+  for (int a = 0; a < 2; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++) {
+      const int i = wi * 32 + a * 16 + (lane >> 2), j = wj * 32 + b * 8 + 2 * (lane & 3);
+      const double* v = acc64 + (a * 4 + b) * 4 * NT;
+      *reinterpret_cast<double2*>(out + (long)i * C + j) = make_double2(v[0], v[NT]);
+      *reinterpret_cast<double2*>(out + (long)(i + 8) * C + j) = make_double2(v[2 * NT], v[3 * NT]);
+    }
+  cp_wait<0>();
+  __syncthreads();                           // every stage read: the ring holds the S1 reduction now
+  double* red = reinterpret_cast<double*>(sm);
+  red[q * C + c] = s1;
+  __syncthreads();
+  if (tid < C) {
+    double v = 0.0;
+#pragma unroll
+    for (int g = 0; g < Q; g++) v += red[g * C + tid];
+    out[C * C + tid] = v;
+  }
+}
+
+// sstart[p] = first slice of pair p (pairs + 1 entries) from the tile starts gstart (one thread: pairs is small)
+__global__ void pn_slices_kernel(const int* __restrict__ gstart, int pairs, int* __restrict__ sstart) {
+  int acc = 0;
+  for (int p = 0; p < pairs; p++) {
+    sstart[p] = acc;
+    acc += (gstart[p + 1] - gstart[p] + SLICE - 1) / SLICE;
+  }
+  sstart[pairs] = acc;
+}
+
+// mom[p][e] = sum over pair p's slices, in slice order, of part[slice][e]   (E = C*C + C)
+__global__ void pn_moments_reduce_kernel(const double* __restrict__ part, const int* __restrict__ sstart, int E,
+                                         double* __restrict__ mom) {
+  const int p = blockIdx.y, e = blockIdx.x * 256 + threadIdx.x;
+  if (e >= E) return;
+  double a = 0.0;
+  for (int s = sstart[p]; s < sstart[p + 1]; s++) a += part[(long)s * E + e];
+  mom[(long)p * E + e] = a;
+}
+
+// stats[p][o] = (sum y, sum y^2) over pair p's n points of y = x Wt[:, o] + bias[o] (+ addend[det][o]), the format
+// gn_finalize reads, from the pair's moments mom[p] = (S2, S1) in centred form (no cancellation in y):
+//   mu = S1 / n,  Cov = S2 / n - mu mu^T,  mean = w.mu + b,  var = w^T Cov w.
+// With the addend a_d = addend[d] + b (per detection d of n_d points with sums s1_d = detsum[d] 2^-32) and its
+// point-weighted mean abar:  mean = w.mu + abar,  var += (2/n) sum_d (a_d - abar) w.(s1_d - n_d mu)
+//                                                       + (1/n) sum_d n_d (a_d - abar)^2.
+// Wt [C][M] are the fp32 master weights.  CTA = 64 output channels x 4 row groups of the quadratic form.
+template <int C>
+__global__ void __launch_bounds__(256) pn_moments_stats_kernel(const double* __restrict__ mom, const int* __restrict__ cnt,
+                                                               const float* __restrict__ Wt, const float* __restrict__ bias,
+                                                               int M, const float* __restrict__ addend,
+                                                               const unsigned long long* __restrict__ detsum,
+                                                               const int* __restrict__ det_split, int L,
+                                                               double* __restrict__ stats) {
+  __shared__ float ws[C][64];
+  __shared__ double mu[C];
+  __shared__ double cv[8][C];
+  __shared__ double red[4][64];
+  const int p = blockIdx.y, o0 = blockIdx.x * 64, ol = threadIdx.x & 63, q = threadIdx.x >> 6, o = o0 + ol;
+  const double* S2 = mom + (long)p * (C * C + C);
+  const double n = (double)cnt[p];
+  for (int i = threadIdx.x; i < C * 64; i += 256) ws[i / 64][i % 64] = o0 + i % 64 < M ? Wt[(long)(i / 64) * M + o0 + i % 64] : 0.f;
+  for (int i = threadIdx.x; i < C; i += 256) mu[i] = S2[C * C + i] / n;
+  __syncthreads();
+  double wmu = 0.0;
+  for (int k = 0; k < C; k++) wmu += (double)ws[k][ol] * mu[k];
+  double var = 0.0;
+  for (int i0 = 0; i0 < C; i0 += 8) {
+    for (int e = threadIdx.x; e < 8 * C; e += 256) {
+      const int r = e / C, j = e % C;
+      cv[r][j] = S2[(long)(i0 + r) * C + j] / n - mu[i0 + r] * mu[j];
+    }
+    __syncthreads();
+    for (int r = 2 * q; r < 2 * q + 2; r++) {
+      double t = 0.0;
+      for (int j = 0; j < C; j++) t += cv[r][j] * (double)ws[j][ol];
+      var += (double)ws[i0 + r][ol] * t;
+    }
+    __syncthreads();
+  }
+  const bool valid = o < M;
+  double mean = wmu + (valid ? (double)bias[o] : 0.0);
+  if (addend && valid) {
+    const double b = (double)bias[o];
+    double abar = 0.0;
+    for (int l = 0; l < L; l++) {
+      const int d = p * L + l;
+      abar += (double)(det_split[d + 1] - det_split[d]) * ((double)addend[(long)d * M + o] + b);
+    }
+    abar /= n;
+    double cross = 0.0, between = 0.0;
+    for (int l = q; l < L; l += 4) {
+      const int d = p * L + l;
+      const double nd = (double)(det_split[d + 1] - det_split[d]);
+      const double a = (double)addend[(long)d * M + o] + b - abar;
+      double ws1 = 0.0;
+      for (int k = 0; k < C; k++)
+        ws1 += (double)ws[k][ol] * ((double)(long long)detsum[(long)d * C + k] * (1.0 / 4294967296.0) - nd * mu[k]);
+      cross += a * ws1;
+      between += nd * a * a;
+    }
+    var += (2.0 * cross + between) / n;
+    mean = wmu + abar;
+  }
+  red[q][ol] = var;
+  __syncthreads();
+  if (q == 0 && valid) {
+    const double v = fmax(red[0][ol] + red[1][ol] + red[2][ol] + red[3][ol], 0.0);
+    stats[((long)p * M + o) * 2] = n * mean;
+    stats[((long)p * M + o) * 2 + 1] = n * (v + mean * mean);
+  }
+}
+}  // namespace pnm
+
 struct PnWs {
   float *xt, *y1, *t0, *t1, *big, *gmean, *u, *ut, *hmean, *o;
   unsigned long long* segsum;   // tensor-core path: [ndet][1024] fixed-point per-detection sums
   __half *x1p, *xp;     // tensor-core path: FP16 hi/lo planes of normalised activations [2][P][64], [2][P][128]
   float *sc1, *sh1, *sc, *sh;
-  double* stats;
-  double2* part;
-  int *seg, *cnt, *gstart;
+  double *stats, *mom;  // mom (tensor-core path): [pairs][128*128 + 128] input moments of the widest layers
+  double2* part;        // tensor-core path: also the moments kernel's per-slice partials (used one at a time)
+  int *seg, *cnt, *gstart, *sstart;
   int4 *tiles, *ctab;
 };
 
@@ -216,8 +490,11 @@ PnWs carve(MmArena& a, int pairs, int L, long P, long max_tiles, bool use_tc) {
   w.sc = a.take<float>((size_t)pairs * 1024);
   w.sh = a.take<float>((size_t)pairs * 1024);
   w.stats = a.take<double>((size_t)pairs * 1024 * 2);
-  w.part = a.take<double2>((size_t)max_tiles * 1024);
+  w.mom = a.take<double>(use_tc ? (size_t)pairs * (128 * 128 + 128) : 0);
+  w.part = a.take<double2>(use_tc ? std::max((size_t)max_tiles * 1024, (size_t)(pnm::part_doubles(max_tiles, pairs) + 1) / 2)
+                                  : (size_t)max_tiles * 1024);
   w.gstart = a.take<int>(pairs + 1);
+  w.sstart = a.take<int>(use_tc ? pairs + 1 : 0);
   w.seg = a.take<int>(P);
   w.cnt = a.take<int>(pairs);
   w.tiles = a.take<int4>(max_tiles);
@@ -247,6 +524,71 @@ int pn_tables(const int* det_split, int pairs, int L, long P, int tw, long n_til
     tma::seg_chunk_tab_kernel<<<mm_cdiv(n_tiles * 2, 128), 128, 0, st>>>(tiles, (int)n_tiles, seg, ctab);
     MM_LAUNCH_CHECK();
   }
+  return 0;
+}
+
+template <int C, bool DET>
+int pn_moments_launch(const PnWs& w, const __half* X, long P, int pairs, long n_slices, cudaStream_t st) {
+  static std::atomic<unsigned long long> smem_set{0};
+  MM_TRY(mm_ensure_smem(pnm::pn_moments_kernel<C, DET>, pnm::smem_bytes<C>(), smem_set));
+  pnm::pn_moments_kernel<C, DET><<<(int)n_slices, pnm::threads<C>(), pnm::smem_bytes<C>(), st>>>(
+      X, P, w.tiles, w.gstart, w.sstart, pairs, w.seg, (double*)w.part, w.segsum);
+  MM_LAUNCH_CHECK();
+  return 0;
+}
+
+// GroupNorm(M, M) statistics w.stats [pairs][M] (sum, sum of squares per pair and channel) of the tensor-core path's
+// widest layers, y = x Wt + bias (+ addend[det], [ndet][M]) over the FP16 hi/lo planes X [2][P][K], K = 128 (layer 5,
+// 128 -> 1024) or 64 (head, 64 -> 512, with the addend).  Default: from the input's moments (pnm above); Wt [K][M] are
+// the fp32 master weights.  Debug bit 4: the contraction itself with only its GroupNorm partials kept (Wp / wps, the
+// packed tiles), then their fixed-order reduction.  Tables (tiles, gstart, cnt, seg, ctab) as pn_tables left them.
+int pn_wide_stats(const PnWs& w, const int* h_det_split, const int* det_split, long P, int pairs, int L, long n_tiles,
+                  const __half* X, int K, const float* Wt, const uint4* Wp, float wps, const float* bias, int M,
+                  const float* addend, cudaStream_t st) {
+  const bool timed = mm_timing_on();
+  if (mm_debug_flags() & 16) {
+    GemmP p = gemm_defaults();
+    p.bias = bias; p.M = M; p.K = K;
+    p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
+    p.Y = nullptr; p.y_ms = M;
+    p.part = w.part;
+    if (addend) { p.addend = addend; p.seg = w.seg; p.ld_add = M; }
+    if (timed) mm_timing_begin(st, K == 128 ? MM_T_PN_L5A : MM_T_PN_HEADA, 2.0 * M * K * (double)P, 4.0 * K * (double)P);
+    MM_TRY(gemm_tma_launch_mat(p, Wp, wps, X, P * K, P, K, tc::OUT_CL, 0, st, nullptr, nullptr, addend ? w.ctab : nullptr));
+    if (timed) mm_timing_end(st);
+    return stats_reduce(w.part, M, pairs, 0, w.gstart, w.stats, st, 2);
+  }
+  long n_slices = 0;
+  for (int p = 0; p < pairs; p++)
+    n_slices += mm_cdiv(mm_cdiv((long)h_det_split[(p + 1) * L] - h_det_split[p * L], tc::BN), pnm::SLICE);
+  const int E = K * K + K;
+  if (timed) mm_timing_begin(st, MM_T_PN_MOMFIN, 0.0, 0.0);
+  pnm::pn_slices_kernel<<<1, 1, 0, st>>>(w.gstart, pairs, w.sstart);
+  MM_LAUNCH_CHECK();
+  if (timed) mm_timing_end(st);
+  // algorithmic work: S2 (2 K^2 FLOPs per point; the MMAs issue three times that); compulsory traffic: the two FP16
+  // planes (and the point -> detection map with the per-detection sums)
+  if (K == 128) {
+    if (timed) mm_timing_begin(st, MM_T_PN_MOM128, 2.0 * K * K * (double)P, 4.0 * K * (double)P);
+    MM_TRY((pn_moments_launch<128, false>(w, X, P, pairs, n_slices, st)));
+  } else {
+    MM_CUDA(cudaMemsetAsync(w.segsum, 0, (size_t)pairs * L * 64 * sizeof(unsigned long long), st));
+    if (timed) mm_timing_begin(st, MM_T_PN_MOM64, 2.0 * K * K * (double)P, (4.0 * K + 4.0) * (double)P);
+    MM_TRY((pn_moments_launch<64, true>(w, X, P, pairs, n_slices, st)));
+  }
+  if (timed) mm_timing_end(st);
+  // slice partials in, pair moments out; the quadratic forms w^T Cov w (2 K^2 FLOPs per pair and channel)
+  if (timed) mm_timing_begin(st, MM_T_PN_MOMFIN, 2.0 * K * K * (double)M * pairs, 8.0 * E * (double)(n_slices + pairs));
+  pnm::pn_moments_reduce_kernel<<<dim3(mm_cdiv(E, 256), pairs), 256, 0, st>>>((const double*)w.part, w.sstart, E, w.mom);
+  MM_LAUNCH_CHECK();
+  if (K == 128)
+    pnm::pn_moments_stats_kernel<128><<<dim3(mm_cdiv(M, 64), pairs), 256, 0, st>>>(w.mom, w.cnt, Wt, bias, M, nullptr, nullptr,
+                                                                                   det_split, L, w.stats);
+  else
+    pnm::pn_moments_stats_kernel<64><<<dim3(mm_cdiv(M, 64), pairs), 256, 0, st>>>(w.mom, w.cnt, Wt, bias, M, addend, w.segsum,
+                                                                                  det_split, L, w.stats);
+  MM_LAUNCH_CHECK();
+  if (timed) mm_timing_end(st);
   return 0;
 }
 
@@ -322,7 +664,7 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
       GemmP p = gemm_defaults();
       p.bias = q[1]; p.M = cout[i]; p.K = cin[i];
       p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
-      p.Y = ybuf[i]; p.y_ms = cout[i];       // layer 5 (1024 wide): statistics only, nothing stored
+      p.Y = ybuf[i]; p.y_ms = cout[i];
       p.part = w.part;
       const uint4* wp = (const uint4*)wts->w[MMMOT_W_PN_WP1 + i];
       const float wps = wts->tc_scale[MMMOT_W_PN_WP1 + i];
@@ -332,10 +674,13 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
         pn_l1_stats_kernel<<<(int)n_tiles, 256, 0, st>>>(points, w.tiles, q[0], q[1], w.part);
         MM_LAUNCH_CHECK();
         if (timed) mm_timing_end(st);
+      } else if (i == 4) {
+        // layer 5 (1024 wide): statistics only, nothing stored
+        MM_TRY(pn_wide_stats(w, h_det_split, det_split, P, pairs, L, n_tiles, w.xp, cin[i], q[0], wp, wps, q[1], cout[i],
+                             nullptr, st));
       } else {
-        // compulsory traffic: activation in (4 B per element) + fp32 activation out (none for the statistics pass)
-        if (timed) mm_timing_begin(st, i == 4 ? MM_T_PN_L5A : MM_T_PN_L2 + (i - 1), 2.0 * cout[i] * cin[i] * cols,
-                                   4.0 * (cin[i] + (i == 4 ? 0 : cout[i])) * cols);
+        // compulsory traffic: activation in (4 B per element) + fp32 activation out
+        if (timed) mm_timing_begin(st, MM_T_PN_L2 + (i - 1), 2.0 * cout[i] * cin[i] * cols, 4.0 * (cin[i] + cout[i]) * cols);
         if (gen_mid && (i == 2 || i == 3)) {
           // layers 3, 4: GroupNorm + ReLU of the previous layer applied by this contraction's operand producers
           // (gemm_gen.cuh) straight from its fp32 output: no normalised copy is written
@@ -345,7 +690,7 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
         }
         if (timed) mm_timing_end(st);
       }
-      MM_TRY(stats_reduce(w.part, cout[i], pairs, 0, w.gstart, w.stats, st, 2));
+      if (i < 4) MM_TRY(stats_reduce(w.part, cout[i], pairs, 0, w.gstart, w.stats, st, 2));
       MM_TRY(gn_finalize(w.stats, q[2], q[3], w.cnt, 0, pairs, cout[i], 1, w.sc, w.sh, st, 0, 0, ar.status()));
       if (i == 0) {
         if (timed) mm_timing_begin(st, MM_T_PN_L1, 0.0, (12.0 + 4.0 * 64) * cols);
@@ -383,22 +728,19 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
                                              nullptr, nullptr, 0, 0, 0, st)));
     }
     {
+      const uint4* whp = (const uint4*)wts->w[MMMOT_W_PN_WHAP];
+      const float whs = wts->tc_scale[MMMOT_W_PN_WHAP];
+      MM_TRY(pn_wide_stats(w, h_det_split, det_split, P, pairs, L, n_tiles, w.x1p, 64, wts->w[MMMOT_W_PN_WHAT], whp, whs,
+                           wts->w[MMMOT_W_PN_BH], 512, w.ut, st));
+      MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GHW], wts->w[MMMOT_W_PN_GHB], w.cnt, 0, pairs, 512, 1, w.sc, w.sh, st));
+      // recompute + GroupNorm + ReLU + per-detection mean
+      MM_CUDA(cudaMemsetAsync(w.segsum, 0, (size_t)ndet * 512 * sizeof(unsigned long long), st));
       GemmP p = gemm_defaults();
       p.bias = wts->w[MMMOT_W_PN_BH]; p.M = 512; p.K = 64;
       p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
-      p.Y = nullptr; p.y_ms = 512;           // pass 1: statistics only
-      p.part = w.part;
+      p.Y = nullptr; p.y_ms = 512;
       p.addend = w.ut; p.seg = w.seg; p.ld_add = 512;
-      const uint4* whp = (const uint4*)wts->w[MMMOT_W_PN_WHAP];
-      const float whs = wts->tc_scale[MMMOT_W_PN_WHAP];
-      if (timed) mm_timing_begin(st, MM_T_PN_HEADA, 2.0 * 512 * 64 * (double)P, 4.0 * 64 * (double)P);
-      MM_TRY(gemm_tma_launch_mat(p, whp, whs, w.x1p, P * 64, P, 64, tc::OUT_CL, 0, st, nullptr, nullptr, w.ctab));
-      if (timed) mm_timing_end(st);
-      MM_TRY(stats_reduce(w.part, 512, pairs, 0, w.gstart, w.stats, st, 2));
-      MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GHW], wts->w[MMMOT_W_PN_GHB], w.cnt, 0, pairs, 512, 1, w.sc, w.sh, st));
-      // pass 2: recompute + GroupNorm + ReLU + per-detection mean
-      MM_CUDA(cudaMemsetAsync(w.segsum, 0, (size_t)ndet * 512 * sizeof(unsigned long long), st));
-      p.part = nullptr; p.sc = w.sc; p.sh = w.sh;
+      p.sc = w.sc; p.sh = w.sh;
       if (timed) mm_timing_begin(st, MM_T_PN_HEADB, 2.0 * 512 * 64 * (double)P, 4.0 * 64 * (double)P);
       MM_TRY(gemm_tma_launch_mat(p, whp, whs, w.x1p, P * 64, P, 64, tc::OUT_CL, 0, st, w.segsum, nullptr, w.ctab));
       if (timed) mm_timing_end(st);
@@ -525,4 +867,39 @@ extern "C" int mmmot_debug_pn_contraction(const int* det_split, const int* h_det
   if (addend || segsum) p.seg = seg;
   return gemm_tma_launch_mat(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, P * K, P, K, tc::OUT_CL, 0, st, segsum, nullptr,
                              (const int4*)ctab);
+}
+
+// The GroupNorm statistics of PointNet's widest layers exactly as pointnet_impl computes them (pn_wide_stats under the
+// current debug bits), then gn_finalize.  The workspace is a PointNet one (mmmot_pointnet_workspace(pairs, L, P)).
+extern "C" int mmmot_debug_pn_stats(const int* det_split, const int* h_det_split, int pairs, int L, const void* Xhi, int K,
+                                    const float* Wt, const void* Wp, float wp_scale, const float* bias, int M,
+                                    const float* addend, const float* gamma, const float* beta, float* sc, float* sh,
+                                    double* stats, double* mom, unsigned long long* detsum, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  if (!det_split || !h_det_split || pairs <= 0 || L <= 0 || !Xhi || !bias || !gamma || !beta || !sc || !sh || !workspace)
+    return MMMOT_E_ARG;
+  if (!(K == 64 || (K == 128 && !addend)) || M <= 0 || M > 1024 || M % 64) return MMMOT_E_ARG;
+  const bool two_pass = mm_debug_flags() & 16;
+  if (two_pass ? !Wp : !Wt) return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ndet = pairs * L;
+  const long P = h_det_split[ndet];
+  if (h_det_split[0] != 0 || P <= 0) return MMMOT_E_SHAPE;
+  for (int d = 0; d < ndet; d++)
+    if (h_det_split[d + 1] <= h_det_split[d]) return MMMOT_E_SHAPE;
+  const long n_tiles = pn_tile_count(h_det_split, pairs, L, tc::BN);
+  const long max_tiles = P / 128 + 2 * pairs + 2;
+  MmArena ar(workspace, workspace_bytes);
+  PnWs w = carve(ar, pairs, L, P, max_tiles, true);
+  if (!ar.ok() || n_tiles > max_tiles) return MMMOT_E_WORKSPACE;
+  MM_TRY(pn_tables(det_split, pairs, L, P, tc::BN, n_tiles, w.cnt, w.gstart, w.tiles, w.seg, w.ctab, st));
+  MM_TRY(pn_wide_stats(w, h_det_split, det_split, P, pairs, L, n_tiles, (const __half*)Xhi, K, Wt, (const uint4*)Wp, wp_scale,
+                       bias, M, addend, st));
+  MM_TRY(gn_finalize(w.stats, gamma, beta, w.cnt, 0, pairs, M, 1, sc, sh, st));
+  if (stats) MM_CUDA(cudaMemcpyAsync(stats, w.stats, (size_t)pairs * M * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  if (mom && !two_pass)
+    MM_CUDA(cudaMemcpyAsync(mom, w.mom, (size_t)pairs * (K * K + K) * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  if (detsum && K == 64 && !two_pass)
+    MM_CUDA(cudaMemcpyAsync(detsum, w.segsum, (size_t)ndet * 64 * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+  return 0;
 }
