@@ -308,6 +308,16 @@ int mmmot_set_debug(int flags);
 int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scale, const float* bias, const float* X,
                        float* Y, int M, int K, int S, int engine, void* stream);
 
+/* Test hook of the FP32 FFMA engine with its GroupNorm partials (device pointers).  mode 0: x = X, mode 1: x =
+ * relu(X*sc[g][k] + sh[g][k]) (sc, sh [groups][K]).  Y[g*y_gs + co*y_ms + col] (or NULL) = Wt^T x + bias (+ ReLU if
+ * relu), Wt [K][M] fp32, M a multiple of 64; x read at X[g*x_gs + k*x_ks + col].  Columns: uniform tiling (tile_tab
+ * NULL) `groups` groups of S columns in 128-column tiles, or tile_tab int4 [num_tiles] {group, first absolute column,
+ * length <= 128, 0} with x_gs = y_gs = 0.  part (or NULL): double2 [num_tiles][M] = (sum, sum of squares) of each
+ * tile's columns. */
+int mmmot_debug_simt(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X, long x_gs,
+                     long x_ks, const float* sc, const float* sh, int S, int groups, const void* tile_tab, int num_tiles,
+                     float* Y, long y_gs, long y_ms, void* part, void* stream);
+
 /* Test hooks of the generated-operand tensor-core engine (csrc/gemm_gen.cuh), run through the same launch code as the
  * affinity, PointNet and fusion stages.  gen: 0-2 = pairwise multiply / |minus| / minus (MMMOT_AFF_*), 3 = GroupNorm +
  * ReLU of an fp32 source (GEN_NORM), 4 = an fp32 source as it is (GEN_COPY).

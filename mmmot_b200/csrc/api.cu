@@ -195,6 +195,30 @@ extern "C" int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scal
   return gemm_simt_launch<XM_DIRECT>(p, st);
 }
 
+// One contraction of the FP32 engine (gemm_simt.cuh) with its GroupNorm partials, in the channel-major layout the
+// PointNet, affinity, fusion and w_det stages give it.  mode: XM_DIRECT or XM_NORM_RELU.
+extern "C" int mmmot_debug_simt(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X,
+                                long x_gs, long x_ks, const float* sc, const float* sh, int S, int groups,
+                                const void* tile_tab, int num_tiles, float* Y, long y_gs, long y_ms, void* part,
+                                void* stream) {
+  if (M <= 0 || K <= 0 || !Wt || !X || (mode != XM_DIRECT && mode != XM_NORM_RELU)) return MMMOT_E_ARG;
+  if (mode == XM_NORM_RELU && (!sc || !sh)) return MMMOT_E_ARG;
+  GemmP p = gemm_defaults();
+  p.Wt = Wt; p.ldw = M; p.bias = bias; p.M = M; p.K = K; p.relu = relu;
+  if (tile_tab) {
+    if (num_tiles <= 0 || x_gs || y_gs) return MMMOT_E_ARG;
+    p.tile_tab = (const int4*)tile_tab; p.num_tiles = num_tiles;
+  } else {
+    if (S <= 0 || groups <= 0) return MMMOT_E_ARG;
+    p.S = S; p.tiles_per_group = mm_cdiv(S, 128); p.num_tiles = p.tiles_per_group * groups;
+  }
+  p.X = X; p.x_gs = x_gs; p.x_ks = x_ks; p.sc = sc; p.sh = sh;
+  p.Y = Y; p.y_gs = y_gs; p.y_ms = y_ms;
+  p.part = (double2*)part;
+  cudaStream_t st = (cudaStream_t)stream;
+  return mode == XM_DIRECT ? gemm_simt_launch<XM_DIRECT>(p, st) : gemm_simt_launch<XM_NORM_RELU>(p, st);
+}
+
 // The producer variant gemm_gen_launch takes (1 = prefetching), computed on the host without any CUDA call.
 extern "C" int mmmot_debug_gen_prefetch(int gen, int m) {
   if (gen < gen::GEN_PAIR_MUL || gen > gen::GEN_COPY) return MMMOT_E_ARG;

@@ -69,6 +69,19 @@ static inline int mm_ensure_smem(K kernel, size_t bytes, std::atomic<unsigned lo
 static inline size_t mm_align(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 static inline int mm_cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 
+// GroupNorm partials of all three contraction engines.  A thread holds a run of k values of one channel in registers,
+// takes their fp32 mean pv, sums d = y - pv (s1) and d^2 (s2) in fp32 and folds the run into its fp64 (sum y, sum y^2)
+// as (k pv + s1, k pv^2 + 2 pv s1 + s2) -- a two-pass mean and variance per run, combined exactly in fp64.  The fp32
+// rounding then scales with the spread of the run, not with its mean: summing y^2 directly loses about (mean/std)^2 of
+// relative accuracy in var = sum y^2 / n - mean^2 (gn_finalize), the centred runs about mean/std, GroupNorm's own
+// conditioning (DESIGN.md §4.2).  A pivot taken from the run's values instead (say its first) is worse than no shift
+// when that value is far from the rest, as a rare positive value among ReLU zeros is.
+__device__ __forceinline__ void stat_fold(double& f1, double& f2, int k, float pv, float s1, float s2) {
+  const double p = pv, a = s1;
+  f1 += k * p + a;
+  f2 += p * (k * p + 2.0 * a) + (double)s2;
+}
+
 // Bump allocator over the caller-provided workspace.  The first MM_STATUS_BYTES of EVERY workspace are the status
 // block (word 0 = range flag, see mmmot_status_reset / mmmot_status_check): all stages carve behind it, so a flag
 // raised by one stage survives the stages that reuse the workspace after it.

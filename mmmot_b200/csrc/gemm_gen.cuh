@@ -179,7 +179,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
         const int co = mg * 128 + q * 32 + lane;
         const bool rowok = co < p.M;
         const float bv = (rowok && p.bias) ? __ldg(p.bias + co) : 0.f;
-        float f1 = 0.f, f2 = 0.f;   // (sum, sum of squares) over this thread's 128 columns: four fp32 chunk sums
+        double f1 = 0.0, f2 = 0.0;   // (sum, sum of squares) over this thread's 128 columns: four shifted chunk sums
         // channels-last: a warp's 32 consecutive channels of one column are one 128-byte line
         float* dst = p.Y + ((long)g * p.y_gs + c0 + half * 128) * p.y_ms + co;
 #pragma unroll 1
@@ -189,21 +189,25 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
           uint32_t v[32];
           acc_ld32(img, BN, q * 32 + lane, col0, v);
           if (P.t.dbg & 1) continue;
-          float s1 = 0.f, s2 = 0.f;
+          float s1 = 0.f, s2 = 0.f, pv = 0.f;
           if (col0 + 32 <= len) {
-            if (p.relu) epi_fast<true>(v, P.t.out_scale, bv, s1, s2);
-            else epi_fast<false>(v, P.t.out_scale, bv, s1, s2);
+            if (p.relu) epi_fast<true>(v, P.t.out_scale, bv, pv, s1, s2);
+            else epi_fast<false>(v, P.t.out_scale, bv, pv, s1, s2);
           } else {
+            float t = 0.f;
 #pragma unroll
             for (int j = 0; j < 32; j++) {
               float x = fmaf(__uint_as_float(v[j]), P.t.out_scale, bv);
               if (p.relu) x = fmaxf(x, 0.f);
-              if (col0 + j >= len) x = 0.f;          // columns beyond the group are not counted (and not stored)
               v[j] = __float_as_uint(x);
-              s1 += x; s2 = fmaf(x, x, s2);
+              if (col0 + j < len) t += x;            // columns beyond the group are not counted (and not stored)
             }
+            pv = t / (float)(len - col0);
+#pragma unroll
+            for (int j = 0; j < 32; j++)
+              if (col0 + j < len) { const float d = __uint_as_float(v[j]) - pv; s1 += d; s2 = fmaf(d, d, s2); }
           }
-          f1 += s1; f2 += s2;
+          stat_fold(f1, f2, min(32, len - col0), pv, s1, s2);
           if (p.Y && rowok) {
             float* d = dst + (long)cc * 32 * p.y_ms;
             if (col0 + 32 <= len) {
@@ -216,7 +220,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
             }
           }
         }
-        if (p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2((double)f1, (double)f2);
+        if (p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2(f1, f2);
       }
       fence_async_smem();   // the image's generic-proxy reads precede the next tile's operand and weight writes
       __syncwarp();

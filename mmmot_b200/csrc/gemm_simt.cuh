@@ -227,20 +227,30 @@ __global__ void __launch_bounds__(256, 2) gemm_simt_kernel(const GemmP p) {
     const int row = (i < 4) ? (ty * 4 + i) : (TM / 2 + ty * 4 + (i - 4));
     const int co = m0 + row;
     const float bv = p.bias ? __ldg(p.bias + co) : 0.f;
+    // this thread's 8 values (columns hhalf*64 + tx*4 + j), then shifted sums over the valid ones from their fp32 mean
+    // (stat_fold); columns past the group are skipped: a zero would not be neutral in the shifted sums
+    float xs[8], t = 0.f;
+    int nv = 0;
+#pragma unroll
+    for (int e = 0; e < 8; e++) {
+      float x = acc[i][e] + bv;
+      const int col = (e >> 2) * 64 + tx * 4 + (e & 3);
+      if (p.addend && col < len) x += __ldg(p.addend + (long)co * p.ld_add + __ldg(p.seg + c0 + col));
+      if (p.relu) x = fmaxf(x, 0.f);
+      xs[e] = x;
+      if (col < len) { t += x; nv++; }
+    }
+    const float pv = nv ? t / (float)nv : 0.f;
     float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; e++)
+      if ((e >> 2) * 64 + tx * 4 + (e & 3) < len) { const float d = xs[e] - pv; s1 += d; s2 = fmaf(d, d, s2); }
 #pragma unroll
     for (int hhalf = 0; hhalf < 2; hhalf++) {
       const int cb = hhalf * 64 + tx * 4;
       float v[4];
 #pragma unroll
-      for (int j = 0; j < 4; j++) {
-        float x = acc[i][hhalf * 4 + j] + bv;
-        const int col = cb + j;
-        if (p.addend && col < len) x += __ldg(p.addend + (long)co * p.ld_add + __ldg(p.seg + c0 + col));
-        if (p.relu) x = fmaxf(x, 0.f);
-        v[j] = x;
-        if (col < len) { s1 += x; s2 += x * x; }
-      }
+      for (int j = 0; j < 4; j++) v[j] = xs[hhalf * 4 + j];
       if (p.Y) {
         float* yp;
         bool vec;
@@ -272,7 +282,8 @@ __global__ void __launch_bounds__(256, 2) gemm_simt_kernel(const GemmP p) {
       }
     }
     if (p.part) {
-      double d1 = s1, d2 = s2;
+      double d1 = 0.0, d2 = 0.0;
+      stat_fold(d1, d2, nv, pv, s1, s2);
 #pragma unroll
       for (int o = 8; o >= 1; o >>= 1) {
         d1 += __shfl_xor_sync(0xffffffffu, d1, o);

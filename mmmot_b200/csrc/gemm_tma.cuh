@@ -381,7 +381,7 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
         const int co = mg * 128 + q * 32 + lane;
         const bool rowok = co < p.M;
         const float bv = (rowok && p.bias) ? __ldg(p.bias + co) : 0.f;
-        float f1 = 0.f, f2 = 0.f;   // this thread's (sum, sum of squares) over its 128 columns: four fp32 chunk sums
+        double f1 = 0.0, f2 = 0.0;   // this thread's (sum, sum of squares) over its 128 columns: four shifted chunk sums
         const bool pass2 = P.segsum && !p.part && !p.Y && !p.relu;
         // Everything the four 32-column chunks need from global memory is fetched up front, so its latency is paid once
         // per subtile instead of once (or twice, seg -> addend) per chunk: the detection index at both ends of every
@@ -412,7 +412,7 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
           uint32_t v[32];
           acc_ld32(img, BN, q * 32 + lane, col0, v);
           if (P.t.dbg & 1) continue;
-          float s1 = 0.f, s2 = 0.f;
+          float s1 = 0.f, s2 = 0.f, pv = 0.f;
           bool fast = col0 + 32 <= len;
           if (pass2 && fast) {
             // second (recomputing) pass, whole chunk inside one detection: bias, addend and the GroupNorm affine
@@ -438,9 +438,10 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
             else fast = false;
           }
           if (fast) {
-            if (p.relu) epi_fast<true>(v, P.t.out_scale, bva, s1, s2);
-            else epi_fast<false>(v, P.t.out_scale, bva, s1, s2);
+            if (p.relu) epi_fast<true>(v, P.t.out_scale, bva, pv, s1, s2);
+            else epi_fast<false>(v, P.t.out_scale, bva, pv, s1, s2);
           } else {
+            float t = 0.f;
 #pragma unroll
             for (int j = 0; j < 32; j++) {
               float x = fmaf(__uint_as_float(v[j]), P.t.out_scale, bv);
@@ -449,10 +450,14 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
                 x += __ldg(p.addend + (long)__ldg(p.seg + c0 + col) * p.ld_add + co);
               if (p.relu) x = fmaxf(x, 0.f);
               v[j] = __float_as_uint(x);
-              if (col < len) { s1 += x; s2 = fmaf(x, x, s2); }
+              if (col < len) t += x;
             }
+            pv = t / (float)min(32, len - col0);
+#pragma unroll
+            for (int j = 0; j < 32; j++)
+              if (col0 + j < len) { const float d = __uint_as_float(v[j]) - pv; s1 += d; s2 = fmaf(d, d, s2); }
           }
-          f1 += s1; f2 += s2;
+          stat_fold(f1, f2, min(32, len - col0), pv, s1, s2);
           if (P.segsum && rowok) {
             // GroupNorm + ReLU + per-detection sum fused into the (recomputing) second pass: the activation never
             // reaches HBM.  Run sums are fp32 in column order; runs are merged with integer atomics, so the result
@@ -517,7 +522,7 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
             }
           }
         }
-        if (p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2((double)f1, (double)f2);
+        if (p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2(f1, f2);
         if (P.conv && P.pool && rowok) pool_flush(co);
       }
       fence_async_smem();   // the image's generic-proxy reads precede the loader's next TMA writes
