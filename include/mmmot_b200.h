@@ -259,6 +259,34 @@ int mmmot_crop_scatter(const float* points, int n_points, int stride, const void
                        size_t workspace_bytes, void* stream);
 
 /*
+ * Per-frame LiDAR preparation of many frames in one call (SURVEY.md 8f row N1): reference
+ * point_cloud/preprocess.py:64-93 (read_and_prep_points minus the file read) — the camera field-of-view cull
+ * (box_np_ops.py:629-640) followed by each detection's region, its 3-D box or the frustum of its 2-D image box
+ * (box_np_ops.py:643-653).  Same predicate and kernels as mmmot_crop_*, always in float64.
+ *   points [frame_offsets[n_frames]][stride] (device, stride 3 or 4): the frames' scans concatenated in frame order
+ *   frame_offsets [n_frames + 1] (HOST): frame f's scan is points[frame_offsets[f] .. frame_offsets[f + 1]);
+ *                 starts at 0, non-decreasing
+ *   fov_planes [n_frames][6][4] (device, float64): each frame's field-of-view planes
+ *   det_planes [n_dets][6][4] (device, float64): each detection's region
+ *   det_frame  [n_dets] (HOST): frame of each detection; non-decreasing (detections grouped by frame, in frame order)
+ * A point belongs to detection d when it is inside its frame's field of view AND inside d's region.
+ *   mmmot_prep_count   -> split[n_dets + 1] (device) global CSR offsets; an empty detection counts one (zero) point
+ *   mmmot_prep_scatter -> out_points[split[n_dets]][out_channels] (out_channels 3..4, <= stride), scan order inside
+ *                         a detection, detections in order
+ * Both take the same arguments and the same workspace (mmmot_prep_workspace bytes, max_frame_points = the largest
+ * frame's point count); the count step's contents are consumed by scatter.  The launch count does not depend on
+ * n_frames.  MMMOT_E_ARG on bad offsets or frame indices.
+ */
+size_t mmmot_prep_workspace(int max_frame_points, int n_frames, int n_dets);
+int mmmot_prep_count(const float* points, const int* frame_offsets, int n_frames, int stride, const double* fov_planes,
+                     const double* det_planes, const int* det_frame, int n_dets, int* split, void* workspace,
+                     size_t workspace_bytes, void* stream);
+int mmmot_prep_scatter(const float* points, const int* frame_offsets, int n_frames, int stride,
+                       const double* fov_planes, const double* det_planes, const int* det_frame, int n_dets,
+                       const int* split, int out_channels, float* out_points, void* workspace,
+                       size_t workspace_bytes, void* stream);
+
+/*
  * Per-detection image crop-and-resize (SURVEY.md 8f row N2 — the image-side step right before the hot path).
  * Replaces reference dataset/test_seq_dataset.py:212-218 (PIL crop + 224x224 BILINEAR resize per detection) and
  * utils/build_util.py:137-142 (ToTensor + Normalize): image uint8 [img_h][img_w][3] (device), boxes int32

@@ -3,7 +3,7 @@ forward behind the reference's own Python surface.  See DESIGN.md."""
 from .config import build_model, model_kwargs  # noqa: F401
 from .solvers import ortools_solve, solve_batch  # noqa: F401
 from .tracking_net import TrackingNet  # noqa: F401
-from .lidar_crop import box_camera_to_lidar, box_planes, crop_points  # noqa: F401
+from .lidar_crop import box_camera_to_lidar, box_planes, crop_points, prep_points, prep_points_batch  # noqa: F401
 from .image_crop import crop_boxes, crop_resize  # noqa: F401
 from .tracking_model import TrackingModule, kitti_result_line, write_kitti_result  # noqa: F401
 from .cost import DetLoss, LinkLoss, TrackingLoss  # noqa: F401

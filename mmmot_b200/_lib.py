@@ -96,6 +96,9 @@ SIGNATURES = {
     "mmmot_crop_workspace": (_sz, [_i, _i]),
     "mmmot_crop_count": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "mmmot_crop_scatter": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "mmmot_prep_workspace": (_sz, [_i, _i, _i]),
+    "mmmot_prep_count": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _sz, _vp]),
+    "mmmot_prep_scatter": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "mmmot_crop_resize_max_taps": (_i, []),
     "mmmot_crop_resize_workspace": (_sz, [_i, _l, _i, _i]),
     "mmmot_crop_resize": (_i, [_vp, _i, _i, _vp, _vp, _i, _l, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),

@@ -60,6 +60,11 @@ boxes = np.concatenate([centers, rng.uniform([1.2, 2.5, 1.2], [2.2, 5.0, 2.0], s
 for b in (boxes.astype(np.float32), boxes.astype(np.float64)):
     out, sp = mmmot_b200.crop_points(torch.from_numpy(pc).cuda(), b)
 print("crop points", tuple(out.shape))
+from tools.prep_points_times import frame   # noqa: E402
+prep_frames = [frame(P, k, 50 + k, torch.device("cuda")) for k in (3, 1, 9)]   # several frames, image shapes, counts
+for kw in (dict(det_type="3D"), dict(use_frustum=True, without_reflectivity=True)):
+    out, sp = mmmot_b200.prep_points_batch(prep_frames, **kw)
+print("prep points", tuple(out.shape))
 img = torch.from_numpy(rng.integers(0, 256, size=(120, 200, 3), dtype=np.uint8)).cuda()
 bb = np.array([[10.2, 5.5, 80.9, 70.1], [-4.0, 30.0, 60.0, 130.0], [150.0, 20.0, 199.0, 119.0]], np.float32)
 print("crop_resize", tuple(mmmot_b200.crop_resize(img, bb, out_size=32).shape))
