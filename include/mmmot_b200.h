@@ -346,6 +346,19 @@ int mmmot_debug_simt(int mode, int M, int K, const float* Wt, const float* bias,
                      long x_ks, const float* sc, const float* sh, int S, int groups, const void* tile_tab, int num_tiles,
                      float* Y, long y_gs, long y_ms, void* part, void* stream);
 
+/* Test hook: one launch of the FP32 FFMA engine in any operand mode (device pointers), with the arguments of
+ * mmmot_debug_simt and the fields the other modes read.  mode 0 / 1 as mmmot_debug_simt; 2-4 pairwise multiply /
+ * |minus| / minus: x[k][s] = f(F[g][k][i], F[g][k][n + j]), s = i*m + j, F = X [groups][K][Lf], uniform tiling with S =
+ * n*m, Lf >= n + m, Y as mode 0; 5 3x3 / pad 1 convolution: X = in[img][Cin][H][W], K = 9*Cin, x[k][s] =
+ * im2col with k = (ky*3 + kx)*Cin + ci and s = (img, y, x), Y = out[img][M][H][W], uniform tiling with groups = 1, S =
+ * n_img*H*W, x_gs = y_gs = 0 (x_ks, y_ms unused).  addend (or NULL): Y += addend[co*ld_add + seg[c]] before the ReLU,
+ * c the column (absolute for table tiling, inside the group otherwise).  MMMOT_E_ARG, before any CUDA call, for any
+ * other combination. */
+int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X, long x_gs,
+                        long x_ks, const float* sc, const float* sh, int n, int m, int Lf, int H, int W, int Cin, int S,
+                        int groups, const void* tile_tab, int num_tiles, const float* addend, const int* seg, int ld_add,
+                        float* Y, long y_gs, long y_ms, void* part, void* stream);
+
 /* Test hooks of the generated-operand tensor-core engine (csrc/gemm_gen.cuh), run through the same launch code as the
  * affinity, PointNet and fusion stages.  gen: 0-2 = pairwise multiply / |minus| / minus (MMMOT_AFF_*), 3 = GroupNorm +
  * ReLU of an fp32 source (GEN_NORM), 4 = an fp32 source as it is (GEN_COPY).

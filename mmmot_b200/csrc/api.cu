@@ -219,6 +219,50 @@ extern "C" int mmmot_debug_simt(int mode, int M, int K, const float* Wt, const f
   return mode == XM_DIRECT ? gemm_simt_launch<XM_DIRECT>(p, st) : gemm_simt_launch<XM_NORM_RELU>(p, st);
 }
 
+// One launch of the FP32 engine in any operand mode, with every field the modes read: the pairwise generator's
+// (n, m, Lf), the 3x3 convolution's (H, W, Cin) and the per-detection addend of the epilogue.
+extern "C" int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X,
+                                   long x_gs, long x_ks, const float* sc, const float* sh, int n, int m, int Lf, int H,
+                                   int W, int Cin, int S, int groups, const void* tile_tab, int num_tiles,
+                                   const float* addend, const int* seg, int ld_add, float* Y, long y_gs, long y_ms,
+                                   void* part, void* stream) {
+  if (mode < XM_DIRECT || mode > XM_CONV3 || M <= 0 || M % 64 || K <= 0 || !Wt || !X) return MMMOT_E_ARG;
+  if (mode == XM_NORM_RELU && (!sc || !sh)) return MMMOT_E_ARG;
+  if (addend && (!seg || ld_add <= 0)) return MMMOT_E_ARG;
+  const bool pair = mode >= XM_PAIR_MUL && mode <= XM_PAIR_SUB;
+  if (tile_tab) {
+    if (num_tiles <= 0 || x_gs || y_gs || pair || mode == XM_CONV3) return MMMOT_E_ARG;
+  } else if (S <= 0 || groups <= 0) {
+    return MMMOT_E_ARG;
+  }
+  if (pair && (n <= 0 || m <= 0 || Lf < n + m || (long)n * m != S)) return MMMOT_E_ARG;
+  if (mode == XM_CONV3 && (H <= 0 || W <= 0 || Cin <= 0 || K != 9 * Cin || groups != 1 || S % ((long)H * W) ||
+                           x_gs || y_gs))
+    return MMMOT_E_ARG;
+  GemmP p = gemm_defaults();
+  p.Wt = Wt; p.ldw = M; p.bias = bias; p.M = M; p.K = K; p.relu = relu;
+  if (tile_tab) {
+    p.tile_tab = (const int4*)tile_tab; p.num_tiles = num_tiles;
+  } else {
+    p.S = S; p.tiles_per_group = mm_cdiv(S, 128); p.num_tiles = p.tiles_per_group * groups;
+  }
+  p.X = X; p.x_gs = x_gs; p.x_ks = x_ks; p.sc = sc; p.sh = sh;
+  p.n = n; p.m = m; p.Lf = Lf;
+  p.H = H; p.W = W; p.Cin = Cin;
+  p.addend = addend; p.seg = seg; p.ld_add = ld_add;
+  p.Y = Y; p.y_gs = y_gs; p.y_ms = y_ms;
+  p.part = (double2*)part;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (mode) {
+    case XM_DIRECT: return gemm_simt_launch<XM_DIRECT>(p, st);
+    case XM_NORM_RELU: return gemm_simt_launch<XM_NORM_RELU>(p, st);
+    case XM_PAIR_MUL: return gemm_simt_launch<XM_PAIR_MUL>(p, st);
+    case XM_PAIR_ABS: return gemm_simt_launch<XM_PAIR_ABS>(p, st);
+    case XM_PAIR_SUB: return gemm_simt_launch<XM_PAIR_SUB>(p, st);
+    default: return gemm_simt_launch<XM_CONV3>(p, st);
+  }
+}
+
 // The producer variant gemm_gen_launch takes (1 = prefetching), computed on the host without any CUDA call.
 extern "C" int mmmot_debug_gen_prefetch(int gen, int m) {
   if (gen < gen::GEN_PAIR_MUL || gen > gen::GEN_COPY) return MMMOT_E_ARG;

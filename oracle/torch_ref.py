@@ -61,7 +61,7 @@ def vgg_maps(sd, dets):
 def drop_block(x, block_size, drop_prob=0.1):
     """modules/dropblock.py:28-67 (DropBlock2D.forward in training): seeds from the CPU generator, max-pooled into
     blocks, inverted, rescaled by numel / sum."""
-    mask = (torch.rand(x.shape[0], *x.shape[2:]) < drop_prob / (block_size ** 2)).float()
+    mask = (torch.rand(x.shape[0], *x.shape[2:]) < drop_prob / (block_size ** 2)).float().to(x.device)
     bm = F.max_pool2d(mask[:, None], kernel_size=(block_size, block_size), stride=(1, 1), padding=block_size // 2)
     if block_size % 2 == 0:
         bm = bm[:, :, :-1, :-1]
