@@ -446,6 +446,34 @@ int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const flo
                           float wp_scale, const void* Wpx, void* Yhi, long y_plane, void* cols, int* status, int* variant,
                           void* stream);
 
+/* Test hooks of the kernels between the contractions.
+ * stage_layout: where one run of a stage leaves its intermediates in the caller's workspace, computed on the host without
+ *   any CUDA call from the same carve of the workspace the stage runs.  stage 0 = mmmot_affinity_fwd of shape
+ *   (pairs, n, m), stage 1 = mmmot_fusion_det_fwd of shape (pairs, L = n; m ignored).  offsets (host) receives byte
+ *   offsets from the start of the workspace, G = 3 pairs groups g = pair*3 + stack, NM = n*m, ldv = G*(n + m),
+ *   "TC" the tensor-core path, "FP32" the FP32-engine path:
+ *     stage 0, 16 offsets:
+ *       [0] y01   first layer [conv1.0 ; new/end conv0]: TC [g*NM + i*m + j][1024], FP32 [g][1024][NM]
+ *       [1] y3    third affinity layer: TC [g*NM + s][128], FP32 [g][128][NM]
+ *       [2] z     link logits [g][NM] (softmax_mode != NONE; with NONE they go straight to link)
+ *       [3] fcl   TC only: the feature stacks channels-last [g][n + m][512]
+ *       [4] sc0 [5] sh0   GroupNorm(1, 512) affine of new/end conv0 [g][512]
+ *       [6] sc3 [7] sh3   GroupNorm affine of the third layer [g][128]
+ *       [8] v     new/end row and column means (or maxima), column col = g*(n + m) + j (new) or + m + i (end):
+ *                 TC [col][512], FP32 [512][ldv]
+ *       [9] h2    second new/end MLP layer: TC [col][128], FP32 [128][ldv]
+ *       [10] nsc2 [11] nsh2  its GroupNorm affine [2g + (0 new | 1 end)][128]
+ *       [12] rmax [13] rsum  softmax over j per row [g][n];  [14] cmax [15] csum  over i per column [g][m]
+ *     stage 1, 2 offsets:
+ *       [0] f3    TC only: detection-major rows [(pair*L + l)*3 + stack][512]
+ *       [1] h2    second w_det layer (after its ReLU): TC [(pair*L + l)*3 + stack][256], FP32 [g][256][L]
+ *   *tensor_cores (host, or NULL) = 1 if that stage takes the tensor-core path under the current mmmot_set_engine.
+ * skip_heads: the four SkipPool heads of mmmot_appearance_fwd on pooled vectors pooledS [n_img][C_S] (C = 128, 256, 512,
+ *   512) chosen by the caller -> feats[pair][0][S*128 + t][l] for image pair*L + l; a NULL pooledS skips head S. */
+int mmmot_debug_stage_layout(int stage, int pairs, int n, int m, size_t* offsets, int* tensor_cores);
+int mmmot_debug_skip_heads(const mmmot_weights* wts, const float* pooled0, const float* pooled1, const float* pooled2,
+                           const float* pooled3, int n_img, int L, float* feats, void* stream);
+
 /* Per-launch timing of the hot kernels with CUDA events on the launching stream; used by bench.py's roofline
  * figures.  Every timed launch carries a tag = (stage, layer) — mmmot_timing_tag_count() tags, named by
  * mmmot_timing_tag_name() — and its ALGORITHMIC work (FLOPs; compulsory HBM bytes of that launch).

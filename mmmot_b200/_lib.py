@@ -80,6 +80,8 @@ SIGNATURES = {
                                         _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "mmmot_debug_pn_stats": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                   _sz, _vp]),
+    "mmmot_debug_stage_layout": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz), ctypes.POINTER(_i)]),
+    "mmmot_debug_skip_heads": (_i, [_wp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     "mmmot_timing_collect": (_i, [ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_long)]),
     "mmmot_appearance_workspace": (_sz, [_i, _i, _i]),
     "mmmot_appearance_fwd": (_i, [_wp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),

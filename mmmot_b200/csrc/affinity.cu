@@ -289,6 +289,10 @@ AfWs carve(MmArena& a, int pairs, int n, int m) {
   return w;
 }
 
+// engine choice from the per-pair shape only (see appearance.cu); a quarter-filled 256-column tile on the tensor cores
+// still beats the FP32 engine (N = 8: 31k -> see DESIGN §6)
+bool affinity_use_tc(int n, int m) { return mm_engine() == 2 || (mm_engine() == 0 && n * m >= 64); }
+
 template <int GEN>
 int launch_gen(const GemmP& p, const mmmot_weights* wts, int wid, const float* src, int src_m, const float* gsc,
                const float* gsh, int n, int m, int Lf, cudaStream_t st) {
@@ -301,6 +305,17 @@ extern "C" size_t mmmot_affinity_workspace(int pairs, int n, int m) {
   MmArena a(nullptr, 0);
   carve(a, pairs, n, m);
   return a.off;
+}
+
+// mmmot_debug_stage_layout, stage 0: where mmmot_affinity_fwd leaves its intermediates (a dry carve; no CUDA call)
+int mm_affinity_layout(int pairs, int n, int m, size_t* off, int* tensor_cores) {
+  MmArena a(nullptr, 0);
+  const AfWs w = carve(a, pairs, n, m);
+  const void* const bufs[16] = {w.y01, w.y3, w.z, w.fcl, w.sc0, w.sh0, w.sc3, w.sh3,
+                                w.v, w.h2, w.nsc2, w.nsh2, w.rmax, w.rsum, w.cmax, w.csum};
+  for (int i = 0; i < 16; i++) off[i] = (size_t)reinterpret_cast<uintptr_t>(bufs[i]);
+  if (tensor_cores) *tensor_cores = affinity_use_tc(n, m) ? 1 : 0;
+  return 0;
 }
 
 extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs,
@@ -316,8 +331,7 @@ extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int
   AfWs w = carve(ar, pairs, n, m);
   if (!ar.ok()) return MMMOT_E_WORKSPACE;
   const int G = pairs * 3, NM = n * m, L = n + m;
-  const bool use_tc = mm_engine() == 2 || (mm_engine() == 0 && NM >= 64);   // per-pair shape only (see appearance.cu); a
-  // quarter-filled 256-column tile on the tensor cores still beats the FP32 engine (N = 8: 31k -> see DESIGN §6)
+  const bool use_tc = affinity_use_tc(n, m);
   const int tpg = mm_cdiv(NM, use_tc ? tc::BN : 128);
   const float* const* W = wts->w;
   const bool timed = mm_timing_on();

@@ -450,9 +450,11 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
   return mm_launch_skip_heads(wts, pooled, n_img, L, feats, st);
 }
 
-// the four SkipPool heads on the pooled maps -> stack 0 of feats (shared with the training-mode variant, train.cu)
+// the four SkipPool heads on the pooled maps -> stack 0 of feats (shared with the training-mode variant, train.cu); a NULL
+// map skips its head (mmmot_debug_skip_heads)
 int mm_launch_skip_heads(const mmmot_weights* wts, float* const* pooled, int n_img, int L, float* feats, cudaStream_t st) {
   for (int s = 0; s < 4; s++) {
+    if (!pooled[s]) continue;
     const float* const* q = &wts->w[MMMOT_W_SKIP0 + 10 * s];
     int C = kSkipC[s], mid = C / 4 > 64 ? C / 4 : 64;
     skip_head_kernel<<<n_img, 128, 0, st>>>(pooled[s], q[0], q[1], q[2], q[3], q[4], q[5], q[6], q[7],
@@ -460,4 +462,14 @@ int mm_launch_skip_heads(const mmmot_weights* wts, float* const* pooled, int n_i
     MM_LAUNCH_CHECK();
   }
   return 0;
+}
+
+// Test hook: the SkipPool heads on pooled vectors the caller chooses, through mm_launch_skip_heads.
+extern "C" int mmmot_debug_skip_heads(const mmmot_weights* wts, const float* pooled0, const float* pooled1,
+                                      const float* pooled2, const float* pooled3, int n_img, int L, float* feats,
+                                      void* stream) {
+  if (!wts || !feats || n_img <= 0 || L <= 0 || n_img % L) return MMMOT_E_ARG;
+  float* const pooled[4] = {const_cast<float*>(pooled0), const_cast<float*>(pooled1), const_cast<float*>(pooled2),
+                            const_cast<float*>(pooled3)};
+  return mm_launch_skip_heads(wts, pooled, n_img, L, feats, (cudaStream_t)stream);
 }

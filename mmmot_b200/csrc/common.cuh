@@ -89,13 +89,13 @@ constexpr size_t MM_STATUS_BYTES = 256;
 struct MmArena {
   char* base;
   size_t cap, off;
-  bool dry;  // dry run: only measure
+  bool dry;  // dry run: only measure; take() returns the byte offset itself (mmmot_debug_stage_layout reads a carve that way)
   MmArena(void* p, size_t c) : base((char*)p), cap(c), off(MM_STATUS_BYTES), dry(p == nullptr) {}
   int* status() const { return dry ? nullptr : reinterpret_cast<int*>(base); }
   template <typename T>
   T* take(size_t n) {
     size_t bytes = mm_align(n * sizeof(T));
-    char* r = dry ? nullptr : base + off;
+    char* r = dry ? reinterpret_cast<char*>(static_cast<uintptr_t>(off)) : base + off;
     off += bytes;
     return (T*)r;
   }

@@ -142,12 +142,25 @@ FdWs carve(MmArena& a, int pairs, int L) {
   return w;
 }
 
+// engine choice from the per-pair shape only (see appearance.cu)
+bool fusion_det_use_tc(int L) { return mm_engine() == 2 || (mm_engine() == 0 && L >= 64); }
+
 }  // namespace
 
 extern "C" size_t mmmot_fusion_det_workspace(int pairs, int L) {
   MmArena a(nullptr, 0);
   carve(a, pairs, L);
   return a.off;
+}
+
+// mmmot_debug_stage_layout, stage 1: where mmmot_fusion_det_fwd leaves F3 and h2 (a dry carve; no CUDA call)
+int mm_fusion_det_layout(int pairs, int L, size_t* off, int* tensor_cores) {
+  MmArena a(nullptr, 0);
+  const FdWs w = carve(a, pairs, L);
+  off[0] = (size_t)reinterpret_cast<uintptr_t>(w.f3);
+  off[1] = (size_t)reinterpret_cast<uintptr_t>(w.h2);
+  if (tensor_cores) *tensor_cores = fusion_det_use_tc(L) ? 1 : 0;
+  return 0;
 }
 
 extern "C" int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold,
@@ -161,8 +174,7 @@ extern "C" int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, i
   if (!ar.ok()) return MMMOT_E_WORKSPACE;
   const long fs = 3L * 512 * L;  // floats per pair in feats
 
-  // engine choice from the per-pair shape only (see appearance.cu)
-  if (mm_engine() == 2 || (mm_engine() == 0 && L >= 64)) {
+  if (fusion_det_use_tc(L)) {
     // ---------------- tensor-core path: every contraction on the generated-operand engine (GEN_COPY) over
     // detection-major channels-last rows F3[(pair*L + l)*3 + stack][512]
     const int tpg2 = mm_cdiv(L, tc::BN);

@@ -148,7 +148,8 @@ def test_features_match_oracle(fusion, op, sm, engine):
 
 
 @pytest.mark.parametrize("n,m", [(8, 8), (32, 32), (64, 64), (20, 45), (128, 128)])
-@pytest.mark.parametrize("op,sm", [("multiply", "none"), ("minus_abs", "dual_add")])
+@pytest.mark.parametrize("op,sm", [("multiply", "none"), ("minus_abs", "dual_add"), ("minus", "single"), ("multiply", "dual"),
+                                   ("minus_abs", "dual_max")])
 def test_affinity_stage_matches_oracle(n, m, op, sm, engine):
     """BASELINE config 5 (N sweep): affinity + start/end + softmax alone on identical feature tensors."""
     net, sd = make_net("C", op, sm, 0.2, 7)
