@@ -449,7 +449,8 @@ int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const flo
 /* Test hooks of the kernels between the contractions.
  * stage_layout: where one run of a stage leaves its intermediates in the caller's workspace, computed on the host without
  *   any CUDA call from the same carve of the workspace the stage runs.  stage 0 = mmmot_affinity_fwd of shape
- *   (pairs, n, m), stage 1 = mmmot_fusion_det_fwd of shape (pairs, L = n; m ignored).  offsets (host) receives byte
+ *   (pairs, n, m), stage 1 = mmmot_fusion_det_fwd of shape (pairs, L = n; m ignored), stage 2 = mmmot_pointnet_fwd of
+ *   shape (pairs, L = n, P = m points in all).  offsets (host) receives byte
  *   offsets from the start of the workspace, G = 3 pairs groups g = pair*3 + stack, NM = n*m, ldv = G*(n + m),
  *   "TC" the tensor-core path, "FP32" the FP32-engine path:
  *     stage 0, 16 offsets:
@@ -467,6 +468,28 @@ int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const flo
  *     stage 1, 2 offsets:
  *       [0] f3    TC only: detection-major rows [(pair*L + l)*3 + stack][512]
  *       [1] h2    second w_det layer (after its ReLU): TC [(pair*L + l)*3 + stack][256], FP32 [g][256][L]
+ *     stage 2, 27 offsets (carve order; ndet = pairs*L detections, d = pair*L + l; a buffer a path does not use has
+ *     size 0 there; sc / sh / stats / part are reused layer after layer and end as conv2's):
+ *       [0] xt    FP32: the points channel-major [3][P]
+ *       [1] y1    FP32: layer 1 (3 -> 64, before its GroupNorm) [64][P]
+ *       [2] t0    TC: layer 4 [P][128];  FP32: layer 4 [128][P]
+ *       [3] t1    TC: layer 3 [P][64];   FP32: layer 3 [64][P]
+ *       [4] big   FP32: [1024][P], layer 5, whose first 512 rows the head (64 -> 512 + U addend, before its GroupNorm)
+ *                 then overwrites
+ *       [5] segsum  TC: 2^-32 fixed-point per-detection sums, u64; at the end the head's [ndet][512]
+ *       [6] x1p   TC: relu(GN(layer 1)) as FP16 planes [2][P][64] (hi, lo)
+ *       [7] xp    TC: relu(GN(layer 4)) as FP16 planes [2][P][128]
+ *       [8] gmean per-detection mean of relu(GN(layer 5)): TC [ndet][1024], FP32 [1024][ndet]
+ *       [9] u     FP32: U = Wh[:, 64:] gmean [512][ndet]     [10] ut  TC: U [ndet][512]
+ *       [11] hmean  per-detection mean of relu(GN(head)): TC [ndet][512], FP32 [512][ndet]
+ *       [12] o    conv2 (512 -> 512, before its GroupNorm): TC [ndet][512], FP32 [512][ndet]
+ *       [13] sc1 [14] sh1   FP32: layer 1's GroupNorm affine [pairs][64]
+ *       [15] sc [16] sh     [pairs][1024]; at the end the first [pairs][512] hold conv2's GroupNorm(16, 512) affine
+ *       [17] stats          [pairs][1024][2] fp64; at the end the first [pairs][512][2] hold conv2's (sum, sum of squares)
+ *       [18] mom  [19] part  moments / partials scratch   [20] gstart [pairs + 1]   [21] sstart (TC) [pairs + 1]
+ *       [22] seg [P] detection of each point   [23] cnt [pairs] points per pair
+ *       [24] tiles int4 {pair, first point, length, 0} (256-point tiles on TC, 128 on FP32)   [25] ctab (TC) int4
+ *       [26] end  = mmmot_pointnet_workspace(pairs, L, P)
  *   *tensor_cores (host, or NULL) = 1 if that stage takes the tensor-core path under the current mmmot_set_engine.
  * skip_heads: the four SkipPool heads of mmmot_appearance_fwd on pooled vectors pooledS [n_img][C_S] (C = 128, 256, 512,
  *   512) chosen by the caller -> feats[pair][0][S*128 + t][l] for image pair*L + l; a NULL pooledS skips head S. */

@@ -361,13 +361,16 @@ extern "C" int mmmot_debug_conv_layer(const void* Wp, const void* Wpx, float wp_
 }
 
 // ---------------------------------------------------------------------------------------------
-// Where the affinity (stage 0) and fusion / detection-score (stage 1) stages leave their intermediates, on the host.
+// Where the affinity (stage 0), fusion / detection-score (stage 1) and PointNet (stage 2) stages leave their
+// intermediates, on the host.
 int mm_affinity_layout(int pairs, int n, int m, size_t* off, int* tensor_cores);
 int mm_fusion_det_layout(int pairs, int L, size_t* off, int* tensor_cores);
+int mm_pointnet_layout(int pairs, int L, long P, size_t* off, int* tensor_cores);
 
 extern "C" int mmmot_debug_stage_layout(int stage, int pairs, int n, int m, size_t* offsets, int* tensor_cores) {
   if (!offsets || pairs <= 0 || n <= 0) return MMMOT_E_ARG;
   if (stage == 0) return m <= 0 ? MMMOT_E_ARG : mm_affinity_layout(pairs, n, m, offsets, tensor_cores);
   if (stage == 1) return mm_fusion_det_layout(pairs, n, offsets, tensor_cores);
+  if (stage == 2) return m <= 0 ? MMMOT_E_ARG : mm_pointnet_layout(pairs, n, m, offsets, tensor_cores);
   return MMMOT_E_ARG;
 }

@@ -468,12 +468,13 @@ struct PnWs {
   int4 *tiles, *ctab;
 };
 
-// use_tc: the tensor-core path never materialises the 1024-wide activation (537 MB per frame-pair at cfg4)
+// use_tc: the tensor-core path never materialises the 1024-wide activation (537 MB per frame-pair at cfg4), reads the
+// points row-major (no xt), never stores layer 1 in fp32 (no y1) and keeps U channels-last (ut; the FP32 path: u)
 PnWs carve(MmArena& a, int pairs, int L, long P, long max_tiles, bool use_tc) {
   PnWs w;
   long nd = (long)pairs * L;
-  w.xt = a.take<float>(3 * P);
-  w.y1 = a.take<float>(64 * P);
+  w.xt = a.take<float>(use_tc ? 0 : 3 * P);
+  w.y1 = a.take<float>(use_tc ? 0 : 64 * P);
   w.t0 = a.take<float>(128 * P);
   w.t1 = a.take<float>(64 * P);
   w.big = a.take<float>(use_tc ? 0 : 1024 * P);
@@ -481,8 +482,8 @@ PnWs carve(MmArena& a, int pairs, int L, long P, long max_tiles, bool use_tc) {
   w.x1p = a.take<__half>(2 * 64 * P);
   w.xp = a.take<__half>(2 * 128 * P);
   w.gmean = a.take<float>(1024 * nd);
-  w.u = a.take<float>(512 * nd);
-  w.ut = a.take<float>(512 * nd);
+  w.u = a.take<float>(use_tc ? 0 : 512 * nd);
+  w.ut = a.take<float>(use_tc ? 512 * nd : 0);
   w.hmean = a.take<float>(512 * nd);
   w.o = a.take<float>(512 * nd);
   w.sc1 = a.take<float>((size_t)pairs * 64);
@@ -609,6 +610,20 @@ extern "C" size_t mmmot_pointnet_train_workspace(int pairs, int L, long p_total)
   return a.off;
 }
 
+// mmmot_debug_stage_layout, stage 2: where mmmot_pointnet_fwd leaves its intermediates (a dry carve; no CUDA call)
+int mm_pointnet_layout(int pairs, int L, long P, size_t* off, int* tensor_cores) {
+  MmArena a(nullptr, 0);
+  const bool use_tc = pointnet_use_tc(L);
+  const PnWs w = carve(a, pairs, L, P, P / 128 + 2 * pairs + 2, use_tc);
+  const void* const bufs[26] = {w.xt, w.y1, w.t0, w.t1, w.big, w.segsum, w.x1p, w.xp, w.gmean, w.u, w.ut, w.hmean, w.o,
+                                w.sc1, w.sh1, w.sc, w.sh, w.stats, w.mom, w.part, w.gstart, w.sstart, w.seg, w.cnt,
+                                w.tiles, w.ctab};
+  for (int i = 0; i < 26; i++) off[i] = (size_t)reinterpret_cast<uintptr_t>(bufs[i]);
+  off[26] = a.off;
+  if (tensor_cores) *tensor_cores = use_tc ? 1 : 0;
+  return 0;
+}
+
 // train: FP32 engine; head_mask (optional) = the Dropout mask of the head activation, [512][P] with values {0, 1/(1-p)}
 static int pointnet_impl(const mmmot_weights* wts, const float* points, const int* det_split, const int* h_det_split,
                          int pairs, int L, float* feats, void* workspace, size_t workspace_bytes, void* stream, bool train,
@@ -647,8 +662,6 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
   MmArena ar(workspace, workspace_bytes);
   PnWs w = carve(ar, pairs, L, P, max_tiles, use_tc);
   if (!ar.ok() || n_tiles > max_tiles) return MMMOT_E_WORKSPACE;
-  transpose_points_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(points, w.xt, P);
-  MM_LAUNCH_CHECK();
   MM_TRY(pn_tables(det_split, pairs, L, P, TNW, n_tiles, w.cnt, w.gstart, w.tiles, w.seg, use_tc ? w.ctab : nullptr, st));
 
   const int cin[5] = {3, 64, 64, 64, 128}, cout[5] = {64, 64, 64, 128, 1024};
@@ -657,7 +670,7 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
     // ---------------- tensor-core path: channels-last activations ----------------
     // layer i writes fp32 Y[p][cout] + GroupNorm partials; norm_split turns it into the packed FP16
     // operand of layer i+1.  y1's packed form (x1p) is kept for the head.
-    float* ybuf[5] = {w.y1, w.t0, w.t1, w.t0, nullptr};
+    float* ybuf[5] = {nullptr, w.t0, w.t1, w.t0, nullptr};   // layer 1 is recomputed, never stored
     const bool gen_mid = !(mm_debug_flags() & 8192);   // debug bit 13: layers 3, 4 through norm_split + the TMA-fed kernel
     for (int i = 0; i < 5; i++) {
       const float* const* q = &wts->w[MMMOT_W_PN_L1 + 4 * i];
@@ -765,6 +778,8 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
       return 0;
     }
   } else {
+  transpose_points_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(points, w.xt, P);
+  MM_LAUNCH_CHECK();
   // trunk: 3 -> 64 -> 64 -> 64 -> 128 -> 1024, each conv + GroupNorm(C,C) over the pair's points + ReLU
   const float* src[5] = {w.xt, w.y1, w.t0, w.t1, w.t0};
   float* dst[5] = {w.y1, w.t0, w.t1, w.t0, w.big};

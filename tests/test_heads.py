@@ -279,7 +279,7 @@ def test_stage_layout_without_device():
     finally:
         lib.mmmot_set_engine(0)
     off = (ctypes.c_size_t * 16)()
-    for args in ((2, 1, 4, 4), (0, 0, 4, 4), (0, 1, 0, 4), (0, 1, 4, 0), (1, 1, 0, 0), (-1, 1, 4, 4)):
+    for args in ((3, 1, 4, 4), (0, 0, 4, 4), (0, 1, 0, 4), (0, 1, 4, 0), (1, 1, 0, 0), (-1, 1, 4, 4)):
         assert lib.mmmot_debug_stage_layout(*args, off, None) == -1, args
     assert lib.mmmot_debug_stage_layout(0, 1, 4, 4, None, None) == -1
     # the SkipPool hook checks its shape before any CUDA call: images must fill whole pairs
