@@ -331,29 +331,17 @@ int mmmot_set_kseg(int chunks);
  *   bit 14 (16384) first VGG layer with a separate im2col pre-pass instead of in-kernel operand producers */
 int mmmot_set_debug(int flags);
 
-/* Test hook: Y[M][S] = W X + bias through the FP32 FFMA engine (engine must be 1); Wt is [K][M] fp32, X is [K][S],
- * all device pointers (Wp / wp_scale are ignored; the tensor-core engines have the planar / gen hooks below). */
-int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scale, const float* bias, const float* X,
-                       float* Y, int M, int K, int S, int engine, void* stream);
-
-/* Test hook of the FP32 FFMA engine with its GroupNorm partials (device pointers).  mode 0: x = X, mode 1: x =
- * relu(X*sc[g][k] + sh[g][k]) (sc, sh [groups][K]).  Y[g*y_gs + co*y_ms + col] (or NULL) = Wt^T x + bias (+ ReLU if
- * relu), Wt [K][M] fp32, M a multiple of 64; x read at X[g*x_gs + k*x_ks + col].  Columns: uniform tiling (tile_tab
- * NULL) `groups` groups of S columns in 128-column tiles, or tile_tab int4 [num_tiles] {group, first absolute column,
- * length <= 128, 0} with x_gs = y_gs = 0.  part (or NULL): double2 [num_tiles][M] = (sum, sum of squares) of each
- * tile's columns. */
-int mmmot_debug_simt(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X, long x_gs,
-                     long x_ks, const float* sc, const float* sh, int S, int groups, const void* tile_tab, int num_tiles,
-                     float* Y, long y_gs, long y_ms, void* part, void* stream);
-
-/* Test hook: one launch of the FP32 FFMA engine in any operand mode (device pointers), with the arguments of
- * mmmot_debug_simt and the fields the other modes read.  mode 0 / 1 as mmmot_debug_simt; 2-4 pairwise multiply /
- * |minus| / minus: x[k][s] = f(F[g][k][i], F[g][k][n + j]), s = i*m + j, F = X [groups][K][Lf], uniform tiling with S =
- * n*m, Lf >= n + m, Y as mode 0; 5 3x3 / pad 1 convolution: X = in[img][Cin][H][W], K = 9*Cin, x[k][s] =
- * im2col with k = (ky*3 + kx)*Cin + ci and s = (img, y, x), Y = out[img][M][H][W], uniform tiling with groups = 1, S =
- * n_img*H*W, x_gs = y_gs = 0 (x_ks, y_ms unused).  addend (or NULL): Y += addend[co*ld_add + seg[c]] before the ReLU,
- * c the column (absolute for table tiling, inside the group otherwise).  MMMOT_E_ARG, before any CUDA call, for any
- * other combination. */
+/* Test hook: one launch of the FP32 FFMA engine in any operand mode, with its GroupNorm partials (device pointers).
+ * mode 0: x = X, mode 1: x = relu(X*sc[g][k] + sh[g][k]) (sc, sh [groups][K]).  Y[g*y_gs + co*y_ms + col] (or NULL) =
+ * Wt^T x + bias (+ ReLU if relu), Wt [K][M] fp32, M a multiple of 64; x read at X[g*x_gs + k*x_ks + col].  Columns:
+ * uniform tiling (tile_tab NULL) `groups` groups of S columns in 128-column tiles, or tile_tab int4 [num_tiles] {group,
+ * first absolute column, length <= 128, 0} with x_gs = y_gs = 0.  part (or NULL): double2 [num_tiles][M] = (sum, sum of
+ * squares) of each tile's columns.  mode 2-4 pairwise multiply / |minus| / minus: x[k][s] = f(F[g][k][i],
+ * F[g][k][n + j]), s = i*m + j, F = X [groups][K][Lf], uniform tiling with S = n*m, Lf >= n + m, Y as mode 0; mode 5
+ * 3x3 / pad 1 convolution: X = in[img][Cin][H][W], K = 9*Cin, x[k][s] = im2col with k = (ky*3 + kx)*Cin + ci and s =
+ * (img, y, x), Y = out[img][M][H][W], uniform tiling with groups = 1, S = n_img*H*W, x_gs = y_gs = 0 (x_ks, y_ms
+ * unused).  addend (or NULL): Y += addend[co*ld_add + seg[c]] before the ReLU, c the column (absolute for table
+ * tiling, inside the group otherwise).  MMMOT_E_ARG, before any CUDA call, for any other combination. */
 int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X, long x_gs,
                         long x_ks, const float* sc, const float* sh, int n, int m, int Lf, int H, int W, int Cin, int S,
                         int groups, const void* tile_tab, int num_tiles, const float* addend, const int* seg, int ld_add,
@@ -413,14 +401,10 @@ int mmmot_debug_pn_stats(const int* det_split, const int* h_det_split, int pairs
                          const float* gamma, const float* beta, float* sc, float* sh, double* stats, double* mom,
                          unsigned long long* detsum, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Test hooks of the TMA-fed tensor-core engine: operands are two FP16 planes (hi, lo), channels-last.
- * linear: Y[rows][M] fp32 = X W^T + bias, X planes [2][rows][K].  conv: 3x3 pad 1 + bias + ReLU on NHWC planes
- * [2][n][H][W][C] -> [2][n][H][W][M] (weights packed with K order (ky*3+kx)*C + ci). */
+/* Test hook of the TMA-fed tensor-core engine in matrix mode on uniform tiling: Y[rows][M] fp32 (channels-last) =
+ * X W^T + bias, X two FP16 planes (hi, lo) [2][rows][K]. */
 int mmmot_debug_linear_planar(const void* Wp, float wp_scale, const float* bias, const void* Xhi, float* Y,
                               int M, int K, long rows, void* stream);
-int mmmot_debug_conv_planar(const void* Wp, float wp_scale, const float* bias, const void* Xhi, void* Yhi,
-                            int n_img, int H, int W, int C, int M, float* kseg_scratch /* fp32 [n*H*W][M] or NULL */,
-                            void* stream);
 
 /* Test hooks of the VGG trunk's convolutions, run through the same launch code as mmmot_appearance_fwd.
  * conv_plan: the launch plan of one 3x3 conv layer (n_img x H x W, C -> M channels), computed on the host without any

@@ -55,12 +55,9 @@ SIGNATURES = {
     "mmmot_set_engine": (_i, [_i]),
     "mmmot_set_debug": (_i, [_i]),
     "mmmot_set_kseg": (_i, [_i]),
-    "mmmot_debug_linear": (_i, [_vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
-    "mmmot_debug_simt": (_i, [_i, _i, _i, _vp, _vp, _i, _vp, _l, _l, _vp, _vp, _i, _i, _vp, _i, _vp, _l, _l, _vp, _vp]),
     "mmmot_debug_simt_op": (_i, [_i, _i, _i, _vp, _vp, _i, _vp, _l, _l, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i,
                                  _vp, _vp, _i, _vp, _l, _l, _vp, _vp]),
     "mmmot_debug_linear_planar": (_i, [_vp, _f, _vp, _vp, _vp, _i, _i, _l, _vp]),
-    "mmmot_debug_conv_planar": (_i, [_vp, _f, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "mmmot_debug_conv_plan": (_i, [_i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(_i)]),
     "mmmot_debug_conv_layer": (_i, [_vp, _vp, _f, _vp, _vp, _l, _i, _i, _i, _i, _i, _vp, _l, _l, ctypes.POINTER(_i), _vp, _vp,
                                     _vp, ctypes.POINTER(_i), _vp]),

@@ -181,46 +181,9 @@ extern "C" int mmmot_set_engine(int engine) {
   return 0;
 }
 
-extern "C" int mmmot_debug_linear(const float* Wt, const void* Wp, float wp_scale, const float* bias, const float* X,
-                                  float* Y, int M, int K, int S, int engine, void* stream) {
-  (void)Wp; (void)wp_scale;
-  if (!Wt || !X || !Y || M <= 0 || K <= 0 || S <= 0 || engine != 1) return MMMOT_E_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  GemmP p = gemm_defaults();
-  p.Wt = Wt; p.ldw = M; p.bias = bias; p.M = M; p.K = K;
-  p.S = S;
-  p.X = X; p.x_ks = S;
-  p.Y = Y; p.y_ms = S;
-  p.tiles_per_group = mm_cdiv(S, 128); p.num_tiles = p.tiles_per_group;
-  return gemm_simt_launch<XM_DIRECT>(p, st);
-}
-
-// One contraction of the FP32 engine (gemm_simt.cuh) with its GroupNorm partials, in the channel-major layout the
-// PointNet, affinity, fusion and w_det stages give it.  mode: XM_DIRECT or XM_NORM_RELU.
-extern "C" int mmmot_debug_simt(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X,
-                                long x_gs, long x_ks, const float* sc, const float* sh, int S, int groups,
-                                const void* tile_tab, int num_tiles, float* Y, long y_gs, long y_ms, void* part,
-                                void* stream) {
-  if (M <= 0 || K <= 0 || !Wt || !X || (mode != XM_DIRECT && mode != XM_NORM_RELU)) return MMMOT_E_ARG;
-  if (mode == XM_NORM_RELU && (!sc || !sh)) return MMMOT_E_ARG;
-  GemmP p = gemm_defaults();
-  p.Wt = Wt; p.ldw = M; p.bias = bias; p.M = M; p.K = K; p.relu = relu;
-  if (tile_tab) {
-    if (num_tiles <= 0 || x_gs || y_gs) return MMMOT_E_ARG;
-    p.tile_tab = (const int4*)tile_tab; p.num_tiles = num_tiles;
-  } else {
-    if (S <= 0 || groups <= 0) return MMMOT_E_ARG;
-    p.S = S; p.tiles_per_group = mm_cdiv(S, 128); p.num_tiles = p.tiles_per_group * groups;
-  }
-  p.X = X; p.x_gs = x_gs; p.x_ks = x_ks; p.sc = sc; p.sh = sh;
-  p.Y = Y; p.y_gs = y_gs; p.y_ms = y_ms;
-  p.part = (double2*)part;
-  cudaStream_t st = (cudaStream_t)stream;
-  return mode == XM_DIRECT ? gemm_simt_launch<XM_DIRECT>(p, st) : gemm_simt_launch<XM_NORM_RELU>(p, st);
-}
-
-// One launch of the FP32 engine in any operand mode, with every field the modes read: the pairwise generator's
-// (n, m, Lf), the 3x3 convolution's (H, W, Cin) and the per-detection addend of the epilogue.
+// One launch of the FP32 engine (gemm_simt.cuh) in any operand mode, with its GroupNorm partials, in the channel-major
+// layout the PointNet, affinity, fusion and w_det stages give it, and every field the modes read: the pairwise
+// generator's (n, m, Lf), the 3x3 convolution's (H, W, Cin) and the per-detection addend of the epilogue.
 extern "C" int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, const float* bias, int relu, const float* X,
                                    long x_gs, long x_ks, const float* sc, const float* sh, int n, int m, int Lf, int H,
                                    int W, int Cin, int S, int groups, const void* tile_tab, int num_tiles,
@@ -318,16 +281,6 @@ extern "C" int mmmot_debug_linear_planar(const void* Wp, float wp_scale, const f
   p.Y = Y; p.y_ms = M;
   return gemm_tma_launch_mat(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, rows * (long)K, rows, K, tc::OUT_CL, 0,
                              (cudaStream_t)stream);
-}
-
-// 3x3 conv + bias + ReLU on planar FP16 NHWC: X planes [2][n][H][W][C] -> Y planes [2][n][H][W][M]
-extern "C" int mmmot_debug_conv_planar(const void* Wp, float wp_scale, const float* bias, const void* Xhi, void* Yhi,
-                                       int n_img, int H, int W, int C, int M, float* kseg_scratch, void* stream) {
-  if (!Wp || !Xhi || !Yhi) return MMMOT_E_ARG;
-  GemmP p = gemm_defaults();
-  p.bias = bias; p.M = M; p.relu = 1;
-  return gemm_tma_launch_conv(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, (long)n_img * H * W * C, n_img, H, W, C,
-                              (__half*)Yhi, (long)n_img * H * W * M, (cudaStream_t)stream, kseg_scratch);
 }
 
 static void conv_plan_words(const ConvPlan& c, int* plan) {

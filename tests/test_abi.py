@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import mmmot_b200
+from kernel_kit import lib_state
 from mmmot_b200 import _lib
 from mmmot_b200.schema import state_schema
 from mmmot_b200.synthetic import synthetic_batch, synthetic_pair, synthetic_state_dict
@@ -42,11 +43,8 @@ def test_workspace_queries_need_no_gpu(lib_built):
     # tensor-core path (L >= 16): fp32 trunk activations + FP16 hi/lo planes, but never the 1024-wide layer
     tc_ws = lib.mmmot_pointnet_workspace(1, 16, 4096)
     assert (64 + 128 + 64) * 4096 * 4 < tc_ws < 1024 * 4096 * 4
-    lib.mmmot_set_engine(1)                              # FP32 engine materialises it
-    try:
+    with lib_state(lib, engine="fp32"):                 # FP32 engine materialises it
         assert lib.mmmot_pointnet_workspace(1, 16, 4096) > 1024 * 4096 * 4
-    finally:
-        lib.mmmot_set_engine(0)
     assert lib.mmmot_fusion_det_workspace(2, 16) > 0 and lib.mmmot_lp_workspace(4, 8, 8) > 0
     # argument validation happens before any CUDA call
     assert lib.mmmot_lp_assign(None, 0, None, 0, None, 0, None, 0, 1, 1, 1, None, None, None, None, None, None, 0, None) == -1

@@ -5,7 +5,8 @@ The end-to-end tests see the trunk only through SkipPool's global averages, whic
 pixel of a partial box or image slab, a misplaced pooled pixel or a missing lo term.  These tests run one layer through
 the product's own launch code (mmmot_debug_conv_layer / mmmot_debug_vgg_conv0) and bound every output element by
 
-    |y - y_ref| <= TAU * S,   S = conv2d(|X|, |W|) + |b|   (max-pooled like y for pooled outputs),
+    |y - y_ref| <= TAU * S,   S = conv2d(|X|, |W|) + |b|   (max-pooled like y for pooled outputs; TAU = 2^-18, see
+                                                            kernel_kit.TAU),
 
 the forward-error form of a dot product: meaningful at ReLU zeros and cancellations, where a bound relative to |y| is
 not.  X is exactly what the kernel reads (hi + lo of the input planes, or the fp32 crops), W the fp32 weights handed
@@ -24,21 +25,17 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from kernel_kit import KSEG_DEFAULT, TAU, bench_n_imgs, fp16_split, lib_state, vp
 from mmmot_b200 import _lib
 from mmmot_b200.schema import VGG_STAGES
 from mmmot_b200.weights import pack_px, pack_tc
 
-# TAU = 2^-18: with the fp32 accumulator truncating at every K=16 step, about 216 roundings per 36-chunk K segment
-# with random-sign partial sums give ~1e-6 S at K = 4608.  Measured on an H100 80GB HBM3 (400 W power limit): the worst
-# err / (TAU S) over all cases is 0.51 (K = 4608 in one pass, test_kseg_record); 0.28 over the product's plans.
-TAU = 2.0 ** -18
 NAN16 = 0x7E00
 GUARD = 4096                       # guard band (elements) after every output plane
-KSEG_DEFAULT = 36                  # mmmot_set_kseg default (api.cu)
 PLAN_KEYS = ("px", "halo", "pool", "bx", "by", "bi", "ksegs", "tiles")
+SMS = 132                          # H100 SXM: the persistent grid of the channel-major kernel is min(units, SMs)
 
 gpu = pytest.mark.gpu
-vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
 # ------------------------------------------------------------------------------------------------ case table
@@ -55,6 +52,25 @@ def _partial_y(p):
 
 def _partial_slab(p):
     return p["bi"] > 1 and p["n"] % p["bi"] != 0
+
+
+def half_dim(p):
+    """The box dimension that separates a tile's two 128-column halves (columns (ii*by + yy)*bx + xx): the outermost
+    one larger than 1."""
+    return "bi" if p["bi"] > 1 else "by" if p["by"] > 1 else "bx"
+
+
+def empty_halves(p):
+    """Column tiles of a conv plan whose half 1 lies wholly outside the image."""
+    d = half_dim(p)
+    lim = {"bi": p["n"], "by": p["H"], "bx": p["W"]}[d]
+    count = {"bi": math.ceil(p["n"] / p["bi"]), "by": math.ceil(p["H"] / p["by"]), "bx": math.ceil(p["W"] / p["bx"])}[d]
+    others = p["tiles"] // count
+    return others * sum(1 for k in range(count) if k * p[d] + p[d] // 2 >= lim)
+
+
+def units(p, M):
+    return p["tiles"] * math.ceil(M / 128)
 
 
 CASES = [
@@ -110,6 +126,34 @@ CASES = [
     # K segmentation: many middle segments (kseg 8 on K = 1152: five segments)
     ("cm_kseg8_pool", 128, 128, 8, 8, 4, 0, 8, True, False,
      lambda p: not p["px"] and p["pool"] and p["ksegs"] == 5),
+    # The edges of the channel-major kernel's work schedule: the persistent grid of min(units, SMs) CTAs walks
+    # (column tile, M group) units, each in K segments, and consumer warpgroup h takes column half h of every tile.
+    # One 16 x 16 box: a single unit, halves split along the box rows, fused pool
+    ("one_tile_pool", 64, 128, 16, 16, 1, 0, None, True, False,
+     lambda p: not p["px"] and p["tiles"] == 1 and half_dim(p) == "by" and p["pool"]),
+    # 49 boxes x 3 M groups = 147 units on 132 CTAs: odd, not a multiple of the grid
+    ("odd_units_147", 32, 384, 112, 112, 1, 0, None, False, False,
+     lambda p: not p["px"] and units(p, 384) == 147 and p["ksegs"] == 1),
+    # 3 boxes (odd) and 2, 3, 4, 5 K segments per half, fused pool
+    ("kseg2_tiles3", 128, 128, 16, 16, 3, 0, 18, True, False,
+     lambda p: not p["px"] and p["tiles"] == 3 and p["ksegs"] == 2 and p["pool"] and half_dim(p) == "by"),
+    ("kseg3_tiles3", 128, 128, 16, 16, 3, 0, 12, True, False,
+     lambda p: not p["px"] and p["tiles"] == 3 and p["ksegs"] == 3 and p["pool"]),
+    ("kseg4_tiles3", 128, 128, 16, 16, 3, 0, 9, True, False,
+     lambda p: not p["px"] and p["tiles"] == 3 and p["ksegs"] == 4 and p["pool"]),
+    ("kseg5_tiles3", 128, 128, 16, 16, 3, 0, 8, True, False,
+     lambda p: not p["px"] and p["tiles"] == 3 and p["ksegs"] == 5 and p["pool"]),
+    # halves split along the image slab (8 x 8 x 4 box): 5 images leave the second box's half 1 (images 6, 7) empty
+    ("slab_half_empty_pool", 64, 128, 8, 8, 5, 0, None, True, False,
+     lambda p: not p["px"] and half_dim(p) == "bi" and p["pool"] and empty_halves(p) == 1),
+    ("slab_half_empty_pool_kseg3", 64, 128, 8, 8, 5, 0, 8, True, False,
+     lambda p: not p["px"] and half_dim(p) == "bi" and p["pool"] and p["ksegs"] == 3 and empty_halves(p) == 1),
+    # halves split along the box width (256 x 1 x 1 box on one-row images); 300 columns leave the second box's half 1
+    # empty
+    ("width_half_256", 32, 128, 1, 256, 2, 0, None, False, False,
+     lambda p: not p["px"] and half_dim(p) == "bx" and p["tiles"] == 2 and empty_halves(p) == 0),
+    ("width_half_empty_300", 32, 128, 1, 300, 1, 0, None, False, False,
+     lambda p: not p["px"] and half_dim(p) == "bx" and p["tiles"] == 2 and empty_halves(p) == 1),
 ]
 CASE_IDS = [c[0] for c in CASES]
 
@@ -133,33 +177,7 @@ def plan_class(p):
     return (p["px"], p["halo"], p["pool"], p["bx"] if p["pool"] and not p["px"] else 0, min(p["ksegs"], 3), p["bi"] > 1)
 
 
-class _State:
-    """Sets debug bits / kseg for one case and restores the defaults whatever happens."""
-
-    def __init__(self, lib, dbg=0, kseg=None):
-        self.lib, self.dbg, self.kseg = lib, dbg, kseg
-
-    def __enter__(self):
-        self.lib.mmmot_set_debug(self.dbg)
-        self.lib.mmmot_set_kseg(KSEG_DEFAULT if self.kseg is None else self.kseg)
-        return self
-
-    def __exit__(self, *exc):
-        self.lib.mmmot_set_debug(0)
-        self.lib.mmmot_set_kseg(KSEG_DEFAULT)
-        self.lib.mmmot_set_engine(0)
-
-
 # ------------------------------------------------------------------------------------------------ helpers
-def _split(x):
-    hi = x.half()
-    return hi, (x - hi.float()).half()
-
-
-def _planes(hi, lo):
-    return torch.stack([hi, lo]).contiguous()
-
-
 def _weights(g, M, C, scale=1.0):
     w = torch.randn(M, C, 3, 3, generator=g) * (2.0 / (9 * C)) ** 0.5 * scale
     b = torch.randn(M, generator=g) * 0.1 * scale
@@ -240,7 +258,7 @@ class ConvRun:
         full, pooled = n * H * W * M, n * (H // 2) * (W // 2) * M
         self.y_plane, self.p_plane = full + GUARD, pooled + GUARD
         self.Y = _out_buffer(self.y_plane)
-        X = _planes(x_hi, x_lo).cuda()
+        X = torch.stack([x_hi, x_lo]).contiguous().cuda()
         self.Wp_d, self.Wpx_d, self.b_d = Wp.cuda(), None if Wpx is None else Wpx.cuda(), b.cuda()
         self.status = torch.zeros(1, dtype=torch.int32, device="cuda")
         self.psum = None
@@ -281,7 +299,7 @@ class ConvRun:
 def _case_inputs(g, n, H, W, C, M):
     w, b = _weights(g, M, C)
     x = torch.randn(n, H, W, C, generator=g)
-    x_hi, x_lo = _split(x)
+    x_hi, x_lo = fp16_split(x)
     return w, b, x_hi, x_lo
 
 
@@ -309,7 +327,7 @@ def test_conv_layer_vs_fp64(case):
     g = torch.Generator().manual_seed(sum(map(ord, name)))
     w, b, x_hi, x_lo = _case_inputs(g, n, H, W, C, M)
     _, Wp, Wpx, wps = _packed(w, compact)
-    with _State(lib, dbg, kseg):
+    with lib_state(lib, dbg=dbg, kseg=kseg):
         r = ConvRun(lib, Wp, Wpx, wps, b, x_hi, x_lo, n, H, W, C, M, want_pool)
     assert check(r.plan), (name, r.plan)
     x = (x_hi.double() + x_lo.double()).permute(0, 3, 1, 2)
@@ -344,9 +362,9 @@ def test_fused_pool_matches_unfused(C, M, H, W, n):
     g = torch.Generator().manual_seed(C + M + H + n)
     w, b, x_hi, x_lo = _case_inputs(g, n, H, W, C, M)
     _, Wp, Wpx, wps = _packed(w, True)
-    with _State(lib, 0):
+    with lib_state(lib):
         fused = ConvRun(lib, Wp, Wpx, wps, b, x_hi, x_lo, n, H, W, C, M, True)
-    with _State(lib, 512):
+    with lib_state(lib, dbg=512):
         unf = ConvRun(lib, Wp, Wpx, wps, b, x_hi, x_lo, n, H, W, C, M, True)
     assert fused.did_pool and not unf.did_pool
     yf = fused.output().permute(0, 2, 3, 1)
@@ -377,7 +395,7 @@ def test_conv_split_terms_alone(kind):
     w_hi, w_lo = _w_terms(wt)
     to_nchw = lambda t: t.permute(0, 3, 1, 2)
     wk = lambda t: t.reshape(3, 3, C, M).permute(3, 2, 0, 1)           # Wt layout -> [M][C][3][3]
-    with _State(lib, 0):
+    with lib_state(lib):
         # (0, r): only Xlo * Whi contributes
         r = torch.randn(n, H, W, C, generator=g).half()
         run = ConvRun(lib, Wp, Wpx, wps, b, torch.zeros_like(r), r, n, H, W, C, M, False)
@@ -404,12 +422,12 @@ def test_matrix_split_terms_alone():
     Wp, wps = pack_tc(wt)
     w_hi, w_lo = _w_terms(wt)
     b = torch.zeros(M, device="cuda")
-    x_hi, x_lo = _split(torch.randn(rows, K, generator=g))
+    x_hi, x_lo = fp16_split(torch.randn(rows, K, generator=g))
     r = torch.randn(rows, K, generator=g).half() * 2.0 ** -11
     ratios = []
     for (xh, xl, Wpk, x_ref, w_ref) in ((torch.zeros_like(r), r, Wp, r, w_hi),
                                          (x_hi, x_lo, _zero_hi_tiles(Wp, M, K), x_hi, w_lo)):
-        X = _planes(xh, xl).cuda()
+        X = torch.stack([xh, xl]).contiguous().cuda()
         Y = torch.full((rows, M), float("nan"), device="cuda")
         assert lib.mmmot_debug_linear_planar(vp(Wpk.cuda()), wps, vp(b), vp(X), vp(Y), M, K, rows, None) == 0
         torch.cuda.synchronize()
@@ -434,7 +452,7 @@ def test_kseg_record(C, H, W, n):
     ref, S = _conv_ref(x, w.double(), b.double(), False)
     out = {}
     for kseg in (0, KSEG_DEFAULT):
-        with _State(lib, 0, kseg):
+        with lib_state(lib, dbg=0, kseg=kseg):
             r = ConvRun(lib, Wp, None, wps, b, x_hi, x_lo, n, H, W, C, M, False)
         y = r.output()
         nz = ref > 0
@@ -463,7 +481,7 @@ def test_conv_range_flag(C, M, H, W, n, dbg, kseg):
         ws, bs = (w * f).float(), (b * f).float()
         _, Wp, Wpx, wps = _packed(ws, True)
         want_pool = kseg is not None
-        with _State(lib, dbg, kseg):
+        with lib_state(lib, dbg=dbg, kseg=kseg):
             r = ConvRun(lib, Wp, Wpx, wps, bs, x_hi, x_lo, n, H, W, C, M, want_pool)
         top = float(_conv_ref(x, ws.double(), bs.double(), False)[0].max())
         assert (top >= 65504.0) == bool(flagged) and top < 65504 * 1.2
@@ -497,7 +515,7 @@ def _run_conv0(lib, x, w, b, dbg, w_packed=None, wpx=None):
     variant = ctypes.c_int(-1)
     xd = x.contiguous().cuda()
     keep = [t.cuda() for t in (wt_ffma, b, Wp, Wpx)]
-    with _State(lib, dbg):
+    with lib_state(lib, dbg=dbg):
         rc = lib.mmmot_debug_vgg_conv0(vp(xd), n, H, W, vp(keep[0]), vp(keep[1]), vp(keep[2]), wps, vp(keep[3]), vp(Y), plane,
                                        vp(cols), vp(status), ctypes.byref(variant), None)
         torch.cuda.synchronize()
@@ -618,7 +636,7 @@ def test_conv_plans_well_formed(lib_built, dbg, kseg):
     """Every plan over the VGG layers at crop sizes 32..224 and odd image counts is well formed, and its box has the
     least padding waste of all candidates (the pixel-major kernel may take 16 x 16 x 1 when it wastes no more)."""
     lib = _lib.load()
-    with _State(lib, dbg, kseg):
+    with lib_state(lib, dbg=dbg, kseg=kseg):
         for hw in (32, 64, 96, 224):
             for C, M, H, W, pool in _vgg_layers(hw) + [(64, 64, 24, 40, False), (512, 512, 2, 2, True)]:
                 for n in (1, 3, 6, 17, 64, 256):
@@ -653,24 +671,10 @@ def test_case_table_takes_named_paths(lib_built):
     """Each GPU case's plan, computed on the host, is the path the case is named after."""
     lib = _lib.load()
     for name, C, M, H, W, n, dbg, kseg, want_pool, _, check in CASES:
-        with _State(lib, dbg, kseg):
+        with lib_state(lib, dbg=dbg, kseg=kseg):
             p = _plan(lib, n, H, W, C, M, want_pool)
         assert check(p), (name, p)
-
-
-def _bench_n_imgs(pairs, L):
-    """Image counts forward_batch can launch for `pairs` frame-pairs of L detections: its chunk size halves from the
-    whole batch until the workspace fits the free memory, so every size of that chain (and its remainder) can occur."""
-    sizes, c = {pairs}, pairs
-    while c > 1:
-        c = (c + 1) // 2
-        sizes.add(c)
-    chunks = set()
-    for c in sizes:
-        chunks.add(c)
-        if pairs % c:
-            chunks.add(pairs % c)
-    return sorted(k * L for k in chunks)
+    assert 147 % SMS and 147 % 2
 
 
 def test_gpu_cases_cover_bench_plans(lib_built):
@@ -680,14 +684,14 @@ def test_gpu_cases_cover_bench_plans(lib_built):
     lib = _lib.load()
     covered = set()
     for name, C, M, H, W, n, dbg, kseg, want_pool, _, _ in CASES:
-        with _State(lib, dbg, kseg):
+        with lib_state(lib, dbg=dbg, kseg=kseg):
             covered.add(plan_class(_plan(lib, n, H, W, C, M, want_pool)))
     missing = {}
-    with _State(lib, 0):
+    with lib_state(lib):
         for cfg in ("cfg2", "cfg3", "cfg4"):
             c = bench.CONFIGS[cfg]
             assert c["hw"] == 64
-            for n_img in _bench_n_imgs(c["pairs"], 2 * c["n"]):
+            for n_img in bench_n_imgs(c["pairs"], 2 * c["n"]):
                 for C, M, H, W, pool in _vgg_layers(c["hw"]):
                     k = plan_class(_plan(lib, n_img, H, W, C, M, pool))
                     if k not in covered:

@@ -2,8 +2,8 @@
 stage each chunk's sources in shared memory by TMA: the [128 detections x 32 channels] fp32 box (128-byte swizzle) and
 the tile's two object rows.
 
-GPU cases use the fp64 element-wise harness of test_gen_engines.py (|y - y_ref| <= 2^-18 S, partials to their stated
-tolerance, NaN-filled outputs with guard rows) at the edges of the staging: a last tile of one object row (its second
+GPU cases use the fp64 element-wise harness of the generated-operand tests (kernel_kit.run_gen: |y - y_ref| <= 2^-18 S,
+partials to their stated tolerance, NaN-filled outputs with guard rows) at the edges of the staging: a last tile of one object row (its second
 row is the group's first detection row, masked), many groups (the detection box never starts at row 0), a stack whose
 G * Lf rows end exactly at the last box, one- and two-chunk K (fewer chunks than the source look-ahead), and enough
 tiles per CTA that the ring wraps many times.  The staged and the plain producers (debug bit 10) must give bit-identical
@@ -17,10 +17,8 @@ import re
 import pytest
 import torch
 
+from kernel_kit import GEN, Cols, check_part, check_rows, gen_weights, lib_state, ref_linear, report, run_gen
 from mmmot_b200 import _lib
-from test_conv_engines import _State
-from test_gen_engines import (ABS, COPY, GEN_NAMES, MUL, NORM, SUB, Cols, _report, _weights, check_part, check_rows,
-                              ref_linear, run_gen)
 
 gpu = pytest.mark.gpu
 PLAIN = 1024                       # mmmot_set_debug bit 10: producers without the pipeline (no staging)
@@ -30,13 +28,13 @@ PTXAS_LOG = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file_
 # (n, G, M, K): n object rows against m = 128 detections, G groups (feature stacks of Lf = n + 128 rows)
 STAGE_SHAPES = [(128, 3, 1024, 512), (127, 4, 1024, 512), (1, 6, 1024, 512), (128, 12, 1024, 512), (3, 40, 1024, 512),
                 (64, 5, 256, 32), (65, 2, 128, 64)]
-STAGE_CASES = [(op,) + s for op in (MUL, ABS, SUB) for s in STAGE_SHAPES]
+STAGE_CASES = [(op,) + s for op in (GEN.MUL, GEN.ABS, GEN.SUB) for s in STAGE_SHAPES]
 
 
 def _pair_inputs(op, n, G, K, seed):
     g = torch.Generator().manual_seed(seed)
-    F = torch.randn(G, n + 128, K, generator=g) * (1.0 if op == MUL else 2.0)
-    if op == MUL:
+    F = torch.randn(G, n + 128, K, generator=g) * (1.0 if op == GEN.MUL else 2.0)
+    if op == GEN.MUL:
         hot = torch.randint(0, K, (min(16, K),), generator=g)
         F[:, :, hot] = torch.sign(torch.randn(G, n + 128, hot.numel(), generator=g)) * 255.8
     return g, F
@@ -44,7 +42,7 @@ def _pair_inputs(op, n, G, K, seed):
 
 def _run(lib, op, n, G, M, K, seed, dbg=0):
     g, F = _pair_inputs(op, n, G, K, seed)
-    wt, b, Wp, wps = _weights(g, K, M)
+    wt, b, Wp, wps = gen_weights(g, K, M)
     NM, gap = n * 128, 5
     cols = Cols.uniform(NM, G, 0, NM + gap)
     Fd = F.cuda().contiguous()      # exactly G * Lf rows: the last detection box ends at the end of the tensor
@@ -55,34 +53,34 @@ def _run(lib, op, n, G, M, K, seed, dbg=0):
 
 @gpu
 @pytest.mark.parametrize("op,n,G,M,K", STAGE_CASES,
-                         ids=[f"{GEN_NAMES[c[0]]}-n{c[1]}-G{c[2]}-M{c[3]}-K{c[4]}" for c in STAGE_CASES])
+                         ids=[f"{GEN.NAMES[c[0]]}-n{c[1]}-G{c[2]}-M{c[3]}-K{c[4]}" for c in STAGE_CASES])
 def test_staged_pairwise_vs_fp64(op, n, G, M, K):
     lib = _lib.load()
-    with _State(lib, 0):
+    with lib_state(lib):
         assert lib.mmmot_debug_gen_staged(op, 128) == 1
     Fd, wt, b, cols, Y, P, pref = _run(lib, op, n, G, M, K, seed=op * 1000 + n * 7 + G * 13 + K)
     assert pref == 1
     F64 = Fd.double()
     a, d = F64[:, :n, None, :], F64[:, None, n:, :]
-    if op == MUL:
+    if op == GEN.MUL:
         X, A = a * d, a.abs() * d.abs()
     else:
-        X = (a - d).abs() / 2 if op == ABS else (a - d) / 2
+        X = (a - d).abs() / 2 if op == GEN.ABS else (a - d) / 2
         A = (a.abs() + d.abs()) / 2
     ref, S = ref_linear(X.reshape(-1, K), A.reshape(-1, K), wt, b)
     del X, A
     r = check_rows(Y, cols, ref, S)
     rp = check_part(P, cols, ref, S)
-    _report(f"staged pair {GEN_NAMES[op]} n={n} G={G} M={M} K={K}", err_over_bound=r, part_err_over_tol=rp)
+    report(f"staged pair {GEN.NAMES[op]} n={n} G={G} M={M} K={K}", err_over_bound=r, part_err_over_tol=rp)
     assert r <= 1.0
 
 
-BITWISE_CASES = [(op, 127, 4, 1024, 512) for op in (MUL, ABS, SUB)] + [(MUL, 1, 9, 256, 64)]
+BITWISE_CASES = [(op, 127, 4, 1024, 512) for op in (GEN.MUL, GEN.ABS, GEN.SUB)] + [(GEN.MUL, 1, 9, 256, 64)]
 
 
 @gpu
 @pytest.mark.parametrize("op,n,G,M,K", BITWISE_CASES,
-                         ids=[f"{GEN_NAMES[c[0]]}-n{c[1]}-G{c[2]}-M{c[3]}-K{c[4]}" for c in BITWISE_CASES])
+                         ids=[f"{GEN.NAMES[c[0]]}-n{c[1]}-G{c[2]}-M{c[3]}-K{c[4]}" for c in BITWISE_CASES])
 def test_staged_equals_plain_bitwise(op, n, G, M, K):
     """The staged producers and the plain ones (bit 10) on the same launch: Y and the partials agree bit for bit."""
     lib = _lib.load()
@@ -98,16 +96,16 @@ def test_gen_staged_query(lib_built):
     """gen_staged through the library, no GPU: only the pairwise producers at m == 128, never with bit 10."""
     lib = _lib.load()
     ms = (1, 64, 127, 128, 129, 256)
-    with _State(lib, 0):
-        assert [lib.mmmot_debug_gen_staged(op, m) for op in (MUL, ABS, SUB) for m in ms] == [0, 0, 0, 1, 0, 0] * 3
-        assert all(lib.mmmot_debug_gen_staged(gn, m) == 0 for gn in (NORM, COPY) for m in ms)
+    with lib_state(lib):
+        assert [lib.mmmot_debug_gen_staged(op, m) for op in (GEN.MUL, GEN.ABS, GEN.SUB) for m in ms] == [0, 0, 0, 1, 0, 0] * 3
+        assert all(lib.mmmot_debug_gen_staged(gn, m) == 0 for gn in (GEN.NORM, GEN.COPY) for m in ms)
         assert lib.mmmot_debug_gen_staged(5, 128) == -1 and lib.mmmot_debug_gen_staged(-1, 128) == -1
         # the staged path is the pipelined one at exactly those shapes
-        assert all(lib.mmmot_debug_gen_prefetch(op, 128) == 1 for op in (MUL, ABS, SUB))
-    with _State(lib, 4096):
-        assert [lib.mmmot_debug_gen_staged(op, m) for op in (MUL, ABS, SUB) for m in ms] == [0, 0, 0, 1, 0, 0] * 3
+        assert all(lib.mmmot_debug_gen_prefetch(op, 128) == 1 for op in (GEN.MUL, GEN.ABS, GEN.SUB))
+    with lib_state(lib, dbg=4096):
+        assert [lib.mmmot_debug_gen_staged(op, m) for op in (GEN.MUL, GEN.ABS, GEN.SUB) for m in ms] == [0, 0, 0, 1, 0, 0] * 3
     for dbg in (PLAIN, PLAIN | 4096):
-        with _State(lib, dbg):
+        with lib_state(lib, dbg=dbg):
             assert all(lib.mmmot_debug_gen_staged(gn, m) == 0 for gn in range(5) for m in ms)
 
 

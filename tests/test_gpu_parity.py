@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from helpers import TOL, case_tol, check_close, det_close, frac_outside, golden_cases, relerr
+from kernel_kit import XM, eval_net, fp16_planes, vp
 import mmmot_b200
 from mmmot_b200.synthetic import synthetic_batch, synthetic_pair, synthetic_state_dict
 from oracle import lp_ref, torch_ref
@@ -18,11 +19,7 @@ ELEM_OUTSIDE = 1e-3
 
 
 def make_net(fusion, op, sm, thr, seed):
-    net = mmmot_b200.TrackingNet(2, appear_skippool=True, score_arch="branch_cls", score_fusion_arch=fusion,
-                                 affinity_op=op, softmax_mode=sm, neg_threshold=thr, test_mode=2, dropblock=0)
-    sd = synthetic_state_dict(fusion, seed=seed)
-    net.load_state_dict(sd)
-    return net.cuda().eval(), sd
+    return eval_net(fusion, seed, affinity_op=op, softmax_mode=sm, neg_threshold=thr)
 
 
 @pytest.fixture(params=["fp32", "tcgen05"])
@@ -33,34 +30,27 @@ def engine(request):
     mmmot_b200.set_engine("auto")
 
 
-def _planes(x):
-    """fp32 -> FP16 (hi, lo) planes stacked on a new leading axis (the tensor-core engines' operand format)."""
-    hi = x.half()
-    return torch.stack([hi, (x - hi.float()).half()]).contiguous()
-
-
 @pytest.mark.parametrize("M,K,S", [(128, 32, 256), (256, 96, 512), (64, 64, 300), (512, 512, 4099), (1024, 128, 1000),
                                    (128, 4608, 2048)])
 def test_contraction_engines_vs_fp64(M, K, S):
     """Each contraction engine alone (C ABI test hooks) against an fp64 matmul: the FP32 FFMA engine and the TMA-fed
     tensor-core engine (FP16 hi/lo planes in, fp32 out).  The generated-operand engine has its own element-wise tests
     (test_gen_engines.py)."""
-    import ctypes
     from mmmot_b200 import _lib
     from mmmot_b200.weights import pack_tc
     lib = _lib.load()
     g = torch.Generator().manual_seed(M + K + S)
     Wt, X, b = torch.randn(K, M, generator=g), torch.randn(K, S, generator=g), torch.randn(M, generator=g)
     ref = Wt.double().t() @ X.double() + b.double()[:, None]
-    vp = lambda t: ctypes.c_void_p(t.data_ptr())
     Wt_d, X_d, b_d = Wt.cuda(), X.cuda(), b.cuda()
     Wp, wps = pack_tc(Wt)
     Wp = Wp.cuda()
     Y = torch.full((M, S), float("nan"), device="cuda")
-    assert lib.mmmot_debug_linear(vp(Wt_d), None, 0.0, vp(b_d), vp(X_d), vp(Y), M, K, S, 1, None) == 0
+    assert lib.mmmot_debug_simt_op(XM.DIRECT, M, K, vp(Wt_d), vp(b_d), 0, vp(X_d), 0, S, None, None, 0, 0, 0, 0, 0, 0, S, 1,
+                                   None, 0, None, None, 0, vp(Y), 0, S, None, None) == 0
     assert relerr(Y, ref) < 3e-5, "fp32 engine"
     # TMA-fed engine: X as channels-last planes [2][S][K], Y [S][M]
-    Xp = _planes(X.t().contiguous()).cuda()
+    Xp = fp16_planes(X.t().contiguous()).cuda()
     Y2 = torch.full((S, M), float("nan"), device="cuda")
     assert lib.mmmot_debug_linear_planar(vp(Wp), wps, vp(b_d), vp(Xp), vp(Y2), M, K, S, None) == 0
     assert relerr(Y2.t(), ref) < 3e-5, "tma engine"

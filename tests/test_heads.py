@@ -66,23 +66,13 @@ import math
 import pytest
 import torch
 
-import mmmot_b200
+from kernel_kit import (AF_BUFS, ENGINE, EPS, TINY, U, Workspace, assert_written, case_seed, eval_net, lib_state,
+                        nan_output, nan_workspace, norm_operand, report, stage_layout, vp, worst_ratio)
 from mmmot_b200 import _lib
 from mmmot_b200.synthetic import synthetic_state_dict
-from test_gen_engines import _report
-from test_norm_stats import _seed
-from test_simt_engine import worst_ratio
 
 gpu = pytest.mark.gpu
-vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-U = 2.0 ** -24
-TINY = 2.0 ** -126
 FLOOR = 4 * TINY
-EPS = 1e-5
-GUARD = 256
-AF_BUFS = ("y01", "y3", "z", "fcl", "sc0", "sh0", "sc3", "sh3", "v", "h2", "nsc2", "nsh2", "rmax", "rsum", "cmax", "csum")
-FD_BUFS = ("f3", "h2")
-ENGINE = {"auto": 0, "fp32": 1, "tc": 2}
 MODES = ("none", "single", "dual", "dual_add", "dual_max")
 OPS = ("multiply", "minus_abs", "minus")
 SKIP_C = (128, 256, 512, 512)
@@ -92,15 +82,6 @@ CFG_N = {"cfg2": 32, "cfg3": 64, "cfg4": 128, "cfg5": 256}
 
 
 # ------------------------------------------------------------------------------------------------ layout
-def stage_layout(lib, stage, pairs, n, m=0):
-    """mmmot_debug_stage_layout -> ({buffer: byte offset}, tensor-core path?)."""
-    off = (ctypes.c_size_t * 16)()
-    tc = ctypes.c_int(-1)
-    assert lib.mmmot_debug_stage_layout(stage, pairs, n, m, off, ctypes.byref(tc)) == 0
-    names = AF_BUFS if stage == 0 else FD_BUFS
-    return {k: int(off[i]) for i, k in enumerate(names)}, bool(tc.value)
-
-
 def af_sizes(pairs, n, m):
     """Floats in each affinity intermediate (the shapes the header documents)."""
     G, NM, ldv = 3 * pairs, n * m, 3 * pairs * (n + m)
@@ -113,16 +94,7 @@ def fd_sizes(pairs, L):
     return dict(f3=3 * pairs * 512 * L, h2=3 * pairs * 256 * L)
 
 
-def ws_view(ws, off, count):
-    return ws[off:off + 4 * count].view(torch.float32)
-
-
 # ------------------------------------------------------------------------------------------------ fp64 bounds
-def norm_relu(y, sc, sh):
-    """relu(fmaf(y, sc, sh)) in fp32, as fp64."""
-    return (y.double() * sc.double() + sh.double()).float().clamp_min(0).double()
-
-
 def mean_bound(r, cnt, mx):
     """New/end reduction of the fp32 values r (fp64, the reduced axis last) -> (V_ref, bound)."""
     if mx:
@@ -265,9 +237,8 @@ def test_stage_layout_without_device():
     """mmmot_debug_stage_layout works on the host: every buffer lies inside the stage's workspace, behind the status
     block, and no two overlap; the path it reports follows the engine setting; bad arguments are refused."""
     lib = _lib.load()
-    try:
-        for engine in ("auto", "fp32", "tc"):
-            assert lib.mmmot_set_engine(ENGINE[engine]) == 0
+    for engine in ("auto", "fp32", "tc"):
+        with lib_state(lib, engine=engine):
             for pairs, n, m in ((1, 1, 1), (2, 7, 9), (2, 8, 8), (3, 37, 29), (1, 257, 40), (1, 256, 256)):
                 lay, tc = stage_layout(lib, 0, pairs, n, m)
                 assert tc == (af_path(n, m, engine) == "tc"), (engine, n, m)
@@ -276,8 +247,6 @@ def test_stage_layout_without_device():
                 lay, tc = stage_layout(lib, 1, pairs, L)
                 assert tc == (det_path(L, engine) == "tc"), (engine, L)
                 _disjoint_inside(lay, fd_sizes(pairs, L), int(lib.mmmot_fusion_det_workspace(pairs, L)))
-    finally:
-        lib.mmmot_set_engine(0)
     off = (ctypes.c_size_t * 16)()
     for args in ((3, 1, 4, 4), (0, 0, 4, 4), (0, 1, 0, 4), (0, 1, 4, 0), (1, 1, 0, 0), (-1, 1, 4, 4)):
         assert lib.mmmot_debug_stage_layout(*args, off, None) == -1, args
@@ -358,7 +327,7 @@ def test_bounds_reject_planted_defects():
         worst_ok = max(worst_ok, worst_ratio(o32, ref, T))
         worst_bad = min(worst_bad, worst_ratio(bad, ref, T))
     out["skip fp32"], out["skip var / (C-1)"] = worst_ok, worst_bad
-    _report("planted defects (err / bound)", **out)
+    report("planted defects (err / bound)", **out)
     assert max(out["mean fp32"], out["rsum fp32"], out["logit fp32"], out["skip fp32"]) <= 1.0, out
     assert min(out["mean / m"], out["rsum short"], out["logit no bias"]) > 10.0, out
     # the head's bound compounds |W| through two contractions and three GroupNorms (about 1e3 times the fp32 error), and
@@ -367,32 +336,14 @@ def test_bounds_reject_planted_defects():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
+def _peaky(sd):
+    for k in ("w_link.conv1.9.weight", "w_link.conv1.9.bias"):
+        sd[k] = sd[k] * PEAKY
+
+
 @functools.lru_cache(maxsize=None)
 def _net(fusion, peaky=False):
-    sd = synthetic_state_dict(fusion, seed=29)
-    if peaky:
-        for k in ("w_link.conv1.9.weight", "w_link.conv1.9.bias"):
-            sd[k] = sd[k] * PEAKY
-    net = mmmot_b200.TrackingNet(2, appear_skippool=True, score_arch="branch_cls", score_fusion_arch=fusion, test_mode=2,
-                                 dropblock=0)
-    net.load_state_dict(sd)
-    net.cuda().eval()
-    return net, sd
-
-
-def _nan(count):
-    return torch.full((count + GUARD,), float("nan"), device="cuda")
-
-
-def _written(buf, count, what):
-    assert bool(torch.isfinite(buf[:count]).all()), f"{what}: an owned element was not written"
-    assert bool(torch.isnan(buf[count:]).all()), f"{what}: written past its end"
-
-
-def _workspace(lib, nbytes):
-    ws = torch.full((nbytes,), 255, dtype=torch.uint8, device="cuda")      # every float / double of it NaN
-    assert lib.mmmot_status_reset(vp(ws), None) == 0
-    return ws
+    return eval_net(fusion, 29, edit=_peaky if peaky else None)
 
 
 @gpu
@@ -403,25 +354,23 @@ def test_affinity_tail_vs_fp64(n, m, pairs, engine, op, sm, end, peaky):
     net, sd = _net("C", peaky)
     wts = net.prepared()
     G, NM, L = 3 * pairs, n * m, n + m
-    g = torch.Generator().manual_seed(_seed("affinity tail", n, m, pairs, engine, op, sm, end, peaky))
+    g = torch.Generator().manual_seed(case_seed("affinity tail", n, m, pairs, engine, op, sm, end, peaky))
     feats = torch.relu(torch.randn(pairs, 3, 512, L, generator=g)).cuda()
-    link, new, end_s = _nan(G * NM), _nan(G * m), _nan(G * n)
-    assert lib.mmmot_set_engine(ENGINE[engine]) == 0
-    try:
+    link, new, end_s = nan_output(G * NM), nan_output(G * m), nan_output(G * n)
+    with lib_state(lib, engine=engine):
         lay, tc = stage_layout(lib, 0, pairs, n, m)
         assert tc == (af_path(n, m, engine) == "tc")
-        ws = _workspace(lib, int(lib.mmmot_affinity_workspace(pairs, n, m)))
+        ws = nan_workspace(lib, int(lib.mmmot_affinity_workspace(pairs, n, m)))
         rc = lib.mmmot_affinity_fwd(wts.ptr, _lib.AFFINITY[op], _lib.SOFTMAX[sm], _lib.END_MODE[end], pairs, n, m, vp(feats),
                                     vp(link), vp(new), vp(end_s), vp(ws), ws.numel(), None)
         torch.cuda.synchronize()
-    finally:
-        lib.mmmot_set_engine(0)
     assert rc == 0, rc
     assert lib.mmmot_status_check(vp(ws), None) == 0
     for buf, cnt, what in ((link, G * NM, "link"), (new, G * m, "new"), (end_s, G * n, "end")):
-        _written(buf, cnt, what)
+        assert_written(buf, cnt, what)
     size = af_sizes(pairs, n, m)
-    B = {k: ws_view(ws, lay[k], size[k]) for k in AF_BUFS}
+    wsv = Workspace(ws, lay)
+    B = {k: wsv.view(k, size[k]) for k in AF_BUFS}
     r = {}
     # fcl: the channels-last copy of the feature stacks on the tensor-core path, untouched on the FP32 path
     if tc:
@@ -433,7 +382,7 @@ def test_affinity_tail_vs_fp64(n, m, pairs, engine, op, sm, end, peaky):
         y0 = B["y01"].view(G, n, m, 1024)[..., 512:]
     else:
         y0 = B["y01"].view(G, 1024, n, m)[:, 512:].permute(0, 2, 3, 1)
-    rr0 = norm_relu(y0, B["sc0"].view(G, 1, 1, 512), B["sh0"].view(G, 1, 1, 512))
+    rr0 = norm_operand(y0, B["sc0"].view(G, 1, 1, 512), B["sh0"].view(G, 1, 1, 512)).double()
     mx = end == "max"
     vn, tn = mean_bound(rr0.permute(0, 2, 3, 1), n, mx)       # new column j: over i
     ve, te = mean_bound(rr0.permute(0, 1, 3, 2), m, mx)       # end column i: over j
@@ -444,7 +393,7 @@ def test_affinity_tail_vs_fp64(n, m, pairs, engine, op, sm, end, peaky):
     # final new/end layer and its scatter
     h2 = B["h2"].view(G, L, 128) if tc else B["h2"].view(128, G, L).permute(1, 2, 0)
     grp = torch.arange(G, device="cuda")[:, None] * 2 + (torch.arange(L, device="cuda") >= m)[None]
-    r2 = norm_relu(h2, B["nsc2"].view(2 * G, 128)[grp], B["nsh2"].view(2 * G, 128)[grp])
+    r2 = norm_operand(h2, B["nsc2"].view(2 * G, 128)[grp], B["nsh2"].view(2 * G, 128)[grp]).double()
     a, Ta = logit_bound(r2, sd["w_link.w_new_end.conv1.6.weight"].reshape(-1).double().cuda(),
                         float(sd["w_link.w_new_end.conv1.6.bias"]), 128)
     s, Ts = sigmoid_bound(a, Ta)
@@ -452,7 +401,7 @@ def test_affinity_tail_vs_fp64(n, m, pairs, engine, op, sm, end, peaky):
                                worst_ratio(end_s[:G * n].view(G, n), s[:, m:], Ts[:, m:]))
     # link logits
     y3 = B["y3"].view(G, NM, 128) if tc else B["y3"].view(G, 128, NM).transpose(1, 2)
-    r3 = norm_relu(y3, B["sc3"].view(G, 1, 128), B["sh3"].view(G, 1, 128))
+    r3 = norm_operand(y3, B["sc3"].view(G, 1, 128), B["sh3"].view(G, 1, 128)).double()
     zr, Tz = logit_bound(r3, sd["w_link.conv1.9.weight"].reshape(-1).double().cuda(), float(sd["w_link.conv1.9.bias"]), 128)
     zk = (link if sm == "none" else B["z"])[:G * NM].view(G, NM)
     r["link_logit"] = worst_ratio(zk, zr, Tz)
@@ -477,7 +426,7 @@ def test_affinity_tail_vs_fp64(n, m, pairs, engine, op, sm, end, peaky):
             assert bool((got == 1).all()), "a softmax over one element is not exactly 1"
         if peaky:
             r["underflowed"] = float((ref < TINY).double().mean())
-    _report(f"affinity {_af_id((n, m, pairs, engine, op, sm, end, peaky))} [{'tc' if tc else 'fp32'}] (err / bound)",
+    report(f"affinity {_af_id((n, m, pairs, engine, op, sm, end, peaky))} [{'tc' if tc else 'fp32'}] (err / bound)",
             **r, logit_span=float(zr.abs().max()))
     assert all(v <= 1.0 for k, v in r.items() if k != "underflowed"), r
 
@@ -491,12 +440,11 @@ def test_det_score_vs_fp64(L, pairs, engine, flags, fusion):
     lib = _lib.load()
     net, sd = _net(fusion)
     wts = net.prepared()
-    g = torch.Generator().manual_seed(_seed("det score", L, pairs, engine, flags, fusion))
+    g = torch.Generator().manual_seed(case_seed("det score", L, pairs, engine, flags, fusion))
     feats0 = torch.randn(pairs, 3, 512, L, generator=g).cuda()
     feats0[:, 2] = float("nan")                                  # stack 2 is the fusion's output
     w3, b3 = sd["w_det.6.weight"].reshape(-1).double().cuda(), float(sd["w_det.6.bias"])
-    assert lib.mmmot_set_engine(ENGINE[engine]) == 0
-    try:
+    with lib_state(lib, engine=engine):
         lay, tc = stage_layout(lib, 1, pairs, L)
         assert tc == (det_path(L, engine) == "tc")
         thr = 0.0
@@ -505,13 +453,12 @@ def test_det_score_vs_fp64(L, pairs, engine, flags, fusion):
             raw = raw[:pairs * 3 * L].double()
             thr = float((torch.sigmoid(raw) if flags & _lib.SCORE_SIGMOID else raw).median())
         det, feats, ws = _run_det(lib, wts, fusion, flags, thr, pairs, L, feats0.clone())
-    finally:
-        lib.mmmot_set_engine(0)
-    _written(det, pairs * 3 * L, "det")
+    assert_written(det, pairs * 3 * L, "det")
     assert torch.equal(feats[:, :2], feats0[:, :2]), "feature stacks 0, 1 changed"
     assert bool(torch.isfinite(feats[:, 2]).all()), "stack 2 not written"
     size = fd_sizes(pairs, L)
-    f3, h2 = ws_view(ws, lay["f3"], size["f3"]), ws_view(ws, lay["h2"], size["h2"])
+    wsv = Workspace(ws, lay)
+    f3, h2 = wsv.view("f3", size["f3"]), wsv.view("h2", size["h2"])
     if tc:
         f3 = f3.view(pairs, L, 3, 512)
         for s in range(3):
@@ -535,13 +482,13 @@ def test_det_score_vs_fp64(L, pairs, engine, flags, fusion):
         assert 0 < float(step.sum()) < step.numel() or step.numel() == 1
     else:
         r["det"] = worst_ratio(got, s, Ts)
-    _report(f"det score L={L} pairs={pairs} {engine} flags={flags} {fusion} [{'tc' if tc else 'fp32'}] (err / bound)", **r)
+    report(f"det score L={L} pairs={pairs} {engine} flags={flags} {fusion} [{'tc' if tc else 'fp32'}] (err / bound)", **r)
     assert r["det"] <= 1.0, r
 
 
 def _run_det(lib, wts, fusion, flags, thr, pairs, L, feats):
-    det = _nan(pairs * 3 * L)
-    ws = _workspace(lib, int(lib.mmmot_fusion_det_workspace(pairs, L)))
+    det = nan_output(pairs * 3 * L)
+    ws = nan_workspace(lib, int(lib.mmmot_fusion_det_workspace(pairs, L)))
     rc = lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[fusion], flags, thr, pairs, L, vp(feats), vp(det), vp(ws), ws.numel(),
                                   None)
     torch.cuda.synchronize()
@@ -568,7 +515,7 @@ def test_skip_heads_vs_fp64(kind, R, n_img, L):
     net, sd = _net("C")
     wts = net.prepared()
     sdd = {k: v.double().cuda() for k, v in sd.items() if k.startswith("appearance.global_pool")}
-    g = torch.Generator().manual_seed(_seed("skip heads", kind, R, n_img, L))
+    g = torch.Generator().manual_seed(case_seed("skip heads", kind, R, n_img, L))
     pooled = [_pooled(kind, R, n_img, C, g).cuda() for C in SKIP_C]
     pairs = n_img // L
     r = {}
@@ -591,7 +538,7 @@ def test_skip_heads_vs_fp64(kind, R, n_img, L):
     assert lib.mmmot_debug_skip_heads(wts.ptr, *map(vp, pooled), n_img, L, vp(feats), None) == 0
     torch.cuda.synchronize()
     assert torch.equal(feats[:, 0], torch.cat(alone, 1)) and bool(torch.isnan(feats[:, 1:]).all())
-    _report(f"skip heads {kind} R={R} n_img={n_img} L={L} (err / bound)", **r)
+    report(f"skip heads {kind} R={R} n_img={n_img} L={L} (err / bound)", **r)
     assert max(r.values()) <= 1.0, r
 
 

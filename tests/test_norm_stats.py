@@ -7,22 +7,13 @@ they are, the fp32 runs round S2 by about k 2^-24 (var + mean^2), so var loses (
 while GroupNorm itself is conditioned only like mean/std.  The runs are therefore summed as differences from their
 fp32 mean, and each run is folded into the fp64 partial exactly (stat_fold in common.cuh).
 
-Bound.  With u = 2^-24, ybar, delta = y - ybar, and run c of k <= 32 valid columns with pivot p_c (its fp32 mean):
-    d = fl(y - p_c) carries u|d|; sum d takes k - 1 further roundings, sum d^2 k fma roundings, so in the worst case
-    |e1_c| <= 32 u sum_c |d|  and  |e2_c| <= 34 u sum_c d^2.
-  The fold (k p + s1, k p^2 + 2 p s1 + s2) is fp64, as are stats_reduce and gn_finalize: each adds a relative 2^-53 of
-  n (ybar^2 + var), below 2^-29 u (R^2 + 1) var -- invisible up to R = 10^4.  To first order
-    dvar = (1/n) sum_c [2 (p_c - ybar) e1_c + e2_c],      dmean = (1/n) sum_c e1_c,
-  with |d| <= |delta| + |p_c - ybar|.  A worst-case bound from this needs the largest deviation of a run's mean from
-  the group's, which structured data can make several std, and would be several times the var term below.  The tests
-  instead hold the statistics to
+Bound.  The statistics are held to
     |dvar| <= KAPPA u (|ybar| mean|delta| + mean delta^2),   |dmean| <= KAPPA1 u mean|y|,   KAPPA = 64, KAPPA1 = 40,
-  constants set from the rounding counts above (2 x 32 for the cross term, about 36 roundings for a run's sum) on the
-  argument that the k roundings of a run are independent, so their sum grows like sqrt(k) and stays well below the
-  coherent worst case.  They are empirical in that sense, not proven; what they rest on is measured by the CPU test
-  below (an emulation of the gemm_gen epilogue's summation order) and the GPU cases.  (A pivot taken from the run's
-  values, its first say, fails this bound at R = 1 once ReLU zeros surround a rare positive pivot: the ReLU cases.)  The bound is linear in R = |ybar|/std; the unshifted sums err by about sqrt(k) u ybar^2,
-  R / KAPPA times its first term, and the CPU test shows the bound rejects them at R >= 100.
+u = 2^-24, ybar the mean, delta = y - ybar (kernel_kit.stats_ratios, where the constants are derived from the rounding
+counts of a run).  They are empirical, not proven; what they rest on is measured by the CPU test below (an emulation of
+the gemm_gen epilogue's summation order) and the GPU cases.  The bound is linear in R = |ybar|/std; the unshifted sums
+err by about sqrt(k) u ybar^2, R / KAPPA times its first term, and the CPU test shows the bound rejects them at
+R >= 100.
 
 Kernel-level tests (GPU) run one contraction through the product's launch code and compare the statistics of its own
 partials, reduced in fp64 as stats_reduce does, with a two-pass fp64 mean and variance over the kernel's own stored Y,
@@ -32,52 +23,19 @@ columns share, as look-alike detections produce) or from the bias.  Every activa
 import ctypes
 import functools
 import math
-import zlib
 
 import numpy as np
 import pytest
 import torch
 
+from kernel_kit import (GEN, KAPPA, KAPPA1, LAYOUTS, U, Cols, case_seed, eval_net, fp16_split, lib_state, ne_table,
+                        pn_host_tables, reduce_parts, report, run_gen, stats_ratios, vp)
 from mmmot_b200 import _lib
 from mmmot_b200.weights import pack_tc
-from test_gen_engines import (ABS, COPY, LAYOUTS, MUL, NORM, SUB, Cols, _ne_table, _report,
-                              _pn_host_tables, run_gen)
 
 gpu = pytest.mark.gpu
-vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-U = 2.0 ** -24
-KAPPA, KAPPA1 = 64, 40
 RS = (1, 20, 100, 300)
 SOURCES = ("input", "bias")
-
-
-def _seed(*key):
-    return zlib.crc32(repr(key).encode())
-
-
-# ------------------------------------------------------------------------------------------------ bound
-def group_moments(y, grp, G):
-    """Two-pass fp64 over y [cols][M] (fp64) grouped by grp [cols] -> count, mean, var, mean|delta|, mean|y|."""
-    acc = lambda v: torch.zeros(G, y.shape[1], dtype=torch.float64, device=y.device).index_add_(0, grp, v)
-    n = torch.bincount(grp, minlength=G).double()[:, None]
-    mean = acc(y) / n
-    dev = y - mean[grp]
-    return n, mean, acc(dev * dev) / n, acc(dev.abs()) / n, acc(y.abs()) / n
-
-
-def stats_ratios(S1, S2, y, grp, G):
-    """gn_finalize's mean and var from the fp64 group sums (S1, S2) [G][M] against the two-pass values over y:
-    -> (worst dvar / bound, worst dmean / bound, largest |mean| / std over the channels)."""
-    n, mean, var, mad, may = group_moments(y, grp, G)
-    keep = n[:, 0] > 0
-    m = S1 / n
-    v = S2 / n - m * m
-    tv = KAPPA * U * (mean.abs() * mad + var)
-    tm = KAPPA1 * U * may
-    rv = ((v - var).abs() / tv.clamp_min(1e-300))[keep]
-    rm = ((m - mean).abs() / tm.clamp_min(1e-300))[keep]
-    cond = (mean.abs() / var.clamp_min(1e-300).sqrt())[keep]
-    return float(rv.max()), float(rm.max()), float(cond.max())
 
 
 # ------------------------------------------------------------------------------------------------ CPU: emulation
@@ -131,7 +89,7 @@ def test_bound_separates_one_pass_from_shifted(n):
         for form in ("one_pass", "shifted"):
             S1, S2 = emulate_chunk_stats(Y, form == "shifted")
             out[form] = stats_ratios(torch.from_numpy(S1)[None], torch.from_numpy(S2)[None], y, grp, 1)
-        _report(f"emulation n={n} R={R}", one_pass_var=out["one_pass"][0], shifted_var=out["shifted"][0],
+        report(f"emulation n={n} R={R}", one_pass_var=out["one_pass"][0], shifted_var=out["shifted"][0],
                 shifted_mean=out["shifted"][1])
         assert out["shifted"][0] <= 1.0 and out["shifted"][1] <= 1.0, out
         assert out["one_pass"][1] <= 1.0, out
@@ -165,15 +123,9 @@ def pair_features(g, G, n, m, K, c, op):
     detections sqrt2 e' (operand c + (e - e')/sqrt2, |.| leaves it alone since c >= 4); MUL objects c / 8 + e / 8,
     detections 8 + e' / 8 (operand ~ c + e + small terms)."""
     e1, e2 = torch.randn(G, n, K, generator=g), torch.randn(G, m, K, generator=g)
-    if op == MUL:
+    if op == GEN.MUL:
         return torch.cat([(c + e1) / 8, 8 + e2 / 8], 1)
     return torch.cat([2 * c + math.sqrt(2) * e1, math.sqrt(2) * e2], 1)
-
-
-def _reduce_parts(part, slot_group, G):
-    M = part.shape[1]
-    acc = lambda v: torch.zeros(G, M, dtype=torch.float64, device="cuda").index_add_(0, slot_group, v)
-    return acc(part[:, :, 0]), acc(part[:, :, 1])
 
 
 def _slot_groups(cols):
@@ -190,10 +142,10 @@ def check_partials(P, Y, cols, G, name):
     live = sg >= 0
     part = P[:cols.ntiles * 2]
     assert bool((part[~live] == 0).all()), "an empty half-tile has nonzero partials"
-    S1, S2 = _reduce_parts(part[live], sg[live], G)
+    S1, S2 = reduce_parts(part[live], sg[live], G)
     y = Y[cols.y_row.cuda()].double()
     rv, rm, cond = stats_ratios(S1, S2, y, cols.grp.cuda(), G)
-    _report(name, var_err_over_bound=rv, mean_err_over_bound=rm, max_mean_over_std=cond)
+    report(name, var_err_over_bound=rv, mean_err_over_bound=rm, max_mean_over_std=cond)
     return rv, rm, cond
 
 
@@ -203,14 +155,14 @@ def check_partials(P, Y, cols, G, name):
 # tiles per group, the last a 88-column tail); tables with per-group counts (the new/end MLP); pairs: 8 x 8 (N.M = 64),
 # 20 x 45 (tiles across rows, tail) and 2 x 128 (the pipelined producers, two whole rows per tile).  Names ending in
 # _relu take ReLU in the epilogue: its zeros count as values and can be a run's pivot.
-GEN_LAYOUTS = [("copy_S16", COPY, 512, 512, ("uniform", 16, 5)), ("copy_S300", COPY, 512, 512, ("uniform", 300, 3)),
-               ("copy_S600", COPY, 256, 512, ("uniform", 600, 2)), ("copy_ne", COPY, 512, 512, ("table", _ne_table)),
-               ("norm_S300", NORM, 512, 512, ("uniform", 300, 3)),
-               ("norm_ne", NORM, 128, 512, ("table", lambda: _ne_table(G=6, n=400, m=20))),
-               ("mul_8x8", MUL, 1024, 512, ("pair", 8, 8, 3)), ("abs_20x45", ABS, 1024, 512, ("pair", 20, 45, 2)),
-               ("sub_2x128", SUB, 1024, 512, ("pair", 2, 128, 2)), ("abs_2x128", ABS, 1024, 512, ("pair", 2, 128, 2)),
-               ("mul_2x128", MUL, 1024, 512, ("pair", 2, 128, 2)),
-               ("copy_S300_relu", COPY, 512, 512, ("uniform", 300, 3)), ("copy_ne_relu", COPY, 512, 512, ("table", _ne_table))]
+GEN_LAYOUTS = [("copy_S16", GEN.COPY, 512, 512, ("uniform", 16, 5)), ("copy_S300", GEN.COPY, 512, 512, ("uniform", 300, 3)),
+               ("copy_S600", GEN.COPY, 256, 512, ("uniform", 600, 2)), ("copy_ne", GEN.COPY, 512, 512, ("table", ne_table)),
+               ("norm_S300", GEN.NORM, 512, 512, ("uniform", 300, 3)),
+               ("norm_ne", GEN.NORM, 128, 512, ("table", lambda: ne_table(G=6, n=400, m=20))),
+               ("mul_8x8", GEN.MUL, 1024, 512, ("pair", 8, 8, 3)), ("abs_20x45", GEN.ABS, 1024, 512, ("pair", 20, 45, 2)),
+               ("sub_2x128", GEN.SUB, 1024, 512, ("pair", 2, 128, 2)), ("abs_2x128", GEN.ABS, 1024, 512, ("pair", 2, 128, 2)),
+               ("mul_2x128", GEN.MUL, 1024, 512, ("pair", 2, 128, 2)),
+               ("copy_S300_relu", GEN.COPY, 512, 512, ("uniform", 300, 3)), ("copy_ne_relu", GEN.COPY, 512, 512, ("table", ne_table))]
 GEN_CASES = [(lay, R, src) for lay in GEN_LAYOUTS for R in RS for src in SOURCES]
 
 
@@ -220,7 +172,7 @@ def test_gen_stats_conditioned(lay, R, source):
     """gemm_gen through mmmot_debug_gen on conditioned channels: every producer, uniform and table tiling."""
     name, gen, M, K, shape = lay
     lib = _lib.load()
-    g = torch.Generator().manual_seed(_seed(name, R, source))
+    g = torch.Generator().manual_seed(case_seed(name, R, source))
     wt, b, c = conditioned_weights(g, K, M, R, source)
     Wp, wps = pack_tc(wt)
     kw = {}
@@ -242,7 +194,7 @@ def test_gen_stats_conditioned(lay, R, source):
             y_rows = rows
         src = c + torch.randn(rows, K, generator=g)
         kw["ld_src"] = K
-        if gen == NORM:
+        if gen == GEN.NORM:
             kw["gsc"], kw["gsh"] = torch.ones(G, K).cuda(), torch.zeros(G, K).cuda()
     relu = int(name.endswith("_relu"))
     Y, P, _ = run_gen(lib, gen, wt, b, Wp, wps, src.cuda(), cols, y_rows, relu=relu, **kw)
@@ -263,7 +215,7 @@ TMA_CASES = [(lay, kind, R, src) for lay in LAYOUTS for kind in TMA_KINDS for R 
 @gpu
 @pytest.mark.parametrize("layout,kind,R,source", TMA_CASES, ids=[f"{c[0]}-{c[1]}-R{c[2]}-{c[3]}" for c in TMA_CASES])
 def test_tma_stats_conditioned(layout, kind, R, source):
-    """gemm_tma matrix mode through mmmot_debug_pn_contraction on the ragged layouts of test_gen_engines.py (group =
+    """gemm_tma matrix mode through mmmot_debug_pn_contraction on the ragged layouts of kernel_kit.LAYOUTS (group =
     pair)."""
     pairs, L, counts = LAYOUTS[layout]
     M, K, want_add = TMA_KINDS[kind]
@@ -271,15 +223,12 @@ def test_tma_stats_conditioned(layout, kind, R, source):
     ndet = pairs * L
     split = [0] + np.cumsum(counts).tolist()
     Pn = split[-1]
-    tiles_h = _pn_host_tables(split, pairs, L)[0]
+    tiles_h = pn_host_tables(split, pairs, L)[0]
     nt = len(tiles_h)
-    g = torch.Generator().manual_seed(_seed(layout, kind, R, source))
+    g = torch.Generator().manual_seed(case_seed(layout, kind, R, source))
     wt, b, c = conditioned_weights(g, K, M, R, source)
     Wp, wps = pack_tc(wt)
-    x = c + torch.randn(Pn, K, generator=g)
-    hi = x.half()
-    lo = (x - hi.float()).half()
-    X = torch.stack([hi, lo]).contiguous().cuda()
+    X = torch.stack(fp16_split(c + torch.randn(Pn, K, generator=g))).contiguous().cuda()
     add = torch.randn(ndet, M, generator=g) * 0.25 if want_add else None
     cap = nt + 3
     tiles = torch.zeros((cap, 4), dtype=torch.int32, device="cuda")
@@ -318,12 +267,12 @@ SIMT_CASES = [(lay, R, src) for lay in SIMT_LAYOUTS for R in RS for src in SOURC
 @gpu
 @pytest.mark.parametrize("lay,R,source", SIMT_CASES, ids=[f"{c[0][0]}-R{c[1]}-{c[2]}" for c in SIMT_CASES])
 def test_simt_stats_conditioned(lay, R, source):
-    """gemm_simt through mmmot_debug_simt (XM_DIRECT, XM_NORM_RELU with sc = 1, sh = 0), uniform and table tiling; the
+    """gemm_simt through mmmot_debug_simt_op (XM_DIRECT, XM_NORM_RELU with sc = 1, sh = 0), uniform and table tiling; the
     partials are one per (tile, channel)."""
     name, mode, M, K, shape = lay
     relu = int(name.endswith("_relu"))
     lib = _lib.load()
-    g = torch.Generator().manual_seed(_seed(name, R, source))
+    g = torch.Generator().manual_seed(case_seed(name, R, source))
     wt, b, c = conditioned_weights(g, K, M, R, source)
     if shape[0] == "uniform":
         _, S, G = shape
@@ -341,12 +290,12 @@ def test_simt_stats_conditioned(lay, R, source):
     sc, sh = torch.ones(G, K, device="cuda"), torch.zeros(G, K, device="cuda")
     if shape[0] == "uniform":
         # uniform tiling reads X + g*x_gs + k*x_ks + col: the same [K][P] buffer with x_gs = S, x_ks = P
-        rc = lib.mmmot_debug_simt(mode, M, K, vp(wd), vp(bd), relu, vp(x), S, P, vp(sc), vp(sh), S, G, None, 0, vp(Y), S, P,
-                                  vp(part), None)
+        rc = lib.mmmot_debug_simt_op(mode, M, K, vp(wd), vp(bd), relu, vp(x), S, P, vp(sc), vp(sh), 0, 0, 0, 0, 0, 0, S, G,
+                                     None, 0, None, None, 0, vp(Y), S, P, vp(part), None)
     else:
         tt = torch.tensor([[gi, c0, ln, 0] for gi, c0, ln in tiles], dtype=torch.int32, device="cuda")
-        rc = lib.mmmot_debug_simt(mode, M, K, vp(wd), vp(bd), relu, vp(x), 0, P, vp(sc), vp(sh), 0, 0, vp(tt), len(tiles),
-                                  vp(Y), 0, P, vp(part), None)
+        rc = lib.mmmot_debug_simt_op(mode, M, K, vp(wd), vp(bd), relu, vp(x), 0, P, vp(sc), vp(sh), 0, 0, 0, 0, 0, 0, 0, 0,
+                                     vp(tt), len(tiles), None, None, 0, vp(Y), 0, P, vp(part), None)
     torch.cuda.synchronize()
     assert rc == 0, rc
     assert bool(torch.isfinite(Y).all())
@@ -354,20 +303,11 @@ def test_simt_stats_conditioned(lay, R, source):
         assert bool((Y == 0).any()), "no ReLU zero among the outputs"
     grp = torch.tensor(np.repeat(np.arange(G), lens), device="cuda")
     tile_group = torch.tensor([t[0] for t in tiles], device="cuda")
-    S1, S2 = _reduce_parts(part, tile_group, G)
+    S1, S2 = reduce_parts(part, tile_group, G)
     rv, rm, cond = stats_ratios(S1, S2, Y.T.double(), grp, G)
-    _report(f"simt {name} R={R} {source}", var_err_over_bound=rv, mean_err_over_bound=rm, max_mean_over_std=cond)
+    report(f"simt {name} R={R} {source}", var_err_over_bound=rv, mean_err_over_bound=rm, max_mean_over_std=cond)
     assert cond >= 0.5 * R
     assert rv <= 1.0 and rm <= 1.0, (rv, rm)
-
-
-def test_simt_hook_rejects_bad_arguments(lib_built):
-    """mmmot_debug_simt validates its arguments before any CUDA call."""
-    lib = _lib.load()
-    z = ctypes.c_void_p(8)
-    assert lib.mmmot_debug_simt(2, 64, 64, z, None, 0, z, 0, 64, None, None, 64, 1, None, 0, z, 0, 64, None, None) == -1
-    assert lib.mmmot_debug_simt(1, 64, 64, z, None, 0, z, 0, 64, None, None, 64, 1, None, 0, z, 0, 64, None, None) == -1
-    assert lib.mmmot_debug_simt(0, 64, 64, z, None, 0, z, 5, 64, None, None, 0, 0, z, 1, z, 0, 64, None, None) == -1
 
 
 # ------------------------------------------------------------------------------------------------ GPU: affinity stage
@@ -383,9 +323,8 @@ def test_affinity_lookalike_vs_fp64(op, sm, n, m):
     cars give) against torch_ref.associate in float64: the effect a user sees of the statistics above."""
     from helpers import TOL, check_close
     from oracle import torch_ref
-    from test_gpu_parity import make_net
-    net, sd = make_net("C", op, sm, 0.2, 23)
-    g = torch.Generator().manual_seed(_seed(op, sm, n, m))
+    net, sd = eval_net("C", 23, affinity_op=op, softmax_mode=sm, neg_threshold=0.2)
+    g = torch.Generator().manual_seed(case_seed(op, sm, n, m))
     base = torch.relu(torch.randn(1, 3, 512, 1, generator=g)) + 0.5
     feats = base * (1 + 0.02 * torch.randn(1, 3, 512, n + m, generator=g))
     link, new, end = net.associate_batch(feats.cuda(), n, m)
@@ -396,12 +335,12 @@ def test_affinity_lookalike_vs_fp64(op, sm, n, m):
     # link logits of softmax "none" also has no element past that bound; for those logits the fraction past it is
     # reported only: near-zero logits of look-alike pairs miss it in any fp32 implementation (the fp32 oracle differs
     # from the fp64 one by 2.7e-5 max-norm on these inputs).
-    report = []
-    check_close(link[0], rl.squeeze(1), TOL, "link", report, max_outside=1.0 if sm == "none" else 0.0)
-    check_close(new[0], rn, TOL, "new", report)
-    check_close(end[0], re, TOL, "end", report)
-    _report(f"affinity {op} {sm} {n}x{m}", **{f"{w}_{k}": v for w, e, fo, wr in report
-                                              for k, v in (("err", e), ("outside", fo), ("worst", wr))})
+    rep = []
+    check_close(link[0], rl.squeeze(1), TOL, "link", rep, max_outside=1.0 if sm == "none" else 0.0)
+    check_close(new[0], rn, TOL, "new", rep)
+    check_close(end[0], re, TOL, "end", rep)
+    report(f"affinity {op} {sm} {n}x{m}", **{f"{w}_{k}": v for w, e, fo, wr in rep
+                                             for k, v in (("err", e), ("outside", fo), ("worst", wr))})
 
 
 # ------------------------------------------------------------------------------------------------ GPU: fusion, w_det
@@ -424,19 +363,16 @@ def _int_features(g, shape, R):
 def _exact_net(arch, seed):
     """A network whose fusion and w_det layer-1 weights are dyadic (see above); fusion C's gates have zero weights (a
     per-channel constant sigmoid(bias)), so that saturating gates cannot make 0/0."""
-    import mmmot_b200
-    from mmmot_b200.synthetic import synthetic_state_dict
-    sd = synthetic_state_dict(arch, seed=seed)
-    g = torch.Generator().manual_seed(seed)
-    for k, v in sd.items():
-        if (k.startswith("fusion_module.") and ".0." in k) or k.startswith("w_det.0."):
-            sd[k] = _dyadic(torch.randn(v.shape, generator=g) * 3 / 64)
-            if ".gate_" in k and k.endswith("weight"):
-                sd[k] = torch.zeros_like(v)
-    net = mmmot_b200.TrackingNet(2, appear_skippool=True, score_arch="branch_cls", score_fusion_arch=arch, test_mode=2,
-                                 dropblock=0)
-    net.load_state_dict(sd)
-    return net.cuda().eval(), {k: v.double() if v.is_floating_point() else v for k, v in sd.items()}
+    def dyadic(sd):
+        g = torch.Generator().manual_seed(seed)
+        for k, v in sd.items():
+            if (k.startswith("fusion_module.") and ".0." in k) or k.startswith("w_det.0."):
+                sd[k] = _dyadic(torch.randn(v.shape, generator=g) * 3 / 64)
+                if ".gate_" in k and k.endswith("weight"):
+                    sd[k] = torch.zeros_like(v)
+
+    net, sd = eval_net(arch, seed, edit=dyadic)
+    return net, {k: v.double() if v.is_floating_point() else v for k, v in sd.items()}
 
 
 def _gn_bound(y, gamma, beta):
@@ -476,18 +412,15 @@ def test_fusion_stage_conditioned(arch, L, pairs, eng, R):
     lib = _lib.load()
     net, sd64 = _fusion_net(arch)
     wts = net.prepared()
-    g = torch.Generator().manual_seed(_seed(arch, L, pairs, eng, R))
+    g = torch.Generator().manual_seed(case_seed(arch, L, pairs, eng, R))
     feats = torch.full((pairs, 3, 512, L), float("nan"))
     feats[:, :2] = _int_features(g, (pairs, 2, 512, L), R)
     fd = feats.cuda()
     det = torch.empty(pairs, 3, L, device="cuda")
     ws = torch.empty(int(lib.mmmot_fusion_det_workspace(pairs, L)), dtype=torch.uint8, device="cuda")
-    lib.mmmot_set_engine({"auto": 0, "fp32": 1, "tc": 2}[eng])
-    try:
+    with lib_state(lib, engine=eng):
         rc = lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[arch], 0, 0.0, pairs, L, vp(fd), vp(det), vp(ws), ws.numel(), None)
         torch.cuda.synchronize()
-    finally:
-        lib.mmmot_set_engine(0)
     assert rc == 0, rc
     got = fd[:, 2].double().cpu()
     f64 = feats[:, :2].double()
@@ -503,7 +436,7 @@ def test_fusion_stage_conditioned(arch, L, pairs, eng, R):
             T += Tb + 8 * U * z.abs()
             cond = max(cond, cb)
         worst = max(worst, float(((got[p] - ref).abs() / T).max()))
-    _report(f"fusion {arch} L={L} pairs={pairs} {eng} R={R}", err_over_bound=worst, max_mean_over_std=cond)
+    report(f"fusion {arch} L={L} pairs={pairs} {eng} R={R}", err_over_bound=worst, max_mean_over_std=cond)
     assert cond >= 0.5 * R
     assert worst <= 1.0, worst
 
@@ -521,7 +454,7 @@ def test_w_det_train_batch_stats(L, R):
     lib = _lib.load()
     net, sd64 = _fusion_net("C")
     wts = net.prepared()
-    g = torch.Generator().manual_seed(_seed("w_det", L, R))
+    g = torch.Generator().manual_seed(case_seed("w_det", L, R))
     feats = _int_features(g, (3, 512, L), R)
     det = torch.empty(3, L, device="cuda")
     bn = torch.full((2, 2, 512), float("nan"), device="cuda")
@@ -545,7 +478,7 @@ def test_w_det_train_batch_stats(L, R):
     y2 = F.conv1d(h.reshape(512, 3, L).transpose(0, 1), sd64["w_det.3.weight"], sd64["w_det.3.bias"]).transpose(0, 1)
     v2 = y2.reshape(256, -1).var(1, unbiased=False)
     l2 = float(((bn[1, 1, :256] - v2).abs() / v2).max())
-    _report(f"w_det train L={L} R={R}", var_err_over_bound=rv, mean_err_over_bound=rm, max_mean_over_std=cond,
+    report(f"w_det train L={L} R={R}", var_err_over_bound=rv, mean_err_over_bound=rm, max_mean_over_std=cond,
             layer2_var_rel_err=l2)
     assert cond >= 0.5 * R
     assert rv <= 1.0 and rm <= 1.0, (rv, rm)

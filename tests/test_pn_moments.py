@@ -24,29 +24,17 @@ import numpy as np
 import pytest
 import torch
 
+from kernel_kit import LAYOUTS, eval_net, fp16_split, lib_state, report, vp
 from mmmot_b200 import _lib
 from mmmot_b200.weights import pack_tc
-from test_gen_engines import LAYOUTS, _report
 
 gpu = pytest.mark.gpu
-vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
 TWO_PASS = 16                      # mmmot_set_debug bit 4
 PTXAS_LOG = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "mmmot_b200", "csrc", "build",
                          "pointnet.ptxas.log")
-# the matrix-mode layouts of test_gen_engines.py, plus pairs of very different sizes: 11200 points (two 32-tile
+# the matrix-mode layouts of kernel_kit.LAYOUTS, plus pairs of very different sizes: 11200 points (two 32-tile
 # slices, the second partial) between pairs of 16 one-point detections and of 16 x 37 points
 MOM_LAYOUTS = dict(LAYOUTS, skew=(3, 16, [1] * 16 + [700] * 16 + [37] * 16))
-
-
-class _Debug:
-    def __init__(self, lib, flags):
-        self.lib, self.flags = lib, flags
-
-    def __enter__(self):
-        self.lib.mmmot_set_debug(self.flags)
-
-    def __exit__(self, *a):
-        self.lib.mmmot_set_debug(0)
 
 
 def _inputs(layout, K, seed):
@@ -55,8 +43,7 @@ def _inputs(layout, K, seed):
     P = split[-1]
     g = torch.Generator().manual_seed(seed)
     x = torch.relu(torch.randn(P, K, generator=g) + 0.3)     # post-ReLU-like activations, many exact zeros
-    hi = x.half()
-    lo = (x - hi.float()).half()
+    hi, lo = fp16_split(x)
     return pairs, L, split, hi, lo, g
 
 
@@ -73,7 +60,7 @@ def _run(lib, pairs, L, split, hi, lo, K, M, wt, b, add, gamma, beta, dbg=0):
     mom = torch.full((pairs, K * K + K), float("nan"), dtype=torch.float64, device="cuda")
     det = torch.zeros((pairs * L, 64), dtype=torch.int64, device="cuda") if K == 64 else None
     keep = [t.cuda() if t is not None else None for t in (wt, Wp, b, add, gamma, beta)]
-    with _Debug(lib, dbg):
+    with lib_state(lib, dbg=dbg):
         rc = lib.mmmot_debug_pn_stats(vp(d_split), vp(h_split), pairs, L, vp(X), K, vp(keep[0]), vp(keep[1]), wps,
                                       vp(keep[2]), M, vp(keep[3]), vp(keep[4]), vp(keep[5]), vp(sc), vp(sh), vp(stats),
                                       vp(mom), vp(det), vp(ws), ws.numel(), None)
@@ -120,7 +107,7 @@ def test_moments_vs_fp64(layout, K):
         e = float(((got - want).abs() / (n_d * 2.0 ** -33 + 2.0 ** -40 * want.abs())).max())
         res["det"] = e
         assert e <= 1.0, e
-    _report(f"moments {layout} K={K}", **res)
+    report(f"moments {layout} K={K}", **res)
 
 
 # ------------------------------------------------------------------------------------------------ statistics
@@ -168,7 +155,7 @@ def test_stats_vs_fp64(layout, K, dbg):
     rest[heavy] = False
     r = dict(sc_rel=float(esc[:, rest].max()), sh_rel=float(esh[:, rest].max()),
              heavy_sc_rel=float(esc[:, heavy].max()), heavy_sh_rel=float(esh[:, heavy].max()))
-    _report(f"stats {layout} K={K} {'two-pass' if dbg else 'moments'}", **r)
+    report(f"stats {layout} K={K} {'two-pass' if dbg else 'moments'}", **r)
     tol = 1e-4 if dbg else 2e-5
     assert r["sc_rel"] <= tol and r["sh_rel"] <= tol, r
     if not dbg:
@@ -200,12 +187,8 @@ def test_stats_deterministic_and_batch_independent(K):
 def test_pointnet_features_batch_independent():
     """mmmot_pointnet_fwd on a batch of three pairs of different sizes and on its middle pair alone: that pair's
     features are bit-identical."""
-    import mmmot_b200 as mb
-    from mmmot_b200.synthetic import synthetic_state_dict
     lib = _lib.load()
-    net = mb.TrackingNet(2, appear_skippool=True, score_arch="branch_cls", score_fusion_arch="C", test_mode=2, dropblock=0)
-    net.load_state_dict(synthetic_state_dict("C", seed=0))
-    net.cuda().eval()
+    net, _ = eval_net("C", 0)
     wts = net.prepared()
     L = 16
     g = torch.Generator().manual_seed(3)
@@ -223,14 +206,11 @@ def test_pointnet_features_batch_independent():
         torch.cuda.synchronize()
         return feats.cpu()
 
-    lib.mmmot_set_engine(2)
-    try:
+    with lib_state(lib, engine="tc"):
         full = fwd(points, split, 3)
         full2 = fwd(points, split, 3)
         s0, s1 = int(split[L]), int(split[2 * L])
         one = fwd(points[s0:s1].contiguous(), (split[L:2 * L + 1] - s0).astype(np.int32), 1)
-    finally:
-        lib.mmmot_set_engine(0)
     assert torch.equal(full.view(torch.int32), full2.view(torch.int32))
     assert torch.equal(one[0, 1].view(torch.int32), full[1, 1].view(torch.int32))
 

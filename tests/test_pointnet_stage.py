@@ -7,7 +7,7 @@ fp64 (computed on the GPU) from the inputs it read, as stored, so no upstream er
 survives.  Every element a kernel owns must be written; the padding after each buffer, the buffers the path does not
 use, stacks 0 and 2 of feats and its guard band must come back untouched.  Every case prints err / bound (_report).
 
-Notation: u = 2^-24, TAU = 2^-18 (the tensor-core contraction bound of test_gen_engines.py: |y - y_ref| <= TAU S,
+Notation: u = 2^-24, TAU = 2^-18 (the tensor-core contraction bound, kernel_kit.TAU: |y - y_ref| <= TAU S,
 S = |W| A + |b| with A the magnitude of the operand the producer forms), a = gamma / sqrt(var + eps) and
 sh = beta - mean a the fp64 GroupNorm affine of the reference statistics, FP64 = 2^-40 (fp64 summation and
 cancellation, far below every other term).
@@ -16,8 +16,8 @@ GroupNorm statistics (gn_stats).  The kernel's mean and variance of values y_k t
 most T differ from the two-pass fp64 mean / var of y by
     tm = mean(T) + [KAPPA1 u mean|y|] + FP64 mean|y|,
     tv = 2 mean(|y - mean| T) + mean(T^2) + [KAPPA u (|mean| mean|y - mean| + var)] + FP64 (mean^2 + var),
-the bracketed terms only where the sums come from a contraction epilogue's fp32 runs (test_norm_stats.py).  From the
-input moments (layer 5 and the head on the tensor cores, test_pn_moments.py): S2 errs by 2^-18 |X|^T |X|, so
+the bracketed terms only where the sums come from a contraction epilogue's fp32 runs (kernel_kit.stats_ratios).  From
+the input moments (layer 5 and the head on the tensor cores, test_pn_moments.py): S2 errs by 2^-18 |X|^T |X|, so
     tv = 1.01 2^-18 mean_p (|x_p| . |w|)^2 + FP64 (mean^2 + var)  (+ (2/n) sum_d |a_d - abar| n_d 2^-33 sum_k |w_k|,
 the head's cross term with the 2^-33-rounded per-detection sums of x), and tm = FP64 (mean(|x| . |w|) + mean|y|).
 GroupNorm application (gn_apply): relu(fmaf(y_k, sc_k, sh_k)) with sc_k = fl(a_k), sh_k = fl(beta - mean_k a_k) and
@@ -46,8 +46,8 @@ Tensor-core path (L >= 16 under auto, or mmmot_set_engine(2)):
               sc / sh against gn_finalize in fp64 from the stored stats (32 channels per group, count L), one fp32
               rounding each: u |sc| + FP64 |a| (mean^2 + var) / (var + eps), and likewise for sh.
   feats       feats[pair][1][c][l] = relu(fmaf(o, sc, sh)) to u |ref| + 2^-126, from the stored o, sc, sh.
-FP32 path (L < 16 under auto, or mmmot_set_engine(1)): the FP32 engine's chain bound (contraction_bound,
-test_simt_engine.py) replaces TAU S; y1 from the points (xt equals them transposed bit for bit); sc1 / sh1 from y1
+FP32 path (L < 16 under auto, or mmmot_set_engine(1)): the FP32 engine's chain bound (kernel_kit.contraction_bound)
+replaces TAU S; y1 from the points (xt equals them transposed bit for bit); sc1 / sh1 from y1
 (|sc1 - a| <= |a| er + u |a|, |sh1 - sh| <= |a| tm + |mean a| er + u (|sh| + |mean a|)); t1 from y1 through layer 2
 recomputed; t0 from t1; big (the head) from y1, sc1 / sh1 and the addend u; gmean from t0 through layer 5 recomputed
 (its output is overwritten by the head), its statistics carrying the contraction bound, and segment_mean's fp32 lane
@@ -60,7 +60,6 @@ over 16 channels per group instead of 32, and pointnet_out_cl with l and c swapp
 """
 import ctypes
 import functools
-import math
 import os
 import re
 
@@ -68,42 +67,24 @@ import numpy as np
 import pytest
 import torch
 
-import mmmot_b200
+from kernel_kit import (CSRC, ENGINE, EPS, KAPPA, KAPPA1, PN_BUFS, TAU, TINY, U, Workspace, case_seed, contraction_bound,
+                        eval_net, group_moments, lib_state, nan_output, nan_workspace, norm_operand, pn_host_tables,
+                        ref_linear, report, stage_layout, stats_ratios, vp, worst_ratio)
 from mmmot_b200 import _lib
 from mmmot_b200.synthetic import synthetic_state_dict
 from mmmot_b200.weights import prepare
-from test_conv_engines import TAU
-from test_gen_engines import _pn_host_tables, _report, ref_linear
-from test_heads import GUARD, _workspace
-from test_norm_stats import KAPPA, KAPPA1, _seed, group_moments, stats_ratios
-from test_simt_engine import CSRC, contraction_bound, norm_operand, worst_ratio
 
 gpu = pytest.mark.gpu
-vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-U = 2.0 ** -24
-EPS = 1e-5
 FP64 = 2.0 ** -40
-TINY = 2.0 ** -126
 MOM = 2.0 ** -18                   # S2 of the moments kernel (test_pn_moments.py)
 FIX = 2.0 ** -33                   # one rounding to 2^-32 fixed point
-ENGINE = {"auto": 0, "fp32": 1, "tc": 2}
 W = _lib.W
-PN_BUFS = ("xt", "y1", "t0", "t1", "big", "segsum", "x1p", "xp", "gmean", "u", "ut", "hmean", "o", "sc1", "sh1", "sc",
-           "sh", "stats", "mom", "part", "gstart", "sstart", "seg", "cnt", "tiles", "ctab", "end")
 TC_CHECKS = ("tables", "x1p", "t1", "t0", "xp", "gmean", "ut", "hmean", "o", "conv2_stats", "conv2_affine", "feats")
 FP32_CHECKS = ("tables", "xt", "y1", "sc1_sh1", "t1", "t0", "big", "gmean", "u", "hmean", "o", "conv2_stats",
                "conv2_affine", "feats")
 
 
 # ------------------------------------------------------------------------------------------------ layout
-def pn_layout(lib, pairs, L, P):
-    """mmmot_debug_stage_layout(2, ...) -> ({buffer: byte offset, 'end': workspace bytes}, tensor-core path?)."""
-    off = (ctypes.c_size_t * 32)()
-    tc = ctypes.c_int(-1)
-    assert lib.mmmot_debug_stage_layout(2, pairs, L, P, off, ctypes.byref(tc)) == 0
-    return {k: int(off[i]) for i, k in enumerate(PN_BUFS)}, bool(tc.value)
-
-
 def pn_sizes(pairs, L, P, tc):
     """Bytes of each buffer as the header documents them, on the path tc (True: tensor cores)."""
     nd, mt = pairs * L, P // 128 + 2 * pairs + 2
@@ -263,11 +244,7 @@ def _points(kind, counts, g):
 
 @functools.lru_cache(maxsize=None)
 def _net():
-    sd = synthetic_state_dict("C", seed=31)
-    net = mmmot_b200.TrackingNet(2, appear_skippool=True, score_arch="branch_cls", score_fusion_arch="C", test_mode=2,
-                                 dropblock=0)
-    net.load_state_dict(sd)
-    net.cuda().eval()
+    net, sd = eval_net("C", 31)
     t = prepare(sd, "C")[0]
     w = lambda k: t[W[k]].double().cuda()
     wt = dict(layers=[tuple(t[W["PN_L1"] + 4 * j + i].double().cuda() for i in range(4)) for j in range(5)])
@@ -276,44 +253,23 @@ def _net():
     return net, wt
 
 
-class _Ws:
-    """Typed views of one run's workspace at the reported offsets."""
-
-    def __init__(self, ws, lay):
-        self.ws, self.lay = ws, lay
-
-    def view(self, name, count, dtype=torch.float32):
-        off = self.lay[name]
-        nbytes = count * torch.empty(0, dtype=dtype).element_size()
-        return self.ws[off:off + nbytes].view(dtype)
-
-    def untouched_after(self, name, nbytes):
-        """The bytes of buffer `name` past its first nbytes, up to the next buffer, still hold the 0xFF fill."""
-        off = self.lay[name]
-        nxt = min(v for k, v in self.lay.items() if v > off) if off < self.lay["end"] else off
-        return bool((self.ws[off + nbytes:nxt] == 255).all())
-
-
 def _run(lib, case):
     name, pairs, L, kind, engine = case
     net, wt = _net()
-    g = torch.Generator().manual_seed(_seed("pointnet stage", *case))
+    g = torch.Generator().manual_seed(case_seed("pointnet stage", *case))
     counts = _counts(kind, pairs, L, g)
     pts = _points(kind, counts, g).cuda()
     split = [0] + np.cumsum(counts).tolist()
     P = split[-1]
     hs = np.asarray(split, dtype=np.int32)
-    feats = torch.full((pairs * 3 * 512 * L + GUARD,), float("nan"), device="cuda")
-    assert lib.mmmot_set_engine(ENGINE[engine]) == 0
-    try:
-        lay, tc = pn_layout(lib, pairs, L, P)
+    feats = nan_output(pairs * 3 * 512 * L)
+    with lib_state(lib, engine=engine):
+        lay, tc = stage_layout(lib, 2, pairs, L, P)
         nbytes = int(lib.mmmot_pointnet_workspace(pairs, L, P))
-        ws = _workspace(lib, nbytes)
+        ws = nan_workspace(lib, nbytes)
         rc = lib.mmmot_pointnet_fwd(net.prepared().ptr, vp(pts), vp(torch.tensor(hs, device="cuda")),
                                     ctypes.c_void_p(hs.ctypes.data), pairs, L, vp(feats), vp(ws), nbytes, None)
         torch.cuda.synchronize()
-    finally:
-        lib.mmmot_set_engine(0)
     assert rc == 0, rc
     assert tc == (pn_path(L, engine) == "tc")
     assert lay["end"] == nbytes
@@ -326,19 +282,11 @@ def _run(lib, case):
     seg = torch.tensor(np.repeat(np.arange(pairs * L), counts), device="cuda")
     cnt = torch.tensor(counts, dtype=torch.float64, device="cuda")[:, None]
     return dict(pairs=pairs, L=L, P=P, split=split, pts=pts.double(), seg=seg, grp=seg // L, cnt=cnt, wt=wt,
-                W=_Ws(ws, lay), f=f, tc=tc)
-
-
-def _owned(W, name, count, dtype=torch.float32):
-    """The first `count` elements of buffer `name`, all written (finite), the rest of the buffer untouched."""
-    v = W.view(name, count, dtype)
-    assert bool(torch.isfinite(v.float() if dtype == torch.float16 else v).all()), f"{name}: an owned element was not written"
-    assert W.untouched_after(name, v.numel() * v.element_size()), f"{name}: written past its end"
-    return v
+                W=Workspace(ws, lay), f=f, tc=tc)
 
 
 def _planes(W, name, P, C):
-    h = _owned(W, name, 2 * P * C, torch.float16).view(2, P, C)
+    h = W.owned(name, 2 * P * C, torch.float16).view(2, P, C)
     return h[0].double() + h[1].double()
 
 
@@ -346,16 +294,16 @@ def _check_tables(d, tw):
     W, pairs, L, P, split = d["W"], d["pairs"], d["L"], d["P"], d["split"]
     tiles = [(p, c, min(tw, split[(p + 1) * L] - c)) for p in range(pairs) for c in range(split[p * L], split[(p + 1) * L], tw)]
     nt = len(tiles)
-    got = _owned(W, "tiles", 4 * nt, torch.int32).view(nt, 4).tolist()
+    got = W.owned("tiles", 4 * nt, torch.int32).view(nt, 4).tolist()
     assert got == [[p, c, ln, 0] for p, c, ln in tiles], "tiles"
     cnt = [split[(p + 1) * L] - split[p * L] for p in range(pairs)]
-    assert _owned(W, "cnt", pairs, torch.int32).tolist() == cnt, "cnt"
+    assert W.owned("cnt", pairs, torch.int32).tolist() == cnt, "cnt"
     gstart = np.concatenate([[0], np.cumsum([-(-c // tw) for c in cnt])]).tolist()
-    assert _owned(W, "gstart", pairs + 1, torch.int32).tolist() == gstart, "gstart"
-    assert torch.equal(_owned(W, "seg", P, torch.int32).long(), d["seg"]), "seg"
+    assert W.owned("gstart", pairs + 1, torch.int32).tolist() == gstart, "gstart"
+    assert torch.equal(W.owned("seg", P, torch.int32).long(), d["seg"]), "seg"
     if d["tc"]:
-        ctab = _pn_host_tables(split, pairs, L)[2]
-        assert _owned(W, "ctab", 4 * len(ctab), torch.int32).view(-1, 4).tolist() == ctab, "ctab"
+        ctab = pn_host_tables(split, pairs, L)[2]
+        assert W.owned("ctab", 4 * len(ctab), torch.int32).view(-1, 4).tolist() == ctab, "ctab"
     else:
         assert W.untouched_after("ctab", 0), "ctab written on the FP32 path"
     return 0.0
@@ -403,14 +351,14 @@ def check_tc(d):
     st = gn_stats(y2, grp, pairs, TAU * S2)
     z, Tz, mag = gn_apply(y2, TAU * S2, grp, st, g2, be2)
     y3, S3 = ref_linear(z.clamp_min(0), mag, W3, b3)
-    t1 = _owned(W, "t1", 64 * P).view(P, 64)
+    t1 = W.owned("t1", 64 * P).view(P, 64)
     r["t1"] = worst_ratio(t1, y3, TAU * S3 + Tz @ W3.abs())
     # t0: layer 4 from the stored t1
     W4, b4, g4, be4 = lyr[3]
     y = t1.double()
     z, Tz, mag = gn_apply(y, None, grp, gn_stats(y, grp, pairs), g3, be3)
     y4, S4 = ref_linear(z.clamp_min(0), mag, W4, b4)
-    t0 = _owned(W, "t0", 128 * P).view(P, 128)
+    t0 = W.owned("t0", 128 * P).view(P, 128)
     r["t0"] = worst_ratio(t0, y4, TAU * S4 + Tz @ W4.abs())
     # xp: norm_split of the stored t0
     y = t0.double()
@@ -420,7 +368,7 @@ def check_tc(d):
     del y, z, Tz, mag, y2, S2, y3, S3, y4, S4
     # gmean: layer 5 from xp, statistics from the moments, the per-detection means
     W5, b5, g5, be5 = lyr[4]
-    gm = _owned(W, "gmean", nd * 1024).view(nd, 1024)
+    gm = W.owned("gmean", nd * 1024).view(nd, 1024)
     r["gmean"] = 0.0
     for c0 in range(0, 1024, 128):
         cs = slice(c0, c0 + 128)
@@ -431,11 +379,11 @@ def check_tc(d):
         r["gmean"] = max(r["gmean"], worst_ratio(gm[:, cs], ref, T))
     del y, S, z, Tz, mag
     # ut: U = gmean WhG
-    ut = _owned(W, "ut", nd * 512).view(nd, 512)
+    ut = W.owned("ut", nd * 512).view(nd, 512)
     ref, S = ref_linear(gm.double(), gm.double().abs(), wt["PN_WHGT"], torch.zeros(512, dtype=torch.float64, device="cuda"))
     r["ut"] = worst_ratio(ut, ref, TAU * S)
     # hmean: the head from x1p and the stored addend ut
-    hm = _owned(W, "hmean", nd * 512).view(nd, 512)
+    hm = W.owned("hmean", nd * 512).view(nd, 512)
     WhA, bh = wt["PN_WHAT"], wt["PN_BH"]
     ad = ut.double() + bh                                             # a_d of the moments kernel
     n_p = _acc(cnt, torch.arange(nd, device="cuda") // L, pairs)
@@ -454,7 +402,7 @@ def check_tc(d):
         r["hmean"] = max(r["hmean"], worst_ratio(hm[:, cs], ref, T))
     del y, S, z, Tz, mag, add
     # o: conv2 from the stored hmean
-    o = _owned(W, "o", nd * 512).view(nd, 512)
+    o = W.owned("o", nd * 512).view(nd, 512)
     ref, S = ref_linear(hm.double(), hm.double().abs(), wt["PN_WOT"], wt["PN_BO"])
     r["o"] = worst_ratio(o, ref, TAU * S)
     _check_conv2(d, o, r)
@@ -471,20 +419,20 @@ def check_fp32(d):
         assert lay[k] == lay[PN_BUFS[PN_BUFS.index(k) + 1]], k
     for k in ("segsum", "x1p", "xp"):
         assert W.untouched_after(k, 0), f"{k} written on the FP32 path"
-    xt = _owned(W, "xt", 3 * P).view(3, P)
+    xt = W.owned("xt", 3 * P).view(3, P)
     assert torch.equal(xt.double(), d["pts"].T), "xt"
     r["xt"] = 0.0
     # y1 and its GroupNorm affine
     W1, b1, g1, be1 = lyr[0]
-    y1 = _owned(W, "y1", 64 * P).view(64, P)
+    y1 = W.owned("y1", 64 * P).view(64, P)
     ref, T = contraction_bound(W1, d["pts"].T.contiguous(), b1)
     r["y1"] = worst_ratio(y1, ref, T)
     y = y1.double().T
     mean, var, tm, tv = gn_stats(y, grp, pairs)
     a = g1 / torch.sqrt(var + EPS)
     er = tv / (2 * (var + EPS)) + FP64
-    sc1 = _owned(W, "sc1", pairs * 64).view(pairs, 64)
-    sh1 = _owned(W, "sh1", pairs * 64).view(pairs, 64)
+    sc1 = W.owned("sc1", pairs * 64).view(pairs, 64)
+    sh1 = W.owned("sh1", pairs * 64).view(pairs, 64)
     r["sc1_sh1"] = max(worst_ratio(sc1, a, a.abs() * er + U * a.abs()),
                        worst_ratio(sh1, be1 - mean * a, a.abs() * tm + (mean * a).abs() * er
                                    + U * ((be1 - mean * a).abs() + (mean * a).abs())))
@@ -496,18 +444,18 @@ def check_fp32(d):
     st = gn_stats(y2.T, grp, pairs, T2.T)
     z, Tz, _ = gn_apply(y2.T, T2.T, grp, st, g2, be2)
     y3, T3 = contraction_bound(W3, z.clamp_min(0).T.contiguous(), b3)
-    t1 = _owned(W, "t1", 64 * P).view(64, P)
+    t1 = W.owned("t1", 64 * P).view(64, P)
     r["t1"] = worst_ratio(t1, y3, T3 + (Tz @ W3.abs()).T)
     # t0: layer 4 from the stored t1
     W4, b4, g4, be4 = lyr[3]
     y = t1.double().T
     z, Tz, _ = gn_apply(y, None, grp, gn_stats(y, grp, pairs), g3, be3)
     y4, T4 = contraction_bound(W4, z.clamp_min(0).T.contiguous(), b4)
-    t0 = _owned(W, "t0", 128 * P).view(128, P)
+    t0 = W.owned("t0", 128 * P).view(128, P)
     r["t0"] = worst_ratio(t0, y4, T4 + (Tz @ W4.abs()).T)
     # big: the head from y1, sc1, sh1 and the addend u
-    u = _owned(W, "u", 512 * nd).view(512, nd)
-    big = _owned(W, "big", 1024 * P)[:512 * P].view(512, P)     # rows 512.. still hold layer 5's output
+    u = W.owned("u", 512 * nd).view(512, nd)
+    big = W.owned("big", 1024 * P)[:512 * P].view(512, P)     # rows 512.. still hold layer 5's output
     ref, T = contraction_bound(wt["PN_WHAT"], x2, wt["PN_BH"], u.double()[:, seg])
     r["big"] = worst_ratio(big, ref, T)
     del x2, y2, T2, y3, T3, y4, T4, ref, T
@@ -516,7 +464,7 @@ def check_fp32(d):
     y = t0.double().T
     z4, Tz4, _ = gn_apply(y, None, grp, gn_stats(y, grp, pairs), g4, be4)
     x5 = z4.clamp_min(0).T.contiguous()
-    gm = _owned(W, "gmean", 1024 * nd).view(1024, nd)
+    gm = W.owned("gmean", 1024 * nd).view(1024, nd)
     r["gmean"] = 0.0
     for c0 in range(0, 1024, 128):
         cs = slice(c0, c0 + 128)
@@ -532,11 +480,11 @@ def check_fp32(d):
     # hmean from big, the head's statistics recomputed
     y = big.double().T
     z, Tz, _ = gn_apply(y, None, grp, gn_stats(y, grp, pairs), wt["PN_GHW"], wt["PN_GHB"])
-    hm = _owned(W, "hmean", 512 * nd).view(512, nd)
+    hm = W.owned("hmean", 512 * nd).view(512, nd)
     ref, T = seg_mean_fp32(z, Tz, seg, cnt)
     r["hmean"] = worst_ratio(hm.T, ref, T)
     # o: conv2 from the stored hmean
-    o = _owned(W, "o", 512 * nd).view(512, nd)
+    o = W.owned("o", 512 * nd).view(512, nd)
     ref, T = contraction_bound(wt["PN_WOT"], hm.double(), wt["PN_BO"])
     r["o"] = worst_ratio(o, ref, T)
     _check_conv2(d, o.T.contiguous(), r)
@@ -553,7 +501,7 @@ def test_pointnet_stage_vs_fp64(case):
     r = check_tc(d) if d["tc"] else check_fp32(d)
     assert set(r) == set(TC_CHECKS if d["tc"] else FP32_CHECKS), sorted(r)
     extra = {"layer1_mean_over_std": d["cond"]} if "cond" in d else {}
-    _report(f"pointnet {case[0]} pairs={d['pairs']} L={d['L']} P={d['P']} [{'tc' if d['tc'] else 'fp32'}] (err / bound)",
+    report(f"pointnet {case[0]} pairs={d['pairs']} L={d['L']} P={d['P']} [{'tc' if d['tc'] else 'fp32'}] (err / bound)",
             **r, **extra)
     if case[0] == "far":
         assert d["cond"] >= 30, d["cond"]
@@ -566,12 +514,11 @@ def test_pointnet_layout_without_device():
     documented size on the path the engine setting selects (xt, y1, big, u empty on the tensor cores, ut on the FP32
     path), and `end` is mmmot_pointnet_workspace."""
     lib = _lib.load()
-    try:
-        for engine in ENGINE:
-            assert lib.mmmot_set_engine(ENGINE[engine]) == 0
+    for engine in ENGINE:
+        with lib_state(lib, engine=engine):
             for pairs, L, P in ((1, 1, 1), (2, 2, 100), (1, 15, 900), (1, 16, 1000), (3, 16, 9512), (2, 64, 16384),
                                 (1, 256, 131072), (1, 300, 28800)):
-                lay, tc = pn_layout(lib, pairs, L, P)
+                lay, tc = stage_layout(lib, 2, pairs, L, P)
                 assert tc == (pn_path(L, engine) == "tc"), (engine, L)
                 assert lay["end"] == int(lib.mmmot_pointnet_workspace(pairs, L, P))
                 size = pn_sizes(pairs, L, P, tc)
@@ -580,8 +527,6 @@ def test_pointnet_layout_without_device():
                     assert lay[b] - lay[a] == _align(size[a]), (engine, pairs, L, P, a)
                 for k in (("xt", "y1", "big", "u") if tc else ("ut", "sstart", "mom")):
                     assert size[k] == 0
-    finally:
-        lib.mmmot_set_engine(0)
     off = (ctypes.c_size_t * 32)()
     for args in ((2, 1, 4, 0), (2, 0, 4, 10), (2, 1, 0, 10)):
         assert lib.mmmot_debug_stage_layout(*args, off, None) == -1, args
@@ -759,7 +704,7 @@ def test_bounds_reject_planted_defects():
             swapped[:, c0:c0 + n, l0:l0 + n] = good[:, c0:c0 + n, l0:l0 + n].transpose(1, 2)
     out["out fp32"] = worst_ratio(good, ref, T)
     out["out l/c swapped"] = worst_ratio(swapped, ref, T)
-    _report("planted defects (err / bound)", **out)
+    report("planted defects (err / bound)", **out)
     assert max(out["l1 fp32"], out["mean fp32"], out["head fp32"], out["conv2 fp32"], out["out fp32"]) <= 1.0, out
     assert min(out["l1 next pair"], out["mean / (n+1)"], out["head neighbour U"], out["conv2 16 per group"],
                out["out l/c swapped"]) > 10.0, out

@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from helpers import GOLDEN_DIR
+from kernel_kit import vp
 from mmmot_b200.lidar_crop import box_camera_to_lidar, detection_planes, fov_planes
 from oracle.crop_ref import crop_points_ref
 from oracle.make_prep_goldens import kitti_calib, synthetic_scan
@@ -218,7 +219,6 @@ def test_gpu_bad_arguments_are_rejected():
     split = torch.zeros(3, dtype=torch.int32, device="cuda")
     out = torch.zeros(10, 4, device="cuda")
     ws = torch.empty(int(lib.mmmot_prep_workspace(60, 2, 2)), dtype=torch.uint8, device="cuda")
-    vp = lambda t: ctypes.c_void_p(t.data_ptr())
     ints = lambda *v: (ctypes.c_int * len(v))(*v)
 
     def count(offs, det_frame, stride=4):

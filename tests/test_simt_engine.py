@@ -14,19 +14,13 @@ x (XM_DIRECT), relu(fma(x, sc, sh)) (XM_NORM_RELU; the fma as one fp64 multiply-
 and its absolute value (XM_PAIR_*), the zero-padded im2col with k = (ky*3 + kx)*Cin + ci (XM_CONV3).  The contraction
 is then done in fp64.
 
-Bound.  Output (co, c) is the sequential chain acc = fma(w_k, x_k, acc) over k = 0..K-1, then + bias, + addend and ReLU,
-each an fp32 rounding.  With u = 2^-24 and s_k the fp64 prefix sum of w_j x_j, j <= k, in that order, the rounding of
-step k is at most u |s_k| to first order, so
-    |y - y64| <= 1.01 u (sum_k |s_k| + |s_K + b| + |y^| [addend]) + u sum_k |w_k x_k|,
-y^ the value after the addend.  The factor 1.01 covers the second-order terms (K u < 10^-3 here); the last term covers
-the rare double rounding of the fp64 emulation of fma in the NORM_RELU operand.  ReLU is 1-Lipschitz.  The bound is
-derived, not measured: no case needs a looser constant.  On random data sum_k |s_k| grows like K^1.5 while one term of
-the chain is of order 1/K of it at most, so a single dropped or wrong tap at K = 4608 misses the bound by far more than
-an order of magnitude (the CPU self-test shows it with an fp32 emulation of the kernel's arithmetic).
+Bound.  Every output against the chain bound of the engine's sequential fma accumulation, kernel_kit.contraction_bound
+(derived there, not measured); the CPU self-test below shows with an fp32 emulation of the kernel's arithmetic that a
+single dropped or wrong tap at K = 4608 misses it by far more than an order of magnitude.
 
 Every launch also fills Y and the partials with NaN first: every element the launch owns must be written and every
 other element of the buffer (gaps of padded strides and a guard band past the end) must stay NaN.  The GroupNorm
-partials are checked against fp64 statistics of the kernel's own stored Y, to the bound of test_norm_stats.py.
+partials are checked against fp64 statistics of the kernel's own stored Y, to the bound of kernel_kit.stats_ratios.
 """
 import ctypes
 import dataclasses
@@ -38,60 +32,22 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from kernel_kit import (CSRC, XM, case_seed, contraction_bound, nan_output, norm_operand, reduce_parts, report,
+                        stats_ratios, vp, worst_ratio)
 from mmmot_b200 import _lib
-from test_gen_engines import _report
-from test_norm_stats import _reduce_parts, _seed, stats_ratios
 
 gpu = pytest.mark.gpu
-vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-U = 2.0 ** -24
 TN = 128        # the engine's column tile
 GUARD = 512     # NaN floats past the end of every output buffer
-DIRECT, NORM, MUL, ABS, SUB, CONV = range(6)
-CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "mmmot_b200", "csrc")
 
 
-# ------------------------------------------------------------------------------------------------ reference and bound
-def contraction_bound(wt, xin, bias=None, add=None, relu=False, chunk=1 << 25):
-    """fp64 reference and error bound of the engine's outputs (see the module docstring).  wt [K][M] and xin [K][C]
-    hold fp32 values as fp64, bias [M] or None, add [M][C] the addend of each output or None.  Chunked over the
-    columns, on the inputs' device.  -> (y64 [M][C], T [M][C])."""
-    K, M = wt.shape
-    C = xin.shape[1]
-    y = torch.empty(M, C, dtype=torch.float64, device=xin.device)
-    T = torch.empty_like(y)
-    step = max(1, chunk // (K * M))
-    for c0 in range(0, C, step):
-        c1 = min(C, c0 + step)
-        prod = wt[:, :, None] * xin[:, None, c0:c1]          # [K][M][c], exact in fp64
-        t = U * prod.abs().sum(0)
-        prod.cumsum_(0)
-        s = prod[-1] + (0.0 if bias is None else bias[:, None])
-        acc = prod.abs_().sum(0) + s.abs()
-        if add is not None:
-            s = s + add[:, c0:c1]
-            acc += s.abs()
-        T[:, c0:c1] = 1.01 * U * acc + t
-        y[:, c0:c1] = s.clamp_min(0) if relu else s
-    return y, T
-
-
-def worst_ratio(got, ref, T):
-    err = (got.double() - ref).abs()
-    return float(torch.where(err == 0, torch.zeros_like(err), err / T).max())
-
-
-def norm_operand(v, sc, sh):
-    """relu(fmaf(v, sc, sh)) in fp32: the product of two fp32 values is exact in fp64, the add rounds once, then to fp32."""
-    return (v.double() * sc.double() + sh.double()).float().clamp_min(0)
-
-
+# ------------------------------------------------------------------------------------------------ reference
 def pair_operand(f, op, n, m):
     """f [G][K][Lf] fp32 -> the pairwise operand [K][G*n*m], column g*n*m + i*m + j from object i and detection n + j."""
     s = torch.arange(n * m, device=f.device)
     a, b = f[:, :, s // m], f[:, :, n + s % m]
-    x = a * b if op == MUL else (a - b) * 0.5
-    if op == ABS:
+    x = a * b if op == XM.MUL else (a - b) * 0.5
+    if op == XM.ABS:
         x = x.abs()
     return x.permute(1, 0, 2).reshape(f.shape[1], -1)
 
@@ -141,7 +97,7 @@ def test_bound_self_test():
     bad = xin.clone()
     bad[tap * cin + ci, col] = 0
     r_bad = worst_ratio(torch.from_numpy(emulate_fp32(wt.numpy(), bad.numpy(), b.numpy())), ref, T)
-    _report("emulation conv K=4608", err_over_bound=r_ok, dropped_tap=r_bad)
+    report("emulation conv K=4608", err_over_bound=r_ok, dropped_tap=r_bad)
     assert r_ok <= 1.0 and r_bad > 10.0, (r_ok, r_bad)
     # NORM_RELU with the per-detection addend
     K, M = 64, 64
@@ -163,7 +119,7 @@ def test_bound_self_test():
     wrong[:, c] = addend[:, 4]
     bad = emulate_fp32(wt.numpy(), xin.numpy(), b.numpy(), wrong.numpy(), relu=True)
     r_bad = worst_ratio(torch.from_numpy(bad), ref, T)
-    _report("emulation head addend", err_over_bound=r_ok, neighbour_addend=r_bad)
+    report("emulation head addend", err_over_bound=r_ok, neighbour_addend=r_bad)
     assert r_ok <= 1.0 and r_bad > 10.0, (r_ok, r_bad)
 
 
@@ -201,12 +157,12 @@ class Case:
 
 
 def conv_case(cin, cout, h, w, n_img, bias=True, relu=False, part=True):
-    return Case(f"conv{cin}-{cout}-{h}x{w}x{n_img}{'-relu' if relu else ''}", CONV, cout, 9 * cin, S=n_img * h * w, H=h,
+    return Case(f"conv{cin}-{cout}-{h}x{w}x{n_img}{'-relu' if relu else ''}", XM.CONV, cout, 9 * cin, S=n_img * h * w, H=h,
                 W=w, bias=bias, relu=relu, part=part)
 
 
 def pair_case(op, n, m, G, M=1024, pad=0):
-    name = ("mul", "abs", "sub")[op - MUL]
+    name = ("mul", "abs", "sub")[op - XM.MUL]
     return Case(f"{name}-{n}x{m}-G{G}-M{M}", op, M, 512, S=n * m, groups=G, n=n, m=m, Lf=n + m + pad, y_gs=M * n * m,
                 y_ms=n * m)
 
@@ -266,54 +222,54 @@ CONV_CASES = [
     conv_case(512, 512, 5, 9, 4, relu=True),                # odd map at K = 4608
 ]
 PAIR_SHAPES = [(1, 1, 3), (1, 7, 6), (7, 1, 3), (6, 8, 6), (5, 13, 3), (12, 16, 6), (128, 128, 3)]
-PAIR_CASES = ([pair_case(op, n, m, G) for op in (MUL, ABS, SUB) for n, m, G in PAIR_SHAPES]
-              + [pair_case(MUL, 5, 13, 3, M=64, pad=2), pair_case(ABS, 1, 7, 6, M=64), pair_case(SUB, 12, 16, 3, M=64, pad=1)])
+PAIR_CASES = ([pair_case(op, n, m, G) for op in (XM.MUL, XM.ABS, XM.SUB) for n, m, G in PAIR_SHAPES]
+              + [pair_case(XM.MUL, 5, 13, 3, M=64, pad=2), pair_case(XM.ABS, 1, 7, 6, M=64), pair_case(XM.SUB, 12, 16, 3, M=64, pad=1)])
 TABLE_CASES = [
-    table_case("pn-l1", DIRECT, 64, 3),                     # PointNet trunk (FP32 path: training, or L < 16)
-    table_case("pn-l2", NORM, 64, 64),
-    table_case("pn-l4", NORM, 128, 64, relu=True),
-    table_case("pn-l5", NORM, 1024, 128),
-    table_case("pn-head", NORM, 512, 64, addend=True),      # + U[:, det(p)], ld_add = ndet
-    table_case("pn-head-relu", NORM, 512, 64, addend=True, relu=True),
-    ne_case("ne-l1-G3-7x130", DIRECT, 512, 3, 7, 130),      # affinity new/end MLP (FP32 path: N.M < 64 in eval)
-    ne_case("ne-l1-G2-1x1", DIRECT, 512, 2, 1, 1),
-    ne_case("ne-l2-G2-129x1", NORM, 128, 2, 129, 1),
-    table_case("pn-l5-padded", NORM, 1024, 128, ld_pad=5),  # x_ks = y_ms > columns: the gap columns stay NaN
+    table_case("pn-l1", XM.DIRECT, 64, 3),                     # PointNet trunk (FP32 path: training, or L < 16)
+    table_case("pn-l2", XM.NORM, 64, 64),
+    table_case("pn-l4", XM.NORM, 128, 64, relu=True),
+    table_case("pn-l5", XM.NORM, 1024, 128),
+    table_case("pn-head", XM.NORM, 512, 64, addend=True),      # + U[:, det(p)], ld_add = ndet
+    table_case("pn-head-relu", XM.NORM, 512, 64, addend=True, relu=True),
+    ne_case("ne-l1-G3-7x130", XM.DIRECT, 512, 3, 7, 130),      # affinity new/end MLP (FP32 path: N.M < 64 in eval)
+    ne_case("ne-l1-G2-1x1", XM.DIRECT, 512, 2, 1, 1),
+    ne_case("ne-l2-G2-129x1", XM.NORM, 128, 2, 129, 1),
+    table_case("pn-l5-padded", XM.NORM, 1024, 128, ld_pad=5),  # x_ks = y_ms > columns: the gap columns stay NaN
 ]
 STRIDED_CASES = (
-    [strided_case(f"wdet1-L{L}", DIRECT, 512, 512, L, 3, 512 * L, L, 512 * L, L, relu=L % 2 == 1) for L in (1, 5, 127, 128, 129, 300)]
-    + [strided_case(f"wdet2-L{L}", NORM, 256, 512, L, 3, 512 * L, L, 256 * L, L) for L in (1, 5, 127, 128, 129, 300)]
-    + [strided_case(f"wdet2-eval-L{L}", DIRECT, 256, 512, L, 3, 512 * L, L, 256 * L, L, relu=True, part=False) for L in (5, 63)]
-    + [strided_case(f"pn-conv2-L{L}", DIRECT, 512, 512, L, 3, L, 3 * L, L, 3 * L) for L in (5, 130)]
-    + [strided_case(f"pn-U-{nd}", DIRECT, 512, 1024, nd, 1, 0, nd, 0, nd, bias=False, part=False) for nd in (48, 200)]
-    + [strided_case(f"fusion-K{K}-L{L}", DIRECT, 512, K, L, 2, 1536 * L, L, 512 * L, L) for K in (512, 1024) for L in (16, 63)]
-    + [strided_case(f"aff-l2-{nm}", NORM, 512, 512, nm, 3, 1024 * nm, nm, 512 * nm, nm) for nm in (48, 65)]
-    + [strided_case(f"aff-l3-{nm}", NORM, 128, 512, nm, 3, 512 * nm, nm, 128 * nm, nm) for nm in (48, 65)]
-    + [strided_case("padded-rows", NORM, 192, 96, 130, 2, 140 * 96, 140, 192 * 150, 150, relu=True)]   # gaps stay NaN
+    [strided_case(f"wdet1-L{L}", XM.DIRECT, 512, 512, L, 3, 512 * L, L, 512 * L, L, relu=L % 2 == 1) for L in (1, 5, 127, 128, 129, 300)]
+    + [strided_case(f"wdet2-L{L}", XM.NORM, 256, 512, L, 3, 512 * L, L, 256 * L, L) for L in (1, 5, 127, 128, 129, 300)]
+    + [strided_case(f"wdet2-eval-L{L}", XM.DIRECT, 256, 512, L, 3, 512 * L, L, 256 * L, L, relu=True, part=False) for L in (5, 63)]
+    + [strided_case(f"pn-conv2-L{L}", XM.DIRECT, 512, 512, L, 3, L, 3 * L, L, 3 * L) for L in (5, 130)]
+    + [strided_case(f"pn-U-{nd}", XM.DIRECT, 512, 1024, nd, 1, 0, nd, 0, nd, bias=False, part=False) for nd in (48, 200)]
+    + [strided_case(f"fusion-K{K}-L{L}", XM.DIRECT, 512, K, L, 2, 1536 * L, L, 512 * L, L) for K in (512, 1024) for L in (16, 63)]
+    + [strided_case(f"aff-l2-{nm}", XM.NORM, 512, 512, nm, 3, 1024 * nm, nm, 512 * nm, nm) for nm in (48, 65)]
+    + [strided_case(f"aff-l3-{nm}", XM.NORM, 128, 512, nm, 3, 512 * nm, nm, 128 * nm, nm) for nm in (48, 65)]
+    + [strided_case("padded-rows", XM.NORM, 192, 96, 130, 2, 140 * 96, 140, 192 * 150, 150, relu=True)]   # gaps stay NaN
 )
 CASES = CONV_CASES + PAIR_CASES + TABLE_CASES + STRIDED_CASES
 
 # Every gemm_simt_launch call site of the product: (file, what, mode, M, K, tiling).
 CALL_SITES = (
-    [("appearance.cu", f"eval VGG conv {ci}->{co}", CONV, co, 9 * ci, "uniform") for ci, co in
+    [("appearance.cu", f"eval VGG conv {ci}->{co}", XM.CONV, co, 9 * ci, "uniform") for ci, co in
      ((3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256), (256, 512), (512, 512))]
-    + [("train.cu", f"training VGG conv {ci}->{co}", CONV, co, 9 * ci, "uniform") for ci, co in
+    + [("train.cu", f"training VGG conv {ci}->{co}", XM.CONV, co, 9 * ci, "uniform") for ci, co in
        ((3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256), (256, 512), (512, 512))]
-    + [("train.cu", "w_det layer 1", DIRECT, 512, 512, "uniform"), ("train.cu", "w_det layer 2", NORM, 256, 512, "uniform"),
-       ("affinity.cu", "layer 1 multiply", MUL, 1024, 512, "uniform"),
-       ("affinity.cu", "layer 1 minus_abs", ABS, 1024, 512, "uniform"),
-       ("affinity.cu", "layer 1 minus", SUB, 1024, 512, "uniform"),
-       ("affinity.cu", "new/end layer 1", DIRECT, 512, 512, "table"),
-       ("affinity.cu", "new/end layer 2", NORM, 128, 512, "table"),
-       ("affinity.cu", "layer 2", NORM, 512, 512, "uniform"), ("affinity.cu", "layer 3", NORM, 128, 512, "uniform"),
-       ("fusion_det.cu", "fusion A input", DIRECT, 512, 1024, "uniform"),
-       ("fusion_det.cu", "fusion B/C inputs and gates", DIRECT, 512, 512, "uniform"),
-       ("fusion_det.cu", "w_det layer 1", DIRECT, 512, 512, "uniform"),
-       ("fusion_det.cu", "w_det layer 2", DIRECT, 256, 512, "uniform"),
-       ("pointnet.cu", "trunk layer 1", DIRECT, 64, 3, "table"), ("pointnet.cu", "trunk layers 2, 3", NORM, 64, 64, "table"),
-       ("pointnet.cu", "trunk layer 4", NORM, 128, 64, "table"), ("pointnet.cu", "trunk layer 5", NORM, 1024, 128, "table"),
-       ("pointnet.cu", "U", DIRECT, 512, 1024, "uniform"), ("pointnet.cu", "head", NORM, 512, 64, "table+addend"),
-       ("pointnet.cu", "conv2", DIRECT, 512, 512, "uniform")]
+    + [("train.cu", "w_det layer 1", XM.DIRECT, 512, 512, "uniform"), ("train.cu", "w_det layer 2", XM.NORM, 256, 512, "uniform"),
+       ("affinity.cu", "layer 1 multiply", XM.MUL, 1024, 512, "uniform"),
+       ("affinity.cu", "layer 1 minus_abs", XM.ABS, 1024, 512, "uniform"),
+       ("affinity.cu", "layer 1 minus", XM.SUB, 1024, 512, "uniform"),
+       ("affinity.cu", "new/end layer 1", XM.DIRECT, 512, 512, "table"),
+       ("affinity.cu", "new/end layer 2", XM.NORM, 128, 512, "table"),
+       ("affinity.cu", "layer 2", XM.NORM, 512, 512, "uniform"), ("affinity.cu", "layer 3", XM.NORM, 128, 512, "uniform"),
+       ("fusion_det.cu", "fusion A input", XM.DIRECT, 512, 1024, "uniform"),
+       ("fusion_det.cu", "fusion B/C inputs and gates", XM.DIRECT, 512, 512, "uniform"),
+       ("fusion_det.cu", "w_det layer 1", XM.DIRECT, 512, 512, "uniform"),
+       ("fusion_det.cu", "w_det layer 2", XM.DIRECT, 256, 512, "uniform"),
+       ("pointnet.cu", "trunk layer 1", XM.DIRECT, 64, 3, "table"), ("pointnet.cu", "trunk layers 2, 3", XM.NORM, 64, 64, "table"),
+       ("pointnet.cu", "trunk layer 4", XM.NORM, 128, 64, "table"), ("pointnet.cu", "trunk layer 5", XM.NORM, 1024, 128, "table"),
+       ("pointnet.cu", "U", XM.DIRECT, 512, 1024, "uniform"), ("pointnet.cu", "head", XM.NORM, 512, 64, "table+addend"),
+       ("pointnet.cu", "conv2", XM.DIRECT, 512, 512, "uniform")]
 )
 # gemm_simt_launch expressions per source file (the test hooks in api.cu aside); a new call site changes these counts
 LAUNCH_EXPRESSIONS = {"appearance.cu": 1, "train.cu": 3, "affinity.cu": 7, "fusion_det.cu": 3, "pointnet.cu": 5}
@@ -343,19 +299,19 @@ def test_simt_op_hook_rejects_bad_arguments(lib_built):
     z = ctypes.c_void_p(8)
     zi = ctypes.c_void_p(16)
 
-    def call(mode=DIRECT, M=64, K=64, X=z, x_gs=0, sc=None, sh=None, n=0, m=0, Lf=0, H=0, W=0, Cin=0, S=64, groups=1,
+    def call(mode=XM.DIRECT, M=64, K=64, X=z, x_gs=0, sc=None, sh=None, n=0, m=0, Lf=0, H=0, W=0, Cin=0, S=64, groups=1,
              tt=None, nt=0, addend=None, seg=None, ld_add=0, y_gs=0, Wt=z):
         return lib.mmmot_debug_simt_op(mode, M, K, Wt, None, 0, X, x_gs, 64, sc, sh, n, m, Lf, H, W, Cin, S, groups, tt, nt,
                                        addend, seg, ld_add, z, y_gs, 64, None, None)
 
     bad = [dict(mode=6), dict(mode=-1), dict(M=96), dict(M=0), dict(K=0), dict(X=None), dict(Wt=None),
-           dict(mode=NORM, sc=z), dict(addend=z), dict(addend=z, seg=zi, ld_add=0),
+           dict(mode=XM.NORM, sc=z), dict(addend=z), dict(addend=z, seg=zi, ld_add=0),
            dict(S=0), dict(groups=0), dict(tt=zi, nt=0), dict(tt=zi, nt=2, x_gs=64), dict(tt=zi, nt=2, y_gs=64),
-           dict(mode=MUL, n=0, m=8, Lf=8, S=0), dict(mode=ABS, n=2, m=4, Lf=5, S=8), dict(mode=SUB, n=2, m=4, Lf=6, S=9),
-           dict(mode=MUL, n=2, m=4, Lf=6, S=8, tt=zi, nt=1),
-           dict(mode=CONV, K=63, H=4, W=4, Cin=8, S=32), dict(mode=CONV, K=72, H=4, W=4, Cin=8, S=33),
-           dict(mode=CONV, K=72, H=4, W=4, Cin=8, S=32, groups=2), dict(mode=CONV, K=72, H=0, W=4, Cin=8, S=32),
-           dict(mode=CONV, K=72, H=4, W=4, Cin=8, S=32, x_gs=16), dict(mode=CONV, K=72, H=4, W=4, Cin=8, S=32, tt=zi, nt=1)]
+           dict(mode=XM.MUL, n=0, m=8, Lf=8, S=0), dict(mode=XM.ABS, n=2, m=4, Lf=5, S=8), dict(mode=XM.SUB, n=2, m=4, Lf=6, S=9),
+           dict(mode=XM.MUL, n=2, m=4, Lf=6, S=8, tt=zi, nt=1),
+           dict(mode=XM.CONV, K=63, H=4, W=4, Cin=8, S=32), dict(mode=XM.CONV, K=72, H=4, W=4, Cin=8, S=33),
+           dict(mode=XM.CONV, K=72, H=4, W=4, Cin=8, S=32, groups=2), dict(mode=XM.CONV, K=72, H=0, W=4, Cin=8, S=32),
+           dict(mode=XM.CONV, K=72, H=4, W=4, Cin=8, S=32, x_gs=16), dict(mode=XM.CONV, K=72, H=4, W=4, Cin=8, S=32, tt=zi, nt=1)]
     for kw in bad:
         assert call(**kw) == -1, kw
 
@@ -368,7 +324,7 @@ def build(c, g):
     K, M = c.K, c.M
     d = dict(sc=None, sh=None, tt=None, nt=0, addend=None, seg=None, ld_add=0, add=None, Cin=0)
     co = torch.arange(M)[:, None]
-    if c.mode == CONV:
+    if c.mode == XM.CONV:
         cin, hw = K // 9, c.H * c.W
         n_img = c.S // hw
         x = torch.randn(n_img, cin, c.H, c.W, generator=g).cuda()
@@ -378,7 +334,7 @@ def build(c, g):
         d["grp"] = torch.zeros(c.S, dtype=torch.long)
         d["tile_group"] = torch.zeros(-(-c.S // TN), dtype=torch.long)
         d["G"] = 1
-    elif c.mode in (MUL, ABS, SUB):
+    elif c.mode in (XM.MUL, XM.ABS, XM.SUB):
         f = torch.randn(c.groups, K, c.Lf, generator=g).cuda()
         d["X"], d["xin"] = f, pair_operand(f, c.mode, c.n, c.m)
     elif c.tiling == "uniform":
@@ -404,7 +360,7 @@ def build(c, g):
             d["addend"] = torch.randn(M, ndet, generator=g).cuda()
             d["seg"], d["ld_add"] = seg, ndet
             d["add"] = d["addend"][:, seg.long()]
-    if c.tiling == "uniform" and c.mode != CONV:
+    if c.tiling == "uniform" and c.mode != XM.CONV:
         G, S = c.groups, c.S
         d["G"] = G
         d["grp"] = torch.arange(G).repeat_interleave(S)
@@ -412,7 +368,7 @@ def build(c, g):
         gi, s = torch.arange(G)[:, None], torch.arange(S)[None]
         d["yidx"] = (gi * c.y_gs)[None] + co[:, :, None] * c.y_ms + s[None]
         d["yidx"] = d["yidx"].reshape(M, G * S)
-    if c.mode == NORM:
+    if c.mode == XM.NORM:
         G = d["G"]
         d["sc"] = (torch.randn(G, K, generator=g)).cuda()
         d["sh"] = (torch.randn(G, K, generator=g) * 0.5).cuda()
@@ -429,12 +385,12 @@ def test_simt_vs_fp64(c):
     bound of the module docstring; NaN-filled outputs: every owned element written, every other one untouched; the
     partials against fp64 statistics of the stored Y."""
     lib = _lib.load()
-    g = torch.Generator().manual_seed(_seed("simt", c.name))
+    g = torch.Generator().manual_seed(case_seed("simt", c.name))
     d = build(c, g)
     wt = (torch.randn(c.K, c.M, generator=g) * c.K ** -0.5).cuda()
     bias = (torch.randn(c.M, generator=g) * 0.5).cuda() if c.bias else None
     nt = d["nt"] if d["tt"] is not None else len(d["tile_group"])
-    Y = torch.full((d["ysize"] + GUARD,), float("nan"), device="cuda")
+    Y = nan_output(d["ysize"], guard=GUARD)
     part = torch.full((nt + 1, c.M, 2), float("nan"), dtype=torch.float64, device="cuda") if c.part else None
     rc = lib.mmmot_debug_simt_op(c.mode, c.M, c.K, vp(wt), vp(bias), int(c.relu), vp(d["X"]), c.x_gs, c.x_ks, vp(d["sc"]),
                                  vp(d["sh"]), c.n, c.m, c.Lf, c.H, c.W, d["Cin"], c.S, c.groups, vp(d["tt"]), d["nt"],
@@ -457,9 +413,9 @@ def test_simt_vs_fp64(c):
     if c.part:
         assert bool(torch.isfinite(part[:nt]).all()), "a partial was not written"
         assert bool(torch.isnan(part[nt:]).all()), "a partial past the last tile was written"
-        S1, S2 = _reduce_parts(part[:nt], d["tile_group"].cuda(), d["G"])
+        S1, S2 = reduce_parts(part[:nt], d["tile_group"].cuda(), d["G"])
         rv, rm, _ = stats_ratios(S1, S2, got.T.double(), d["grp"].cuda(), d["G"])
         stats = dict(var_err_over_bound=rv, mean_err_over_bound=rm)
-    _report(f"simt {c.name}", err_over_bound=ratio, **stats)
+    report(f"simt {c.name}", err_over_bound=ratio, **stats)
     assert ratio <= 1.0, ratio
     assert all(v <= 1.0 for v in stats.values()), stats

@@ -5,9 +5,9 @@ batch statistics, and w_det (XM_DIRECT, then XM_NORM_RELU) with its two BatchNor
 statistics are compared per channel, each against its own scale (|dmean| against the channel's mean |y|, |dvar|
 against its own variance), so a channel whose variance is far below the layer's largest is held as tightly as any.
 
-w_det: derived bound.  Layer 1's outputs carry at most T1, the contraction bound of test_simt_engine.py.  BatchNorm
-over n = 3L columns then gives, to first order and with the statistics bound of test_norm_stats.py for the fp32 runs
-of the partials and u for the export to fp32,
+w_det: derived bound.  Layer 1's outputs carry at most T1, the contraction bound of the FP32 engine
+(kernel_kit.contraction_bound).  BatchNorm over n = 3L columns then gives, to first order and with the statistics bound
+of kernel_kit.stats_ratios for the fp32 runs of the partials and u for the export to fp32,
     |dmean| <= mean(T) + KAPPA1 u mean|y| + u |mean|,
     |dvar|  <= 2 mean(|y - mean| T) + mean(T^2) + KAPPA u (|mean| mean|y - mean| + var) + u var,
 and the normalised, rectified output h = relu(gamma (y - mean) rstd + beta) carries
@@ -34,24 +34,17 @@ import torch
 import torch.nn.functional as F
 
 import mmmot_b200
+from kernel_kit import EPS, KAPPA, KAPPA1, U, case_seed, contraction_bound, eval_net, report, vp, worst_ratio
 from mmmot_b200 import _lib
 from mmmot_b200.synthetic import synthetic_pair, synthetic_state_dict
-from test_gen_engines import _report
-from test_norm_stats import KAPPA, KAPPA1, U, _seed
-from test_simt_engine import contraction_bound, worst_ratio
 
 gpu = pytest.mark.gpu
-vp = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-EPS = 1e-5
 TAU_MEAN, TAU_VAR = 2e-5, 6e-5     # measured worst: 1.1e-6 (mean, 64 px, L = 24), 3.0e-6 (var)
 
 
 def _net(seed=17):
-    sd = synthetic_state_dict("C", seed=seed)
-    net = mmmot_b200.TrackingNet(2, appear_skippool=True, score_arch="branch_cls", score_fusion_arch="C", test_mode=2,
-                                 dropblock=0)
-    net.load_state_dict(sd)
-    return net.cuda().eval(), {k: v.double().cuda() if v.is_floating_point() else v for k, v in sd.items()}
+    net, sd = eval_net("C", seed)
+    return net, {k: v.double().cuda() if v.is_floating_point() else v for k, v in sd.items()}
 
 
 def bn_propagate(y, T, gamma, beta):
@@ -107,7 +100,7 @@ def test_channel_tolerance_rejects_one_percent():
     rv = channel_ratios(mean, bad_v, mean, var, mabs)[1]
     rm = channel_ratios(bad_m, var, mean, var, mabs)[0]
     whole = float((bad_v - var).abs().max() / var.abs().max())
-    _report("tolerance check", var_1pct_over_tol=rv / TAU_VAR, mean_1pct_over_tol=rm / TAU_MEAN, whole_vector_relerr=whole)
+    report("tolerance check", var_1pct_over_tol=rv / TAU_VAR, mean_1pct_over_tol=rm / TAU_MEAN, whole_vector_relerr=whole)
     assert rv > 100 * TAU_VAR and rm > 100 * TAU_MEAN and whole < 1e-4
 
 
@@ -123,7 +116,7 @@ def test_w_det_train_vs_fp64(L):
     lib = _lib.load()
     net, sd = _net()
     wts = net.prepared()
-    g = torch.Generator().manual_seed(_seed("w_det train", L))
+    g = torch.Generator().manual_seed(case_seed("w_det train", L))
     feats = torch.randn(3, 512, L, generator=g).cuda()
     det = torch.full((3, L), float("nan"), device="cuda")
     bn = torch.full((2, 2, 512), float("nan"), device="cuda")
@@ -152,7 +145,7 @@ def test_w_det_train_vs_fp64(L):
              mean2=float(((bn[1, 0, :256].double() - m2).abs() / tm2).max()),
              var2=float(((bn[1, 1, :256].double() - v2).abs() / tv2).max()),
              logits=worst_ratio(got.reshape(-1), ref.reshape(-1), T3))
-    _report(f"w_det train L={L} (err / bound)", **r)
+    report(f"w_det train L={L} (err / bound)", **r)
     assert all(val <= 1.0 for val in r.values()), r
 
 
@@ -170,10 +163,10 @@ def test_appearance_train_vs_fp64(hw, L, drop, monkeypatch):
     lib = _lib.load()
     net, sd = _net()
     wts = net.prepared()
-    crops = synthetic_pair(L // 2, L - L // 2, 16, hw, seed=_seed("app", hw, L) % 1000)[0].float().cuda()
+    crops = synthetic_pair(L // 2, L - L // 2, 16, hw, seed=case_seed("app", hw, L) % 1000)[0].float().cuda()
     dm2 = dm3 = None
     if drop:
-        torch.manual_seed(_seed("drop", hw, L))
+        torch.manual_seed(case_seed("drop", hw, L))
         dm2 = net._dropblock_weights(L, hw // 16, hw // 16, drop).cuda()
         dm3 = net._dropblock_weights(L, hw // 32, hw // 32, drop).cuda()
     feats = torch.full((1, 3, 512, L), float("nan"), device="cuda")
@@ -186,7 +179,7 @@ def test_appearance_train_vs_fp64(hw, L, drop, monkeypatch):
     stats, mabs = {}, {}
     _record_mean_abs(monkeypatch, mabs)
     if drop:
-        torch.manual_seed(_seed("drop", hw, L))
+        torch.manual_seed(case_seed("drop", hw, L))
     ref = train_ref.appearance_train(sd, crops.double(), stats, drop)
     worst_m = worst_v = 0.0
     per_layer = {}
@@ -196,11 +189,11 @@ def test_appearance_train_vs_fp64(hw, L, drop, monkeypatch):
         rm, rv = channel_ratios(bn[i, 0, :C].double(), bn[i, 1, :C].double(), m, v, mabs[p])
         per_layer[f"L{i}"] = max(rm / TAU_MEAN, rv / TAU_VAR)
         worst_m, worst_v = max(worst_m, rm), max(worst_v, rv)
-    report = []
-    check_close(feats[0, 0], ref.T, TOL, "stack 0", report)
-    _report(f"appearance train {hw}px L={L} dropblock={drop}", mean_rel=worst_m, var_rel=worst_v,
-            stack0_err=report[0][1], stack0_worst=report[0][3])
-    _report("  per layer (worst ratio to tolerance)", **per_layer)
+    rep = []
+    check_close(feats[0, 0], ref.T, TOL, "stack 0", rep)
+    report(f"appearance train {hw}px L={L} dropblock={drop}", mean_rel=worst_m, var_rel=worst_v,
+           stack0_err=rep[0][1], stack0_worst=rep[0][3])
+    report("  per layer (worst ratio to tolerance)", **per_layer)
     assert worst_m <= TAU_MEAN and worst_v <= TAU_VAR, per_layer
 
 
@@ -218,7 +211,7 @@ def test_pointnet_train_vs_fp64(L, mask, monkeypatch):
     lib = _lib.load()
     net, sd = _net()
     wts = net.prepared()
-    g = torch.Generator().manual_seed(_seed("pointnet train", L, mask))
+    g = torch.Generator().manual_seed(case_seed("pointnet train", L, mask))
     cnt = torch.randint(1, 1024, (L,), generator=g)
     cnt[[0, L // 2, L - 1]] = 1
     split = torch.zeros(L + 1, dtype=torch.int32)
@@ -228,7 +221,7 @@ def test_pointnet_train_vs_fp64(L, mask, monkeypatch):
     points = (torch.randn(P, 3, generator=g) * torch.tensor([2.0, 1.0, 0.8]) + centre.repeat_interleave(cnt, 0)).cuda()
     hmask = None
     if mask:
-        torch.manual_seed(_seed("head mask", L))
+        torch.manual_seed(case_seed("head mask", L))
         hmask = F.dropout(torch.ones(512, P, device="cuda"), p=0.5, training=True)
     feats = torch.full((1, 3, 512, L), float("nan"), device="cuda")
     ws = torch.empty(int(lib.mmmot_pointnet_train_workspace(1, L, P)), dtype=torch.uint8, device="cuda")
@@ -242,9 +235,9 @@ def test_pointnet_train_vs_fp64(L, mask, monkeypatch):
         monkeypatch.setattr(F, "dropout", lambda x, p=0.5, training=True: x * m64)
     ref = torch_ref.pointnet(sd, points.double().T[None], split.long().cuda(), dropout=mask)[0]
     assert bool(torch.isfinite(feats[0, 1]).all())
-    report = []
-    check_close(feats[0, 1], ref.T, TOL, "stack 1", report)
-    _report(f"pointnet train L={L} P={P} mask={mask}", err=report[0][1], outside=report[0][2], worst=report[0][3])
+    rep = []
+    check_close(feats[0, 1], ref.T, TOL, "stack 1", rep)
+    report(f"pointnet train L={L} P={P} mask={mask}", err=rep[0][1], outside=rep[0][2], worst=rep[0][3])
 
 
 # running-average update: per-layer count L h w (VGG) or 3 L (w_det), unbiased factor count / (count - 1), momentum 0.1
@@ -267,7 +260,7 @@ def test_running_averages_vs_fp64(hw, n, m, monkeypatch):
                                  dropblock=0, use_dropout=False)
     net.load_state_dict(sd0)
     net.cuda().train()
-    dets, info, split = synthetic_pair(n, m, 64, hw, seed=_seed("running", hw) % 1000, ragged=True)
+    dets, info, split = synthetic_pair(n, m, 64, hw, seed=case_seed("running", hw) % 1000, ragged=True)
     net(dets.cuda(), {k: v.cuda() for k, v in info.items()}, split)
     torch.cuda.synchronize()
     after = net.state_dict()
@@ -291,5 +284,5 @@ def test_running_averages_vs_fp64(hw, n, m, monkeypatch):
         rv = float(((after[p + ".running_var"].double() - run[p + ".running_var"]).abs() / bv).max())
         worst[p] = max(rm, rv)
         assert int(after[p + ".num_batches_tracked"]) == int(sd0[p + ".num_batches_tracked"]) + 1, p
-    _report(f"running averages {hw}px L={n + m} (err / bound)", **{p.replace("appearance.layers.", "vgg"): v for p, v in worst.items()})
+    report(f"running averages {hw}px L={n + m} (err / bound)", **{p.replace("appearance.layers.", "vgg"): v for p, v in worst.items()})
     assert max(worst.values()) <= 1.0, worst

@@ -20,7 +20,8 @@ for K in (512, 1152, 2304, 4608):
         for eng in (1, 2):
             if eng == 1:
                 Y = torch.zeros(M, S, device="cuda")
-                lib.mmmot_debug_linear(vp(Wt.cuda()), None, 0.0, None, vp(X.cuda()), vp(Y), M, K, S, 1, None)
+                lib.mmmot_debug_simt_op(0, M, K, vp(Wt.cuda()), None, 0, vp(X.cuda()), 0, S, None, None, 0, 0, 0, 0, 0, 0, S, 1,
+                                        None, 0, None, None, 0, vp(Y), 0, S, None, None)
             else:       # TMA-fed tensor-core engine: channels-last FP16 hi/lo planes in, Y[S][M] out
                 Xc = X.t().contiguous()
                 hi = Xc.half()

@@ -53,12 +53,14 @@ for (n, H, W, C, M) in CONVS:
     Yp = torch.zeros(2, n, H, W, M, dtype=torch.half, device="cuda")
     Wp_d, b_d = Wp.cuda(), b.cuda()
     scr = torch.zeros((n + 16) * H * W * M + 256 * M, device="cuda")
+    conv = lambda sp: lib.mmmot_debug_conv_layer(vp(Wp_d), None, wps, vp(b_d), vp(Xp), n * H * W * C, n, H, W, C, M, vp(Yp),
+                                                 n * H * W * M, 0, None, None, sp, None, None, None)
     for seg, sp in (("1pass", None), ("kseg", vp(scr))):
-        rc = lib.mmmot_debug_conv_planar(vp(Wp_d), wps, vp(b_d), vp(Xp), vp(Yp), n, H, W, C, M, sp, None)
+        rc = conv(sp)
         torch.cuda.synchronize()
         t0 = time.time()
         for _ in range(3):
-            lib.mmmot_debug_conv_planar(vp(Wp_d), wps, vp(b_d), vp(Xp), vp(Yp), n, H, W, C, M, sp, None)
+            conv(sp)
         torch.cuda.synchronize()
         dt = (time.time() - t0) / 3
         if ref is not None:
