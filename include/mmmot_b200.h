@@ -239,6 +239,27 @@ int mmmot_lp_assign(const float* det, long det_stride, const float* link, long l
                     void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Association integer programme of samples of K >= 2 frames (reference solvers.py:9-138 for any len(det_split)),
+ * solved exactly as a min-cost flow (csrc/flow_assign.cu).  All samples share the frame counts.
+ *   counts [frames] (HOST): detections per frame, n_0 .. n_{K-1};  L = sum of counts
+ *   det, new_s, end_s [samples][L] (zero-padded like the reference's forward output), links [samples][..]: one
+ *   sample's link matrices back to back, [n0][n1], then [n1][n2], ...; strides in floats between samples.
+ *   outputs (fp32 0/1, same layout as solvers.py:116-131):
+ *   a_det, a_new, a_end [samples][L], a_links [samples][..] packed like links (dense between samples)
+ *   match [samples][L - n_{K-1}] int32: each non-last-frame detection's successor index in the next frame, or -1.
+ * MMMOT_E_ARG, before any CUDA call, for null pointers, samples <= 0, frames < 2 or a count <= 0; MMMOT_E_SHAPE for
+ * frames > 64 or an L whose solver state does not fit one SM's shared memory (L > 4469).  Run time grows about as L^3:
+ * one sample of dense random scores took 14 s at L = 2048 and 116 s at L = 4469 in a single launch on an H100 80GB HBM3
+ * (700 W, 1980 MHz; profiles/flow_times_cap.json), against 2.6 s for 128 samples of L = 1024.
+ */
+size_t mmmot_flow_workspace(int samples, int frames, const int* counts);
+int mmmot_flow_assign(const float* det, long det_stride, const float* links, long links_stride,
+                      const float* new_s, long new_stride, const float* end_s, long end_stride,
+                      int samples, int frames, const int* counts,
+                      float* a_det, float* a_links, float* a_new, float* a_end, int* match,
+                      void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Per-detection LiDAR cropping (SURVEY.md 8f row N1 — the step right before the hot path).
  * Replaces the host loop of reference point_cloud/preprocess.py:72-81 / box_np_ops.py:688-699 /
  * geometry.py:96-114.  planes[n_boxes][6][4]: inward plane equations (nx, ny, nz, d) of each rotated box,

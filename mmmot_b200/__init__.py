@@ -1,7 +1,7 @@
 """mmmot_b200 — CUDA-native (sm_90a, H100) implementation of mmMOT's per-frame-pair association
 forward behind the reference's own Python surface.  See DESIGN.md."""
 from .config import build_model, model_kwargs  # noqa: F401
-from .solvers import ortools_solve, solve_batch  # noqa: F401
+from .solvers import ortools_solve, solve_batch, solve_frames  # noqa: F401
 from .tracking_net import TrackingNet  # noqa: F401
 from .lidar_crop import box_camera_to_lidar, box_planes, crop_points, prep_points, prep_points_batch  # noqa: F401
 from .image_crop import crop_boxes, crop_resize  # noqa: F401

@@ -105,6 +105,9 @@ SIGNATURES = {
     "mmmot_crop_resize": (_i, [_vp, _i, _i, _vp, _vp, _i, _l, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "mmmot_lp_workspace": (_sz, [_i, _i, _i]),
     "mmmot_lp_assign": (_i, [_vp, _l, _vp, _l, _vp, _l, _vp, _l, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "mmmot_flow_workspace": (_sz, [_i, _i, ctypes.POINTER(_i)]),
+    "mmmot_flow_assign": (_i, [_vp, _l, _vp, _l, _vp, _l, _vp, _l, _i, _i, ctypes.POINTER(_i), _vp, _vp, _vp, _vp, _vp,
+                               _vp, _sz, _vp]),
 }
 
 _lib = None

@@ -91,7 +91,7 @@ const char* const kTagNames[MM_T_COUNT] = {
     "pointnet.head_64to512_segsum",
     "affinity.l1_pair_512to1024", "affinity.newend_means", "affinity.l2_512to512", "affinity.l3_512to128",
     "affinity.logit", "lp.assign", "pointnet.moments_128", "pointnet.moments_64",
-    "pointnet.moments_finalize"};
+    "pointnet.moments_finalize", "lp.flow"};
 }  // namespace
 
 bool mm_timing_on() { return g_timing; }

@@ -43,7 +43,8 @@ enum {
   MM_T_LP = 28,
   MM_T_PN_MOM128 = 29, MM_T_PN_MOM64 = 30,   // input moments of layer 5 and of the head (their GroupNorm statistics)
   MM_T_PN_MOMFIN = 31,                       // their slice tables, fixed-order reductions and fp64 statistics
-  MM_T_COUNT = 32
+  MM_T_FLOW = 32,         // association programme of K-frame samples (min-cost flow)
+  MM_T_COUNT = 33
 };
 bool mm_timing_on();
 void mm_timing_begin(cudaStream_t st, int tag, double flop, double bytes);

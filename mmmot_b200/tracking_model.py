@@ -99,11 +99,18 @@ class TrackingModule(object):
     # ------------------------------------------------------------------ predict
     @torch.no_grad()
     def predict(self, det_imgs, det_info, dets, det_split):
-        """tracking_model.py:68-81: forward -> assignment programme on the ``test_mode`` stack -> ids."""
+        """tracking_model.py:68-81: forward -> assignment programme on the ``test_mode`` stack -> ids.
+
+        Samples of K > 2 frames pass every transition's link matrix to the programme.  (The reference passes only
+        ``link_score[0]`` and fails there with a KeyError, solvers.py:91.)"""
         det_score, link_score, new_score, end_score, _ = self.model(det_imgs, det_info, det_split)
         t = self.test_mode
-        assign_det, assign_link, assign_new, assign_end = ortools_solve(
-            det_score[t], [link_score[0][t:t + 1]], new_score[t], end_score[t], det_split)
+        if len(det_split) == 2:
+            assign_det, assign_link, assign_new, assign_end = ortools_solve(
+                det_score[t], [link_score[0][t:t + 1]], new_score[t], end_score[t], det_split)
+        else:
+            assign_det, assign_link, assign_new, assign_end = ortools_solve(
+                det_score[t], [l[t:t + 1] for l in link_score], new_score[t], end_score[t], det_split)
         ids, boxes = self.assign_det_id(assign_det, assign_link, assign_new, assign_end, det_split, dets)
         return self.align_id(ids, boxes)
 

@@ -416,8 +416,8 @@ class TrackingNet(nn.Module):
     def _forward_multi(self, dets, det_info, splits):
         """Samples of more than two frames (reference modules/tracking_net.py:170-182; sample_max_len > 2): the feature
         stages run once over all L detections of the sample (one GroupNorm domain, exactly like the reference), then
-        ``associate`` runs on every pair of consecutive frames.  (The association programme of such samples is a
-        min-cost flow; mmmot_b200.ortools_solve handles two-frame samples only.)"""
+        ``associate`` runs on every pair of consecutive frames.  (mmmot_b200.ortools_solve solves the association
+        programme of such samples as a min-cost flow.)"""
         lib = _lib.load()
         wts = self.prepared()
         dev = wts.flat.device

@@ -1,8 +1,8 @@
 """Small runs of every device path for compute-sanitizer (memcheck / racecheck): eval forward + LP on both engines
 (N=M=8, 32x32 crops; the tensor-core engine forced so that its kernels, incl. the first layer's in-kernel operand
-producers, are the ones checked), all fusion / softmax / affinity variants, end_mode max, a three-frame sample, the
-training-mode forward with DropBlock + Dropout, the pinned-host pipeline, LiDAR cropping in both precisions and image
-crop-and-resize.
+producers, are the ones checked), all fusion / softmax / affinity variants, end_mode max, a three-frame sample and its
+assignment programme, the training-mode forward with DropBlock + Dropout, the pinned-host pipeline, LiDAR cropping in
+both precisions and image crop-and-resize.
   compute-sanitizer --tool memcheck  python tools/sanitize_small.py
   compute-sanitizer --tool racecheck python tools/sanitize_small.py"""
 import os, sys
@@ -37,6 +37,8 @@ net = make("C", "minus_abs", "dual_add", seq=3, end_mode="max")
 dets, info, _ = synthetic_pair(5, 11, 24, 32, seed=61, ragged=True)
 o = net(dets.cuda(), {k: v.cuda() for k, v in info.items()}, [torch.tensor([5]), torch.tensor([7]), torch.tensor([4])])
 print("multi-frame link shapes", [tuple(l.shape) for l in o[1]])
+a = mmmot_b200.ortools_solve(o[0][2], [l[2:3] for l in o[1]], o[2][2], o[3][2], [5, 7, 4])
+print("multi-frame assignment kept", int(a[0].sum()))
 
 # training-mode forward with DropBlock / Dropout
 net = make("C", "minus_abs", "dual_add", dropblock=5, use_dropout=True).train()
