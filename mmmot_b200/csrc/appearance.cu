@@ -1,8 +1,12 @@
-// Appearance branch: VGG16-BN trunk (BN folded) + 4 SkipPool heads.
+// Appearance branch: VGG16-BN trunk + 4 SkipPool heads.
 // Replaces reference modules/appear_net.py:166-190 (vgg_forward + SkipPool.forward :27-32).
+// Eval mode (mmmot_appearance_fwd) folds BatchNorm into the convolutions.  Training mode (mmmot_appearance_train_fwd,
+// SURVEY.md 8f row N4) runs the FP32 trunk with the unfolded weights and normalises every conv with the statistics of
+// the current batch (modules/vgg.py:67-80 under .train()), which it returns for the host's running-average update.
 #include <cuda_fp16.h>
 
 #include "gemm_tma.cuh"
+#include "norm_ops.cuh"
 
 namespace {
 
@@ -31,17 +35,29 @@ __global__ void maxpool2_kernel(const float* __restrict__ in, float* __restrict_
 }
 
 // Global average pool of every (img, channel) plane: one warp per plane.
-__global__ void plane_mean_kernel(const float* __restrict__ in, float* __restrict__ out, long planes,
-                                  int hw) {
+// mask (optional, training): DropBlock weights [img][hw] = block_mask * numel / sum (modules/dropblock.py:49-53),
+// applied before the SkipPool head's average pool (modules/appear_net.py:27-30); C = channels per image
+__global__ void plane_mean_kernel(const float* __restrict__ in, float* __restrict__ out, long planes, int hw,
+                                  const float* __restrict__ mask, int C) {
   long w = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int lane = threadIdx.x & 31;
   if (w >= planes) return;
   const float* src = in + w * hw;
+  const float* mk = mask ? mask + (w / C) * hw : nullptr;
   float s = 0.f;
-  for (int i = lane; i < hw; i += 32) s += src[i];
+  for (int i = lane; i < hw; i += 32) s += mk ? src[i] * mk[i] : src[i];
 #pragma unroll
   for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) out[w] = s / (float)hw;
+}
+
+// training-mode BatchNorm + ReLU: y[img][c][hw] = relu(y*sc[c] + sh[c]) in place
+__global__ void bn_relu_kernel(float* __restrict__ y, const float* __restrict__ sc, const float* __restrict__ sh, int C,
+                               int hw, long n) {
+  long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  const int c = (int)((idx / hw) % C);
+  y[idx] = fmaxf(fmaf(y[idx], sc[c], sh[c]), 0.f);
 }
 
 // ---- FP16 hi/lo planes, NHWC: activations of the tensor-core trunk ([2][n][H][W][C]) ----
@@ -301,6 +317,100 @@ static int vgg_conv0_launch(const float* crops, int n_img, int H, int W, const f
   return 0;
 }
 
+// What the FP32 trunk needs in training mode: the BatchNorm scratch, where the batch statistics go, and the DropBlock
+// weights of the two deepest skip maps
+struct VggTrain {
+  double2* part;              // per-tile (sum, sumsq) partials of one conv
+  double* stats;              // their fixed-order per-channel reduction
+  float *sc, *sh;             // per-channel affine
+  float* bn_stats;            // [13][2][512]: batch mean | biased batch variance of every conv
+  const float* drop_mask[2];  // DropBlock weights [img][hw] of skip maps 2 and 3 (optional)
+};
+
+// The appearance stage's workspace: the two activation buffers and the pooled skip maps, then the tensor-core trunk's
+// scratch (eval) or the BatchNorm scratch (training)
+struct AppWs {
+  float* buf[2];
+  float* pooled[4];
+  float* kseg_scratch;            // K-segment partial sums, tile order (largest: 256 ch at H/4 x W/4)
+  unsigned long long* pool_sum;   // per-image sums of a pooled skip map (fused pool epilogue)
+  VggTrain tr;
+};
+AppWs carve_appearance(MmArena& a, int n_img, int H, int W, bool train) {
+  AppWs w = {};
+  const size_t act = (size_t)n_img * 64 * H * W;
+  w.buf[0] = a.take<float>(act);
+  w.buf[1] = a.take<float>(act);
+  for (int s = 0; s < 4; s++) w.pooled[s] = a.take<float>((size_t)n_img * kSkipC[s]);
+  if (train) {
+    w.tr.sc = a.take<float>(512);
+    w.tr.sh = a.take<float>(512);
+    w.tr.stats = a.take<double>(512 * 2);
+    w.tr.part = a.take<double2>((size_t)mm_cdiv((long)n_img * H * W, 128) * 64);   // tiles x channels: largest at conv 0/1
+  } else {
+    w.kseg_scratch = a.take<float>((size_t)(n_img + 16) * H * W * 16);
+    w.pool_sum = a.take<unsigned long long>((size_t)n_img * 512);
+  }
+  return w;
+}
+
+// The VGG trunk on the FP32 FFMA engine: fp32 NCHW activations in buf[0] / buf[1], the skip maps' global averages into
+// pooled[s].  Eval (tr == nullptr): BatchNorm folded into the weights, ReLU in the conv's epilogue, every conv timed.
+// Training: the conv with the unfolded weights, then BatchNorm2d on the statistics over (batch, H, W) (biased variance,
+// eps 1e-5) and ReLU in place; the DropBlock weights scale skip maps 2 and 3 before their average.
+int vgg_fp32_trunk(const mmmot_weights* wts, const float* crops, int n_img, int H, int W, float* const* buf,
+                   float* const* pooled, const VggTrain* tr, cudaStream_t st) {
+  const float* cur = crops;
+  int which = 0, h = H, w = W;
+  const bool timed = !tr && mm_timing_on();
+  for (int i = 0; i < 13; i++) {
+    GemmP p = gemm_defaults();
+    p.Wt = wts->w[(tr ? MMMOT_W_VGG_RAWW0 : MMMOT_W_VGG_WT0) + i];
+    p.bias = wts->w[(tr ? MMMOT_W_VGG_RAWB0 : MMMOT_W_VGG_B0) + i];
+    p.ldw = kVggCout[i];
+    p.M = kVggCout[i];
+    p.K = 9 * kVggCin[i];
+    p.Cin = kVggCin[i];
+    p.H = h; p.W = w;
+    p.S = n_img * h * w;
+    p.X = cur;
+    p.Y = buf[which];
+    p.relu = !tr;
+    p.part = tr ? tr->part : nullptr;
+    p.tiles_per_group = mm_cdiv(p.S, 128);
+    p.num_tiles = p.tiles_per_group;
+    if (timed) mm_timing_begin(st, MM_T_VGG0 + i, 2.0 * p.M * (double)p.K * (double)p.S, 4.0 * (double)p.S * (p.Cin + p.M));
+    MM_TRY(gemm_simt_launch<XM_CONV3>(p, st));
+    if (timed) mm_timing_end(st);
+    if (tr) {
+      MM_TRY(stats_reduce(tr->part, p.M, 1, p.num_tiles, nullptr, tr->stats, st));
+      MM_TRY(gn_finalize(tr->stats, wts->w[MMMOT_W_VGG_BNW0 + i], wts->w[MMMOT_W_VGG_BNB0 + i], nullptr, p.S, 1, p.M, 1,
+                         tr->sc, tr->sh, st));
+      bn_export_kernel<<<mm_cdiv(p.M, 128), 128, 0, st>>>(tr->stats, p.M, (double)p.S, tr->bn_stats + (long)i * 1024);
+      MM_LAUNCH_CHECK();
+      const long n = (long)p.S * p.M;
+      bn_relu_kernel<<<mm_cdiv(n, 256), 256, 0, st>>>(buf[which], tr->sc, tr->sh, p.M, h * w, n);
+      MM_LAUNCH_CHECK();
+    }
+    cur = buf[which]; which ^= 1;
+    if (kPoolAfter[i]) {
+      h /= 2; w /= 2;
+      long n_out = (long)n_img * kVggCout[i] * h * w;
+      maxpool2_kernel<<<mm_cdiv(n_out, 256), 256, 0, st>>>(cur, buf[which], n_out, h, w);
+      MM_LAUNCH_CHECK();
+      cur = buf[which]; which ^= 1;
+      int s = kSkipAfter[i];
+      if (s >= 0) {
+        long planes = (long)n_img * kSkipC[s];
+        const float* mask = tr && s >= 2 ? tr->drop_mask[s - 2] : nullptr;
+        plane_mean_kernel<<<mm_cdiv(planes * 32, 256), 256, 0, st>>>(cur, pooled[s], planes, h * w, mask, kSkipC[s]);
+        MM_LAUNCH_CHECK();
+      }
+    }
+  }
+  return 0;
+}
+
 }  // namespace
 
 // Test hook: the first VGG layer exactly as mmmot_appearance_fwd runs it (vgg_conv0_launch).
@@ -316,12 +426,13 @@ int mm_launch_skip_heads(const mmmot_weights* wts, float* const* pooled, int n_i
 
 extern "C" size_t mmmot_appearance_workspace(int n_img, int H, int W) {
   MmArena a(nullptr, 0);
-  size_t act = (size_t)n_img * 64 * H * W;
-  a.take<float>(act);
-  a.take<float>(act);
-  for (int s = 0; s < 4; s++) a.take<float>((size_t)n_img * kSkipC[s]);
-  a.take<float>((size_t)(n_img + 16) * H * W * 16);   // K-segment partial sums, tile order (largest: 256 ch at H/4 x W/4)
-  a.take<unsigned long long>((size_t)n_img * 512);     // per-image sums of a pooled skip map (fused pool epilogue)
+  carve_appearance(a, n_img, H, W, false);
+  return a.off;
+}
+
+extern "C" size_t mmmot_appearance_train_workspace(int n_img, int H, int W) {
+  MmArena a(nullptr, 0);
+  carve_appearance(a, n_img, H, W, true);
   return a.off;
 }
 
@@ -332,12 +443,7 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
   if (H % 32 || W % 32 || H <= 0 || W <= 0 || n_img % L) return MMMOT_E_SHAPE;
   cudaStream_t st = (cudaStream_t)stream;
   MmArena ar(workspace, workspace_bytes);
-  size_t act = (size_t)n_img * 64 * H * W;
-  float* buf[2] = {ar.take<float>(act), ar.take<float>(act)};
-  float* pooled[4];
-  for (int s = 0; s < 4; s++) pooled[s] = ar.take<float>((size_t)n_img * kSkipC[s]);
-  float* kseg_scratch = ar.take<float>((size_t)(n_img + 16) * H * W * 16);
-  unsigned long long* pool_sum = ar.take<unsigned long long>((size_t)n_img * 512);
+  AppWs ws = carve_appearance(ar, n_img, H, W, false);
   if (!ar.ok()) return MMMOT_E_WORKSPACE;
 
   // Tensor-core trunk: activations live as FP16 hi/lo NHWC planes between layers; the epilogue of one conv
@@ -346,7 +452,7 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
   // take the same path and stay bit-identical
   const bool tc_trunk = mm_engine() == 2 || (mm_engine() == 0 && (long)L * H * W >= 32768);
   if (tc_trunk) {
-    __half* hb[2] = {reinterpret_cast<__half*>(buf[0]), reinterpret_cast<__half*>(buf[1])};
+    __half* hb[2] = {reinterpret_cast<__half*>(ws.buf[0]), reinterpret_cast<__half*>(ws.buf[1])};
     const __half* cur = nullptr;
     long cur_plane = 0;
     int which = 0, h = H, w = W;
@@ -374,11 +480,11 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
         // a pooled layer asks for the 2x2 max-pool to be fused into the epilogue; a skip map's global average (SkipPool)
         // rides along as per-image fixed-point sums
         const bool skip_layer = kPoolAfter[i] && kSkipAfter[i] >= 0;
-        if (skip_layer) MM_CUDA(cudaMemsetAsync(pool_sum, 0, (size_t)n_img * cout * sizeof(unsigned long long), st));
+        if (skip_layer) MM_CUDA(cudaMemsetAsync(ws.pool_sum, 0, (size_t)n_img * cout * sizeof(unsigned long long), st));
         MM_TRY(gemm_tma_launch_conv(p, (const uint4*)wts->w[MMMOT_W_VGG_WP0 + i], wts->tc_scale[MMMOT_W_VGG_WP0 + i], cur,
-                                    cur_plane, n_img, h, w, cin, hb[which], plane_out, st, kseg_scratch,
+                                    cur_plane, n_img, h, w, cin, hb[which], plane_out, st, ws.kseg_scratch,
                                     kPoolAfter[i] ? plane_out / 4 : 0, &pooled_in_epilogue, status,
-                                    skip_layer ? pool_sum : nullptr, i == 1 ? (const uint4*)wts->w[MMMOT_W_VGG_WPX0 + 1] : nullptr));
+                                    skip_layer ? ws.pool_sum : nullptr, i == 1 ? (const uint4*)wts->w[MMMOT_W_VGG_WPX0 + 1] : nullptr));
       }
       if (timed) mm_timing_end(st);
       cur = hb[which]; cur_plane = plane_out; which ^= 1;
@@ -399,10 +505,10 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
         int s = kSkipAfter[i];
         if (s >= 0 && pooled_in_epilogue && i > 1) {
           const long nn = (long)n_img * kSkipC[s];
-          pool_sum_mean_kernel<<<mm_cdiv(nn, 256), 256, 0, st>>>(pool_sum, pooled[s], nn, 1.0f / (float)(h * w));
+          pool_sum_mean_kernel<<<mm_cdiv(nn, 256), 256, 0, st>>>(ws.pool_sum, ws.pooled[s], nn, 1.0f / (float)(h * w));
           MM_LAUNCH_CHECK();
         } else if (s >= 0) {
-          plane_mean_planar_kernel<<<mm_cdiv((long)n_img * kSkipC[s], 128), 128, 0, st>>>(cur, pooled[s], n_img, h * w,
+          plane_mean_planar_kernel<<<mm_cdiv((long)n_img * kSkipC[s], 128), 128, 0, st>>>(cur, ws.pooled[s], n_img, h * w,
                                                                                          kSkipC[s], cur_plane);
           MM_LAUNCH_CHECK();
         }
@@ -410,47 +516,30 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
       }
     }
   } else {
-  const float* cur = crops;
-  int which = 0, h = H, w = W;
-  for (int i = 0; i < 13; i++) {
-    GemmP p = gemm_defaults();
-    p.Wt = wts->w[MMMOT_W_VGG_WT0 + i];
-    p.bias = wts->w[MMMOT_W_VGG_B0 + i];
-    p.ldw = kVggCout[i];
-    p.M = kVggCout[i];
-    p.K = 9 * kVggCin[i];
-    p.Cin = kVggCin[i];
-    p.H = h; p.W = w;
-    p.S = n_img * h * w;
-    p.X = cur;
-    p.Y = buf[which];
-    p.relu = 1;
-    p.tiles_per_group = mm_cdiv(p.S, 128);
-    p.num_tiles = p.tiles_per_group;
-    const bool timed = mm_timing_on();
-    if (timed) mm_timing_begin(st, MM_T_VGG0 + i, 2.0 * p.M * (double)p.K * (double)p.S, 4.0 * (double)p.S * (p.Cin + p.M));
-    MM_TRY(gemm_simt_launch<XM_CONV3>(p, st));
-    if (timed) mm_timing_end(st);
-    cur = buf[which]; which ^= 1;
-    if (kPoolAfter[i]) {
-      h /= 2; w /= 2;
-      long n_out = (long)n_img * kVggCout[i] * h * w;
-      maxpool2_kernel<<<mm_cdiv(n_out, 256), 256, 0, st>>>(cur, buf[which], n_out, h, w);
-      MM_LAUNCH_CHECK();
-      cur = buf[which]; which ^= 1;
-      int s = kSkipAfter[i];
-      if (s >= 0) {
-        long planes = (long)n_img * kSkipC[s];
-        plane_mean_kernel<<<mm_cdiv(planes * 32, 256), 256, 0, st>>>(cur, pooled[s], planes, h * w);
-        MM_LAUNCH_CHECK();
-      }
-    }
+    MM_TRY(vgg_fp32_trunk(wts, crops, n_img, H, W, ws.buf, ws.pooled, nullptr, st));
   }
-  }
-  return mm_launch_skip_heads(wts, pooled, n_img, L, feats, st);
+  return mm_launch_skip_heads(wts, ws.pooled, n_img, L, feats, st);
 }
 
-// the four SkipPool heads on the pooled maps -> stack 0 of feats (shared with the training-mode variant, train.cu); a NULL
+extern "C" int mmmot_appearance_train_fwd(const mmmot_weights* wts, const float* crops, int n_img, int H, int W, int L,
+                                          float* feats, float* bn_stats, const float* drop_mask2,
+                                          const float* drop_mask3, void* workspace, size_t workspace_bytes,
+                                          void* stream) {
+  if (!wts || !crops || !feats || !bn_stats || !workspace || n_img <= 0 || L <= 0) return MMMOT_E_ARG;
+  if (H % 32 || W % 32 || H <= 0 || W <= 0 || n_img % L) return MMMOT_E_SHAPE;
+  if (!wts->w[MMMOT_W_VGG_RAWW0]) return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  MmArena ar(workspace, workspace_bytes);
+  AppWs ws = carve_appearance(ar, n_img, H, W, true);
+  if (!ar.ok()) return MMMOT_E_WORKSPACE;
+  ws.tr.bn_stats = bn_stats;
+  ws.tr.drop_mask[0] = drop_mask2;
+  ws.tr.drop_mask[1] = drop_mask3;
+  MM_TRY(vgg_fp32_trunk(wts, crops, n_img, H, W, ws.buf, ws.pooled, &ws.tr, st));
+  return mm_launch_skip_heads(wts, ws.pooled, n_img, L, feats, st);
+}
+
+// the four SkipPool heads on the pooled maps -> stack 0 of feats (eval and training mode); a NULL
 // map skips its head (mmmot_debug_skip_heads)
 int mm_launch_skip_heads(const mmmot_weights* wts, float* const* pooled, int n_img, int L, float* feats, cudaStream_t st) {
   for (int s = 0; s < 4; s++) {

@@ -84,3 +84,15 @@ static inline int gn_finalize(const double* stats, const float* gamma, const flo
   MM_LAUNCH_CHECK();
   return 0;
 }
+
+// BatchNorm in training mode, for the host's running-average update: stats[c] = (sum, sumsq) over `count` values ->
+// out[c] = batch mean, out[512 + c] = biased batch variance
+static __global__ void bn_export_kernel(const double* __restrict__ stats, int C, double count, float* __restrict__ out) {
+  int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double mean = stats[2 * c] / count;
+  double var = stats[2 * c + 1] / count - mean * mean;
+  if (var < 0.0) var = 0.0;
+  out[c] = (float)mean;
+  out[512 + c] = (float)var;
+}

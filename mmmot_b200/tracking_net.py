@@ -25,6 +25,10 @@ VGG_POOLED_BEFORE = [idx in VGG_POOL_AFTER[s] for s, stage in enumerate(VGG_STAG
 from .weights import DeviceWeights
 
 
+def _vp(t):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
 class _Holder(nn.Module):
     """Empty module used to build the reference's parameter tree (names only)."""
 
@@ -98,9 +102,6 @@ class TrackingNet(nn.Module):
         self.chunk_pairs = None             # None: pick from free memory
 
     # ------------------------------------------------------------------ weights
-    def _invalidate(self, *a, **k):
-        self._prepared = None
-
     def load_state_dict(self, *a, **k):
         self._prepared = None
         return super().load_state_dict(*a, **k)
@@ -156,36 +157,72 @@ class TrackingNet(nn.Module):
         return self._ws
 
     # ------------------------------------------------------------------ core
-    def _run_chunk(self, lib, wts, crops, points, split_dev, split_host, pairs, n, m, out, p0):
-        """One chunk of `pairs` frame-pairs through the five C-ABI stages on the current stream."""
-        dev = crops.device
-        L = n + m
+    def _workspace_bytes(self, pairs, transitions, L=0, P=0, H=0, W=0):
+        """Workspace of one call on `pairs` samples: the affinity stage on every (n, m) of `transitions` and, when L > 0,
+        the feature stages on L detections, P points and H x W crops (their training variants in training mode)."""
+        lib = _lib.load()
+        need = [lib.mmmot_affinity_workspace(pairs, n, m) for n, m in transitions]
+        if L:
+            if self.training:
+                need += [lib.mmmot_appearance_train_workspace(pairs * L, H, W), lib.mmmot_pointnet_train_workspace(pairs, L, P),
+                         lib.mmmot_w_det_train_workspace(L)]
+            else:
+                need += [lib.mmmot_appearance_workspace(pairs * L, H, W), lib.mmmot_pointnet_workspace(pairs, L, P)]
+            need.append(lib.mmmot_fusion_det_workspace(pairs, L))
+        return max(need)
+
+    def _features(self, wts, ws, st, crops, points, split, pairs, L, feats, det):
+        """Appearance, PointNet and fusion / detection score of `pairs` samples of L detections on stream `st`:
+        feats pairs x 3 x 512 x L, det pairs x 3 x L.  split: the CSR point offsets, CPU int32.
+
+        In training mode (reference TrackingNet.forward with self.training, modules/tracking_net.py:152-162) the
+        BatchNorm layers (VGG trunk, w_det) normalise with the statistics of this call and det scores are raw logits
+        without the neg_threshold step; DropBlock (the two deepest SkipPool heads) and the PointNet head's Dropout
+        (rrc_pfv config: dropblock 5, use_dropout True) draw their masks from torch's generators exactly as the
+        reference does (_dropblock_weights / _dropout_mask) and the library applies them.  Returns the batch statistics
+        (bn_vgg 13 x 2 x 512, bn_det 2 x 2 x 512) in training mode, else None."""
+        lib = _lib.load()
+        dev = feats.device
         H, W = crops.shape[-2:]
-        st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        P = int(split_host[-1])
-        need = max(lib.mmmot_appearance_workspace(pairs * L, H, W),
-                   lib.mmmot_pointnet_workspace(pairs, L, P),
-                   lib.mmmot_fusion_det_workspace(pairs, L),
-                   lib.mmmot_affinity_workspace(pairs, n, m))
-        ws = self._workspace(need, dev)
-        wsp, wsn = ctypes.c_void_p(ws.data_ptr()), ctypes.c_size_t(ws.numel())
-        _lib.check(lib.mmmot_status_reset(wsp, st), "mmmot_status_reset")
-        feats = out["feats"][p0:p0 + pairs]
-        vp = lambda t: ctypes.c_void_p(t.data_ptr())
-        _lib.check(lib.mmmot_appearance_fwd(wts.ptr, vp(crops), pairs * L, H, W, L, vp(feats), wsp, wsn, st),
-                   "mmmot_appearance_fwd")
-        hs = split_host.numpy()
-        _lib.check(lib.mmmot_pointnet_fwd(wts.ptr, vp(points), vp(split_dev), ctypes.c_void_p(hs.ctypes.data),
-                                          pairs, L, vp(feats), wsp, wsn, st), "mmmot_pointnet_fwd")
-        _lib.check(lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[self.score_fusion_arch], self._score_flags(),
-                                            float(self.neg_threshold), pairs, L, vp(feats),
-                                            vp(out["det"][p0:p0 + pairs]), wsp, wsn, st), "mmmot_fusion_det_fwd")
-        _lib.check(lib.mmmot_affinity_fwd(wts.ptr, _lib.AFFINITY[self.affinity_op],
-                                          _lib.SOFTMAX.get(self.softmax_mode, 0), _lib.END_MODE[self.end_mode], pairs, n, m, vp(feats),
-                                          vp(out["link"][p0:p0 + pairs]), vp(out["new"][p0:p0 + pairs]),
-                                          vp(out["end"][p0:p0 + pairs]), wsp, wsn, st), "mmmot_affinity_fwd")
-        # the status word (FP16 range flag) of this chunk, accumulated into out["status"] in stream order
-        out["status"] |= ws[:4].view(torch.int32)
+        wsp, wsn = _vp(ws), ctypes.c_size_t(ws.numel())
+        train = self.training
+        if train:
+            # random masks, in the reference's draw order: appearance heads 2 and 3 (CPU generator), then the PointNet head
+            dm2 = dm3 = hmask = None
+            if self.dropblock:
+                dm2 = self._dropblock_weights(L, H // 16, W // 16, int(self.dropblock)).to(dev)
+                dm3 = self._dropblock_weights(L, H // 32, W // 32, int(self.dropblock)).to(dev)
+            if self.use_dropout:
+                hmask = self._dropout_mask((512, int(split[-1])), dev).contiguous()
+            bn_vgg = torch.zeros(13, 2, 512, device=dev)
+            bn_det = torch.zeros(2, 2, 512, device=dev)
+            _lib.check(lib.mmmot_appearance_train_fwd(wts.ptr, _vp(crops), pairs * L, H, W, L, _vp(feats), _vp(bn_vgg), _vp(dm2),
+                                                      _vp(dm3), wsp, wsn, st), "mmmot_appearance_train_fwd")
+        else:
+            _lib.check(lib.mmmot_appearance_fwd(wts.ptr, _vp(crops), pairs * L, H, W, L, _vp(feats), wsp, wsn, st),
+                       "mmmot_appearance_fwd")
+        split_dev = self._split_to_device(split, dev)
+        hs = ctypes.c_void_p(split.numpy().ctypes.data)
+        if train:
+            _lib.check(lib.mmmot_pointnet_train_fwd(wts.ptr, _vp(points), _vp(split_dev), hs, pairs, L, _vp(hmask), _vp(feats),
+                                                    wsp, wsn, st), "mmmot_pointnet_train_fwd")
+        else:
+            _lib.check(lib.mmmot_pointnet_fwd(wts.ptr, _vp(points), _vp(split_dev), hs, pairs, L, _vp(feats), wsp, wsn, st),
+                       "mmmot_pointnet_fwd")
+        flags, thr = (0, 0.0) if train else (self._score_flags(), float(self.neg_threshold))
+        _lib.check(lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[self.score_fusion_arch], flags, thr, pairs, L, _vp(feats),
+                                            _vp(det), wsp, wsn, st), "mmmot_fusion_det_fwd")
+        if not train:
+            return None
+        _lib.check(lib.mmmot_w_det_train_fwd(wts.ptr, L, _vp(feats), _vp(det), _vp(bn_det), wsp, wsn, st), "mmmot_w_det_train_fwd")
+        return bn_vgg, bn_det
+
+    def _associate(self, wts, ws, st, pairs, n, m, feats, link, new, end):
+        """Affinity / start-end / softmax stage on stream `st`: feats pairs x 3 x 512 x (n+m), contiguous ->
+        link pairs x 3 x n x m, new pairs x 3 x m, end pairs x 3 x n."""
+        _lib.check(_lib.load().mmmot_affinity_fwd(wts.ptr, _lib.AFFINITY[self.affinity_op], _lib.SOFTMAX.get(self.softmax_mode, 0),
+                                                  _lib.END_MODE[self.end_mode], pairs, n, m, _vp(feats), _vp(link), _vp(new),
+                                                  _vp(end), _vp(ws), ctypes.c_size_t(ws.numel()), st), "mmmot_affinity_fwd")
 
     def _score_flags(self):
         """reference tracking_net.py:153-162: sigmoid only when 'cls' is in score_arch; the neg_threshold step is
@@ -201,16 +238,10 @@ class TrackingNet(nn.Module):
     def _pick_chunk(self, B, n, m, P_per_pair, H, W, dev):
         if self.chunk_pairs:
             return min(B, self.chunk_pairs)
-        lib = _lib.load()
         free, _ = torch.cuda.mem_get_info(dev)
         budget = min(free * 0.5, 48e9)
         c = B
-        L = n + m
-        while c > 1:
-            need = max(lib.mmmot_appearance_workspace(c * L, H, W), lib.mmmot_pointnet_workspace(c, L, int(P_per_pair * c) + 1),
-                       lib.mmmot_affinity_workspace(c, n, m))
-            if need <= budget:
-                break
+        while c > 1 and self._workspace_bytes(c, [(n, m)], n + m, int(P_per_pair * c) + 1, H, W) > budget:
             c = (c + 1) // 2
         return c
 
@@ -253,15 +284,23 @@ class TrackingNet(nn.Module):
             "end": torch.empty(B, 3, n, device=dev),
         }
         with torch.cuda.device(dev):        # the library works on the CURRENT device
+            st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             chunk = self._pick_chunk(B, n, m, int(split[-1]) / B, H, W, dev)
             for p0 in range(0, B, chunk):
                 pc = min(chunk, B - p0)
                 s_host = split[p0 * L:(p0 + pc) * L + 1]
                 off = int(s_host[0])
                 s_host = (s_host - off).contiguous()
-                s_dev = self._split_to_device(s_host, dev)
-                self._run_chunk(lib, wts, crops[p0 * L:(p0 + pc) * L], points[off:off + int(s_host[-1])],
-                                s_dev, s_host, pc, n, m, out, p0)
+                P = int(s_host[-1])
+                ws = self._workspace(self._workspace_bytes(pc, [(n, m)], L, P, H, W), dev)
+                _lib.check(lib.mmmot_status_reset(_vp(ws), st), "mmmot_status_reset")
+                feats = out["feats"][p0:p0 + pc]
+                self._features(wts, ws, st, crops[p0 * L:(p0 + pc) * L], points[off:off + P], s_host, pc, L, feats,
+                               out["det"][p0:p0 + pc])
+                self._associate(wts, ws, st, pc, n, m, feats, out["link"][p0:p0 + pc], out["new"][p0:p0 + pc],
+                                out["end"][p0:p0 + pc])
+                # the status word (FP16 range flag) of this chunk, accumulated into out["status"] in stream order
+                out["status"] |= ws[:4].view(torch.int32)
         out["trans"] = [wts.trans1.unsqueeze(0).clone(), wts.trans2.unsqueeze(0).clone()]
         if not keep_feats:
             del out["feats"]
@@ -283,16 +322,12 @@ class TrackingNet(nn.Module):
         link = torch.empty(B, 3, n, m, device=dev)
         new = torch.empty(B, 3, m, device=dev)
         end = torch.empty(B, 3, n, device=dev)
-        vp = lambda t: ctypes.c_void_p(t.data_ptr())
         with torch.cuda.device(dev):
-            ws = self._workspace(lib.mmmot_affinity_workspace(B, n, m), dev)
+            ws = self._workspace(self._workspace_bytes(B, [(n, m)]), dev)
             st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(lib.mmmot_status_reset(vp(ws), st), "mmmot_status_reset")
-            _lib.check(lib.mmmot_affinity_fwd(wts.ptr, _lib.AFFINITY[self.affinity_op],
-                                              _lib.SOFTMAX.get(self.softmax_mode, 0), _lib.END_MODE[self.end_mode], B, n, m, vp(feats),
-                                              vp(link), vp(new), vp(end), vp(ws), ws.numel(), st),
-                       "mmmot_affinity_fwd")
-            _lib.check(lib.mmmot_status_check(vp(ws), st), "mmmot_affinity_fwd")
+            _lib.check(lib.mmmot_status_reset(_vp(ws), st), "mmmot_status_reset")
+            self._associate(wts, ws, st, B, n, m, feats, link, new, end)
+            _lib.check(lib.mmmot_status_check(_vp(ws), st), "mmmot_affinity_fwd")
         return link, new, end
 
     @torch.no_grad()
@@ -346,139 +381,69 @@ class TrackingNet(nn.Module):
         reference consumes for a tensor of this shape."""
         return torch.nn.functional.dropout(torch.ones(shape, device=dev), p=p, training=True)
 
+    # ------------------------------------------------------------------ the reference's forward
     @torch.no_grad()
-    def _forward_train(self, dets, det_info, dets_split):
-        """reference TrackingNet.forward with self.training (modules/tracking_net.py:152-162, 183-192): BatchNorm layers
-        (VGG trunk, w_det) normalise with the statistics of this sample and update their running averages, det_scores are
-        raw logits without the neg_threshold step, new/end scores are not zero-padded.  Forward only — no autograd graph
-        is built through the CUDA library.  DropBlock (the two deepest SkipPool heads) and the PointNet head's Dropout
-        (rrc_pfv config: dropblock 5, use_dropout True) draw their masks from torch's generators exactly as the reference
-        does (_dropblock_weights / _dropout_mask) and the library applies them."""
-        if len(dets_split) != 2:
-            raise NotImplementedError("mmmot_b200.TrackingNet supports 2-frame samples (sample_max_len: 2)")
-        n, m = int(dets_split[0]), int(dets_split[1])
-        L = n + m
-        lib = _lib.load()
-        self._prepared = None                      # parameters move under an optimizer: re-derive the operands every step
-        wts = self.prepared()
-        dev = wts.flat.device
-        crops = dets.contiguous().float()
-        points = det_info['points'].reshape(-1, det_info['points'].shape[-1])[:, :3].contiguous().float()
-        split = det_info['points_split'].reshape(-1).detach().to("cpu", torch.int32).contiguous()
-        if crops.device != dev or points.device != dev or crops.shape[0] != L or split.numel() != L + 1:
-            raise _lib.MmmotError("inputs do not match the module's device / dets_split")
-        H, W = crops.shape[-2:]
-        feats = torch.empty(1, 3, 512, L, device=dev)
-        det = torch.empty(1, 3, L, device=dev)
-        link = torch.empty(1, 3, n, m, device=dev)
-        new = torch.empty(1, 3, m, device=dev)
-        end = torch.empty(1, 3, n, device=dev)
-        bn_vgg = torch.zeros(13, 2, 512, device=dev)
-        bn_det = torch.zeros(2, 2, 512, device=dev)
-        vp = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-        # random masks, in the reference's draw order: appearance heads 2 and 3 (CPU generator), then the PointNet head
-        dm2 = dm3 = hmask = None
-        if self.dropblock:
-            dm2 = self._dropblock_weights(L, H // 16, W // 16, int(self.dropblock)).to(dev)
-            dm3 = self._dropblock_weights(L, H // 32, W // 32, int(self.dropblock)).to(dev)
-        if self.use_dropout:
-            hmask = self._dropout_mask((512, int(split[-1])), dev).contiguous()
-        with torch.cuda.device(dev):
-            st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            need = max(lib.mmmot_appearance_train_workspace(L, H, W), lib.mmmot_pointnet_train_workspace(1, L, int(split[-1])),
-                       lib.mmmot_fusion_det_workspace(1, L), lib.mmmot_affinity_workspace(1, n, m),
-                       lib.mmmot_w_det_train_workspace(L))
-            ws = self._workspace(need, dev)
-            wsp, wsn = vp(ws), ctypes.c_size_t(ws.numel())
-            _lib.check(lib.mmmot_status_reset(wsp, st), "mmmot_status_reset")
-            _lib.check(lib.mmmot_appearance_train_fwd(wts.ptr, vp(crops), L, H, W, L, vp(feats), vp(bn_vgg), vp(dm2), vp(dm3),
-                                                      wsp, wsn, st), "mmmot_appearance_train_fwd")
-            hs = split.numpy()
-            _lib.check(lib.mmmot_pointnet_train_fwd(wts.ptr, vp(points), vp(split.to(dev)), ctypes.c_void_p(hs.ctypes.data), 1, L,
-                                                    vp(hmask), vp(feats), wsp, wsn, st), "mmmot_pointnet_train_fwd")
-            _lib.check(lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[self.score_fusion_arch], 0, 0.0, 1, L, vp(feats), vp(det),
-                                                wsp, wsn, st), "mmmot_fusion_det_fwd")
-            _lib.check(lib.mmmot_w_det_train_fwd(wts.ptr, L, vp(feats), vp(det), vp(bn_det), wsp, wsn, st), "mmmot_w_det_train_fwd")
-            _lib.check(lib.mmmot_affinity_fwd(wts.ptr, _lib.AFFINITY[self.affinity_op], _lib.SOFTMAX.get(self.softmax_mode, 0),
-                                              _lib.END_MODE[self.end_mode], 1, n, m, vp(feats), vp(link), vp(new), vp(end), wsp, wsn, st), "mmmot_affinity_fwd")
-            _lib.check(lib.mmmot_status_check(wsp, st), "mmmot_b200.TrackingNet training forward")
-        # running averages (reference: nn.BatchNorm2d / BatchNorm1d side effect of a training-mode forward)
-        h, w_ = H, W
-        for i, cout in enumerate(cout for stage in VGG_STAGES for _, _, cout in stage):
-            self._update_running(self._VGG_BN[i], bn_vgg[i, 0, :cout], bn_vgg[i, 1, :cout], float(L * h * w_))
-            if VGG_POOLED_BEFORE[i]:
-                h, w_ = h // 2, w_ // 2
-        self._update_running("w_det.1", bn_det[0, 0, :512], bn_det[0, 1, :512], 3.0 * L)
-        self._update_running("w_det.4", bn_det[1, 0, :256], bn_det[1, 1, :256], 3.0 * L)
-        return det[0], [link[0]], new[0], end[0], [wts.trans1.unsqueeze(0).clone(), wts.trans2.unsqueeze(0).clone()]
+    def forward(self, dets, det_info, dets_split):
+        """Reference signature (modules/tracking_net.py:165-193): one sample of K >= 2 frames.
 
-    @torch.no_grad()
-    def _forward_multi(self, dets, det_info, splits):
-        """Samples of more than two frames (reference modules/tracking_net.py:170-182; sample_max_len > 2): the feature
-        stages run once over all L detections of the sample (one GroupNorm domain, exactly like the reference), then
-        ``associate`` runs on every pair of consecutive frames.  (mmmot_b200.ortools_solve solves the association
-        programme of such samples as a min-cost flow.)"""
+        dets L x 3 x H x W; det_info['points'] 1 x P x 3; det_info['points_split'] 1 x (L+1) float;
+        dets_split: K shape-(1,) int tensors, the detections of each frame.  The feature stages run once over all L
+        detections of the sample (one GroupNorm domain, exactly like the reference), then the affinity stage on every
+        pair of consecutive frames (mmmot_b200.ortools_solve solves the association programme of K > 2 frames as a
+        min-cost flow).  Returns (det_scores 3xL, [link_scores 3 x n_k x n_k+1 per pair of frames], new_scores 3xL,
+        end_scores 3xL, trans).
+
+        In training mode (two-frame samples only) the reference's training branch is returned instead
+        (tracking_net.py:183-192; see _features): raw det logits, new_scores 3 x m and end_scores 3 x n not zero-padded,
+        and the BatchNorm layers' running averages are updated.  Forward only: no autograd graph is built through the
+        CUDA library."""
+        splits = [int(s) for s in dets_split]
+        if self.training and len(splits) != 2:
+            raise NotImplementedError("mmmot_b200.TrackingNet supports 2-frame samples (sample_max_len: 2)")
+        L = sum(splits)
         lib = _lib.load()
+        if self.training:
+            self._prepared = None                  # parameters move under an optimizer: re-derive the operands every step
         wts = self.prepared()
         dev = wts.flat.device
-        L = sum(splits)
         crops = dets.contiguous().float()
         points = det_info['points'].reshape(-1, det_info['points'].shape[-1])[:, :3].contiguous().float()
         split = det_info['points_split'].reshape(-1).detach().to("cpu", torch.int32).contiguous()
-        if crops.device != dev or points.device != dev or crops.shape[0] != L or split.numel() != L + 1 or min(splits) <= 0:
+        if (crops.device != dev or points.device != dev or crops.shape[0] != L or split.numel() != L + 1
+                or len(splits) < 2 or min(splits) <= 0):
             raise _lib.MmmotError("inputs do not match the module's device / dets_split")
         H, W = crops.shape[-2:]
+        transitions = list(zip(splits[:-1], splits[1:]))
         feats = torch.empty(1, 3, 512, L, device=dev)
         det = torch.empty(1, 3, L, device=dev)
-        vp = lambda t: ctypes.c_void_p(t.data_ptr())
         links, news, ends = [], [], []
         with torch.cuda.device(dev):
             st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            need = max([lib.mmmot_appearance_workspace(L, H, W), lib.mmmot_pointnet_workspace(1, L, int(split[-1])),
-                        lib.mmmot_fusion_det_workspace(1, L)] +
-                       [lib.mmmot_affinity_workspace(1, a, b) for a, b in zip(splits[:-1], splits[1:])])
-            ws = self._workspace(need, dev)
-            wsp, wsn = vp(ws), ctypes.c_size_t(ws.numel())
-            _lib.check(lib.mmmot_status_reset(wsp, st), "mmmot_status_reset")
-            _lib.check(lib.mmmot_appearance_fwd(wts.ptr, vp(crops), L, H, W, L, vp(feats), wsp, wsn, st), "mmmot_appearance_fwd")
-            hs = split.numpy()
-            _lib.check(lib.mmmot_pointnet_fwd(wts.ptr, vp(points), vp(split.to(dev)), ctypes.c_void_p(hs.ctypes.data), 1, L,
-                                              vp(feats), wsp, wsn, st), "mmmot_pointnet_fwd")
-            _lib.check(lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[self.score_fusion_arch], self._score_flags(),
-                                                float(self.neg_threshold), 1, L, vp(feats), vp(det), wsp, wsn, st),
-                       "mmmot_fusion_det_fwd")
+            ws = self._workspace(self._workspace_bytes(1, transitions, L, int(split[-1]), H, W), dev)
+            _lib.check(lib.mmmot_status_reset(_vp(ws), st), "mmmot_status_reset")
+            bn = self._features(wts, ws, st, crops, points, split, 1, L, feats, det)
             start = 0
-            for a, b in zip(splits[:-1], splits[1:]):
-                f = feats[:, :, :, start:start + a + b].contiguous()
+            for a, b in transitions:
                 link = torch.empty(1, 3, a, b, device=dev)
                 new = torch.empty(1, 3, b, device=dev)
                 end = torch.empty(1, 3, a, device=dev)
-                _lib.check(lib.mmmot_affinity_fwd(wts.ptr, _lib.AFFINITY[self.affinity_op], _lib.SOFTMAX.get(self.softmax_mode, 0),
-                                                  _lib.END_MODE[self.end_mode], 1, a, b, vp(f), vp(link), vp(new), vp(end),
-                                                  wsp, wsn, st), "mmmot_affinity_fwd")
+                self._associate(wts, ws, st, 1, a, b, feats[:, :, :, start:start + a + b].contiguous(), link, new, end)
                 links.append(link[0]); news.append(new[0]); ends.append(end[0])
                 start += a
-            _lib.check(lib.mmmot_status_check(wsp, st), "mmmot_b200.TrackingNet forward")
+            _lib.check(lib.mmmot_status_check(_vp(ws), st),
+                       "mmmot_b200.TrackingNet training forward" if self.training else "mmmot_b200.TrackingNet forward")
+        trans = [wts.trans1.unsqueeze(0).clone(), wts.trans2.unsqueeze(0).clone()]
+        if self.training:
+            # running averages (reference: nn.BatchNorm2d / BatchNorm1d side effect of a training-mode forward)
+            bn_vgg, bn_det = bn
+            h, w_ = H, W
+            for i, cout in enumerate(cout for stage in VGG_STAGES for _, _, cout in stage):
+                self._update_running(self._VGG_BN[i], bn_vgg[i, 0, :cout], bn_vgg[i, 1, :cout], float(L * h * w_))
+                if VGG_POOLED_BEFORE[i]:
+                    h, w_ = h // 2, w_ // 2
+            self._update_running("w_det.1", bn_det[0, 0, :512], bn_det[0, 1, :512], 3.0 * L)
+            self._update_running("w_det.4", bn_det[1, 0, :256], bn_det[1, 1, :256], 3.0 * L)
+            return det[0], links, news[0], ends[0], trans
         new_scores = torch.cat([det.new_zeros(3, splits[0])] + news, dim=1)        # tracking_net.py:183-189
         end_scores = torch.cat(ends + [det.new_zeros(3, splits[-1])], dim=1)
-        return det[0], links, new_scores, end_scores, [wts.trans1.unsqueeze(0).clone(), wts.trans2.unsqueeze(0).clone()]
-
-    def forward(self, dets, det_info, dets_split):
-        """Reference signature (modules/tracking_net.py:165): one frame-pair.
-
-        dets L x 3 x H x W; det_info['points'] 1 x P x 3; det_info['points_split'] 1 x (L+1) float;
-        dets_split list of two shape-(1,) int tensors.  Returns
-        (det_scores 3xL, [link_scores 3xNxM], new_scores 3xL, end_scores 3xL, trans).  In training mode the reference's
-        training branch is returned instead (see _forward_train)."""
-        if self.training:
-            return self._forward_train(dets, det_info, dets_split)
-        if len(dets_split) > 2:
-            return self._forward_multi(dets, det_info, [int(s) for s in dets_split])
-        n, m = int(dets_split[0]), int(dets_split[1])
-        split = det_info['points_split'].reshape(-1)
-        o = self.forward_batch(dets, det_info['points'].reshape(-1, det_info['points'].shape[-1])[:, :3],
-                               split, n, m)
-        det = o["det"][0]
-        new_scores = torch.cat([det.new_zeros(3, n), o["new"][0]], dim=1)
-        end_scores = torch.cat([o["end"][0], det.new_zeros(3, m)], dim=1)
-        return det, [o["link"][0]], new_scores, end_scores, o["trans"]
+        return det[0], links, new_scores, end_scores, trans

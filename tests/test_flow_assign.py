@@ -444,8 +444,8 @@ def test_flow_large_samples_up_to_the_shared_memory_cap(L, K, B, warps):
 
 @pytest.mark.gpu
 def test_predict_three_frame_windows_end_to_end(tmp_path):
-    """A synthetic 5-frame sequence in 3-frame windows (frames 0-2, 2-4) through TrackingModule.predict on
-    _forward_multi's outputs: the stitched ids and the KITTI text equal those of the same host code fed the MILP's
+    """A synthetic 5-frame sequence in 3-frame windows (frames 0-2, 2-4) through TrackingModule.predict on the
+    outputs of TrackingNet.forward: the stitched ids and the KITTI text equal those of the same host code fed the MILP's
     assignment of the same GPU scores."""
     import mmmot_b200
     from mmmot_b200.synthetic import synthetic_pair, synthetic_state_dict
