@@ -468,9 +468,13 @@ struct PnWs {
   int4 *tiles, *ctab;
 };
 
+// capacity of the tile tables: 128-point tiles over `pairs` ragged ranges of P points; also bounds 2 partials per 256-wide tile
+long pn_max_tiles(long P, int pairs) { return P / 128 + 2 * pairs + 2; }
+
 // use_tc: the tensor-core path never materialises the 1024-wide activation (537 MB per frame-pair at cfg4), reads the
 // points row-major (no xt), never stores layer 1 in fp32 (no y1) and keeps U channels-last (ut; the FP32 path: u)
-PnWs carve(MmArena& a, int pairs, int L, long P, long max_tiles, bool use_tc) {
+PnWs carve(MmArena& a, int pairs, int L, long P, bool use_tc) {
+  const long max_tiles = pn_max_tiles(P, pairs);
   PnWs w;
   long nd = (long)pairs * L;
   w.xt = a.take<float>(use_tc ? 0 : 3 * P);
@@ -503,12 +507,21 @@ PnWs carve(MmArena& a, int pairs, int L, long P, long max_tiles, bool use_tc) {
   return w;
 }
 
-// Column tiles of at most tw points over each pair's point range (tiles never straddle two pairs: one pair = one
-// GroupNorm domain).  The host needs only this count for its launch geometry.
-long pn_tile_count(const int* h_det_split, int pairs, int L, int tw) {
-  long n = 0;
-  for (int p = 0; p < pairs; p++) n += mm_cdiv((long)h_det_split[(p + 1) * L] - h_det_split[p * L], tw);
-  return n;
+// The host's checks of the CSR offsets h_det_split [pairs*L + 1]: MMMOT_E_SHAPE unless the first is 0, P > 0 and every
+// detection owns at least one point.  n_tiles: column tiles of at most tw points over each pair's point range (tiles
+// never straddle two pairs: one pair = one GroupNorm domain); the host needs only this count for its launch geometry.
+// max_tiles: how many the tables of a carved workspace hold.
+struct PnShape { long P, n_tiles, max_tiles; };
+int pn_shape(const int* h_det_split, int pairs, int L, int tw, PnShape& s) {
+  const int ndet = pairs * L;
+  s.P = h_det_split[ndet];
+  if (h_det_split[0] != 0 || s.P <= 0) return MMMOT_E_SHAPE;
+  for (int d = 0; d < ndet; d++)
+    if (h_det_split[d + 1] <= h_det_split[d]) return MMMOT_E_SHAPE;
+  s.n_tiles = 0;
+  for (int p = 0; p < pairs; p++) s.n_tiles += mm_cdiv((long)h_det_split[(p + 1) * L] - h_det_split[p * L], tw);
+  s.max_tiles = pn_max_tiles(s.P, pairs);
+  return 0;
 }
 
 // The tables of the ragged per-pair point ranges, built on the device from the CSR offsets det_split [pairs*L + 1]:
@@ -593,194 +606,124 @@ int pn_wide_stats(const PnWs& w, const int* h_det_split, const int* det_split, l
   return 0;
 }
 
-}  // namespace
-
-// engine choice from the per-pair shape only (see appearance.cu)
-static bool pointnet_use_tc(int L) { return mm_engine() == 2 || (mm_engine() == 0 && L >= 16); }
-
-extern "C" size_t mmmot_pointnet_workspace(int pairs, int L, long p_total) {
-  MmArena a(nullptr, 0);
-  carve(a, pairs, L, p_total, p_total / 128 + 2 * pairs + 2, pointnet_use_tc(L));
-  return a.off;
-}
-
-extern "C" size_t mmmot_pointnet_train_workspace(int pairs, int L, long p_total) {
-  MmArena a(nullptr, 0);
-  carve(a, pairs, L, p_total, p_total / 128 + 2 * pairs + 2, false);
-  return a.off;
-}
-
-// mmmot_debug_stage_layout, stage 2: where mmmot_pointnet_fwd leaves its intermediates (a dry carve; no CUDA call)
-int mm_pointnet_layout(int pairs, int L, long P, size_t* off, int* tensor_cores) {
-  MmArena a(nullptr, 0);
-  const bool use_tc = pointnet_use_tc(L);
-  const PnWs w = carve(a, pairs, L, P, P / 128 + 2 * pairs + 2, use_tc);
-  const void* const bufs[26] = {w.xt, w.y1, w.t0, w.t1, w.big, w.segsum, w.x1p, w.xp, w.gmean, w.u, w.ut, w.hmean, w.o,
-                                w.sc1, w.sh1, w.sc, w.sh, w.stats, w.mom, w.part, w.gstart, w.sstart, w.seg, w.cnt,
-                                w.tiles, w.ctab};
-  for (int i = 0; i < 26; i++) off[i] = (size_t)reinterpret_cast<uintptr_t>(bufs[i]);
-  off[26] = a.off;
-  if (tensor_cores) *tensor_cores = use_tc ? 1 : 0;
+// Layer 5 (K = 128 -> M = 1024) or the head (64 -> 512, addend U): statistics only (pn_wide_stats), then a recompute with
+// GroupNorm + ReLU + per-detection sums in its epilogue, out [ndet][M] the per-detection means.  The M x P activation
+// (537 MB per frame-pair at cfg4 for layer 5) is never written.  tag times the recompute; status goes to gn_finalize.
+int pn_wide_layer(const PnWs& w, const int* h_det_split, const int* det_split, long P, int pairs, int L, long n_tiles,
+                  const __half* X, int K, const float* Wt, const uint4* Wp, float wps, const float* bias, int M,
+                  const float* addend, const float* gamma, const float* beta, float* out, int tag, int* status,
+                  cudaStream_t st) {
+  const int ndet = pairs * L;
+  MM_TRY(pn_wide_stats(w, h_det_split, det_split, P, pairs, L, n_tiles, X, K, Wt, Wp, wps, bias, M, addend, st));
+  MM_TRY(gn_finalize(w.stats, gamma, beta, w.cnt, 0, pairs, M, 1, w.sc, w.sh, st, 0, 0, status));
+  MM_CUDA(cudaMemsetAsync(w.segsum, 0, (size_t)ndet * M * sizeof(unsigned long long), st));
+  GemmP p = gemm_defaults();
+  p.bias = bias; p.M = M; p.K = K;
+  p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
+  p.y_ms = M;
+  if (addend) { p.addend = addend; p.ld_add = M; }
+  p.sc = w.sc; p.sh = w.sh; p.seg = w.seg;
+  const bool timed = mm_timing_on();
+  if (timed) mm_timing_begin(st, tag, 2.0 * M * K * (double)P, 4.0 * K * (double)P);
+  MM_TRY(gemm_tma_launch_mat(p, Wp, wps, X, P * K, P, K, tc::OUT_CL, 0, st, w.segsum, nullptr, w.ctab));
+  if (timed) mm_timing_end(st);
+  segsum_mean_cl_kernel<<<mm_cdiv((long)M * ndet, 256), 256, 0, st>>>(w.segsum, det_split, M, ndet, out);
+  MM_LAUNCH_CHECK();
   return 0;
 }
 
-// train: FP32 engine; head_mask (optional) = the Dropout mask of the head activation, [512][P] with values {0, 1/(1-p)}
-static int pointnet_impl(const mmmot_weights* wts, const float* points, const int* det_split, const int* h_det_split,
-                         int pairs, int L, float* feats, void* workspace, size_t workspace_bytes, void* stream, bool train,
-                         const float* head_mask);
-
-extern "C" int mmmot_pointnet_fwd(const mmmot_weights* wts, const float* points, const int* det_split,
-                                  const int* h_det_split, int pairs, int L, float* feats,
-                                  void* workspace, size_t workspace_bytes, void* stream) {
-  return pointnet_impl(wts, points, det_split, h_det_split, pairs, L, feats, workspace, workspace_bytes, stream, false, nullptr);
-}
-
-extern "C" int mmmot_pointnet_train_fwd(const mmmot_weights* wts, const float* points, const int* det_split,
-                                        const int* h_det_split, int pairs, int L, const float* head_drop_mask, float* feats,
-                                        void* workspace, size_t workspace_bytes, void* stream) {
-  return pointnet_impl(wts, points, det_split, h_det_split, pairs, L, feats, workspace, workspace_bytes, stream, true,
-                       head_drop_mask);
-}
-
-static int pointnet_impl(const mmmot_weights* wts, const float* points, const int* det_split, const int* h_det_split,
-                         int pairs, int L, float* feats, void* workspace, size_t workspace_bytes, void* stream, bool train,
-                         const float* head_mask) {
-  if (!wts || !points || !det_split || !h_det_split || !feats || !workspace || pairs <= 0 || L <= 0)
-    return MMMOT_E_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
+// Tensor-core path: channels-last activations; layers 2-4 write fp32 Y[p][cout] + GroupNorm partials, layer 1 and the
+// two widest layers are recomputed instead of stored.  Layer 1's FP16 planes (x1p) are kept for the head.
+int pointnet_tc(const mmmot_weights* wts, const float* points, const int* det_split, const int* h_det_split, int pairs,
+                int L, long P, long n_tiles, const PnWs& w, int* status, float* feats, cudaStream_t st) {
   const int ndet = pairs * L;
-  const long P = h_det_split[ndet];
-  if (h_det_split[0] != 0 || P <= 0) return MMMOT_E_SHAPE;
-  for (int d = 0; d < ndet; d++)
-    if (h_det_split[d + 1] <= h_det_split[d]) return MMMOT_E_SHAPE;  // every detection owns >= 1 point
-
-  // column tiles never straddle two frame-pairs (one pair = one GroupNorm domain)
-  const bool use_tc = !train && pointnet_use_tc(L);
-  const int TNW = use_tc ? tc::BN : 128;
-  const long n_tiles = pn_tile_count(h_det_split, pairs, L, TNW);
-  const long max_tiles = P / 128 + 2 * pairs + 2;   // also bounds 2 partials per 256-wide tile
-  MmArena ar(workspace, workspace_bytes);
-  PnWs w = carve(ar, pairs, L, P, max_tiles, use_tc);
-  if (!ar.ok() || n_tiles > max_tiles) return MMMOT_E_WORKSPACE;
-  MM_TRY(pn_tables(det_split, pairs, L, P, TNW, n_tiles, w.cnt, w.gstart, w.tiles, w.seg, use_tc ? w.ctab : nullptr, st));
-
-  const int cin[5] = {3, 64, 64, 64, 128}, cout[5] = {64, 64, 64, 128, 1024};
   const bool timed = mm_timing_on();
-  if (use_tc) {
-    // ---------------- tensor-core path: channels-last activations ----------------
-    // layer i writes fp32 Y[p][cout] + GroupNorm partials; norm_split turns it into the packed FP16
-    // operand of layer i+1.  y1's packed form (x1p) is kept for the head.
-    float* ybuf[5] = {nullptr, w.t0, w.t1, w.t0, nullptr};   // layer 1 is recomputed, never stored
-    const bool gen_mid = !(mm_debug_flags() & 8192);   // debug bit 13: layers 3, 4 through norm_split + the TMA-fed kernel
-    for (int i = 0; i < 5; i++) {
-      const float* const* q = &wts->w[MMMOT_W_PN_L1 + 4 * i];
-      GemmP p = gemm_defaults();
-      p.bias = q[1]; p.M = cout[i]; p.K = cin[i];
-      p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
-      p.Y = ybuf[i]; p.y_ms = cout[i];
-      p.part = w.part;
-      const uint4* wp = (const uint4*)wts->w[MMMOT_W_PN_WP1 + i];
-      const float wps = wts->tc_scale[MMMOT_W_PN_WP1 + i];
-      const double cols = (double)P;
-      if (i == 0) {
-        if (timed) mm_timing_begin(st, MM_T_PN_L1, 2.0 * 64 * 3 * cols, 12.0 * cols);
-        pn_l1_stats_kernel<<<(int)n_tiles, 256, 0, st>>>(points, w.tiles, q[0], q[1], w.part);
-        MM_LAUNCH_CHECK();
-        if (timed) mm_timing_end(st);
-      } else if (i == 4) {
-        // layer 5 (1024 wide): statistics only, nothing stored
-        MM_TRY(pn_wide_stats(w, h_det_split, det_split, P, pairs, L, n_tiles, w.xp, cin[i], q[0], wp, wps, q[1], cout[i],
-                             nullptr, st));
-      } else {
-        // compulsory traffic: activation in (4 B per element) + fp32 activation out
-        if (timed) mm_timing_begin(st, MM_T_PN_L2 + (i - 1), 2.0 * cout[i] * cin[i] * cols, 4.0 * (cin[i] + cout[i]) * cols);
-        if (gen_mid && (i == 2 || i == 3)) {
-          // layers 3, 4: GroupNorm + ReLU of the previous layer applied by this contraction's operand producers
-          // (gemm_gen.cuh) straight from its fp32 output: no normalised copy is written
-          MM_TRY((gemm_gen_launch<gen::GEN_NORM>(p, wp, wps, ybuf[i - 1], cin[i], w.sc, w.sh, 0, 0, 0, st)));
-        } else {                                                // FP16 hi/lo planes [2][P][cin] via TMA
-          MM_TRY(gemm_tma_launch_mat(p, wp, wps, i == 1 ? w.x1p : w.xp, P * cin[i], P, cin[i], tc::OUT_CL, 0, st));
-        }
-        if (timed) mm_timing_end(st);
-      }
-      if (i < 4) MM_TRY(stats_reduce(w.part, cout[i], pairs, 0, w.gstart, w.stats, st, 2));
-      MM_TRY(gn_finalize(w.stats, q[2], q[3], w.cnt, 0, pairs, cout[i], 1, w.sc, w.sh, st, 0, 0, ar.status()));
-      if (i == 0) {
-        if (timed) mm_timing_begin(st, MM_T_PN_L1, 0.0, (12.0 + 4.0 * 64) * cols);
-        pn_l1_apply_kernel<<<mm_cdiv(P * 16, 256), 256, 0, st>>>(points, q[0], q[1], w.sc, w.sh, w.seg, L, P, w.x1p, ar.status());
-        MM_LAUNCH_CHECK();
-        if (timed) mm_timing_end(st);
-      } else if (gen_mid && (i == 1 || i == 2)) {
-        // consumed in place by the next layer's producers
-      } else if (i < 4) {
-        if (timed) mm_timing_begin(st, MM_T_PN_NORM, 0.0, 8.0 * cout[i] * cols);
-        MM_TRY(norm_split(ybuf[i], cout[i], w.sc, w.sh, cout[i], P, 0, w.seg, L, w.xp, st, ar.status()));
-        if (timed) mm_timing_end(st);
-      } else {
-        // second pass of the 1024-wide layer: recompute, GroupNorm + ReLU + per-detection mean in the epilogue
-        // (its 1024 x P activation, 537 MB per frame-pair at cfg4, is never written)
-        MM_CUDA(cudaMemsetAsync(w.segsum, 0, (size_t)ndet * 1024 * sizeof(unsigned long long), st));
-        p.Y = nullptr; p.part = nullptr;
-        p.sc = w.sc; p.sh = w.sh; p.seg = w.seg;
-        if (timed) mm_timing_begin(st, MM_T_PN_L5B, 2.0 * cout[i] * cin[i] * cols, 4.0 * cin[i] * cols);
-        MM_TRY(gemm_tma_launch_mat(p, wp, wps, w.xp, P * cin[i], P, cin[i], tc::OUT_CL, 0, st, w.segsum, nullptr, w.ctab));
-        if (timed) mm_timing_end(st);
-        segsum_mean_cl_kernel<<<mm_cdiv(1024L * ndet, 256), 256, 0, st>>>(w.segsum, det_split, 1024, ndet, w.gmean);
-        MM_LAUNCH_CHECK();
-      }
+  const double cols = (double)P;
+  // layer 1 (3 -> 64): its statistics, then the layer recomputed, normalised and split into x1p
+  const float* const* l1 = &wts->w[MMMOT_W_PN_L1];
+  if (timed) mm_timing_begin(st, MM_T_PN_L1, 2.0 * 64 * 3 * cols, 12.0 * cols);
+  pn_l1_stats_kernel<<<(int)n_tiles, 256, 0, st>>>(points, w.tiles, l1[0], l1[1], w.part);
+  MM_LAUNCH_CHECK();
+  if (timed) mm_timing_end(st);
+  MM_TRY(stats_reduce(w.part, 64, pairs, 0, w.gstart, w.stats, st, 2));
+  MM_TRY(gn_finalize(w.stats, l1[2], l1[3], w.cnt, 0, pairs, 64, 1, w.sc, w.sh, st, 0, 0, status));
+  if (timed) mm_timing_begin(st, MM_T_PN_L1, 0.0, (12.0 + 4.0 * 64) * cols);
+  pn_l1_apply_kernel<<<mm_cdiv(P * 16, 256), 256, 0, st>>>(points, l1[0], l1[1], w.sc, w.sh, w.seg, L, P, w.x1p, status);
+  MM_LAUNCH_CHECK();
+  if (timed) mm_timing_end(st);
+  float* const ys[3] = {w.t0, w.t1, w.t0};             // outputs of layers 2, 3, 4
+  const bool gen_mid = !(mm_debug_flags() & 8192);   // debug bit 13: layers 3, 4 through norm_split + the TMA-fed kernel
+  for (int i = 1; i < 4; i++) {
+    const float* const* q = &wts->w[MMMOT_W_PN_L1 + 4 * i];
+    const int cin = 64, cout = i == 3 ? 128 : 64;
+    GemmP p = gemm_defaults();
+    p.bias = q[1]; p.M = cout; p.K = cin;
+    p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
+    p.Y = ys[i - 1]; p.y_ms = cout;
+    p.part = w.part;
+    const uint4* wp = (const uint4*)wts->w[MMMOT_W_PN_WP1 + i];
+    const float wps = wts->tc_scale[MMMOT_W_PN_WP1 + i];
+    // compulsory traffic: activation in (4 B per element) + fp32 activation out
+    if (timed) mm_timing_begin(st, MM_T_PN_L2 + (i - 1), 2.0 * cout * cin * cols, 4.0 * (cin + cout) * cols);
+    if (gen_mid && i > 1) {
+      // layers 3, 4: GroupNorm + ReLU of the previous layer applied by this contraction's operand producers
+      // (gemm_gen.cuh) straight from its fp32 output: no normalised copy is written
+      MM_TRY((gemm_gen_launch<gen::GEN_NORM>(p, wp, wps, ys[i - 2], cin, w.sc, w.sh, 0, 0, 0, st)));
+    } else {                                                // FP16 hi/lo planes [2][P][cin] via TMA
+      MM_TRY(gemm_tma_launch_mat(p, wp, wps, i == 1 ? w.x1p : w.xp, P * cin, P, cin, tc::OUT_CL, 0, st));
     }
-    {
-      // U[det][512] = gmean[det][1024] Wh[:, 64:]^T  (the per-detection part of point_net.py:27-28's conv1), on the
-      // tensor cores over channels-last rows; its output is directly the [det][512] addend table of the head
-      GemmP p = gemm_defaults();
-      p.M = 512; p.K = 1024;
-      p.S = ndet; p.tiles_per_group = mm_cdiv(ndet, tc::BN); p.num_tiles = p.tiles_per_group;
-      p.x_gs = ndet;
-      p.Y = w.ut; p.y_gs = ndet; p.y_ms = 512;
-      MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WHGP], wts->tc_scale[MMMOT_W_PN_WHGP], w.gmean, 1024,
-                                             nullptr, nullptr, 0, 0, 0, st)));
-    }
-    {
-      const uint4* whp = (const uint4*)wts->w[MMMOT_W_PN_WHAP];
-      const float whs = wts->tc_scale[MMMOT_W_PN_WHAP];
-      MM_TRY(pn_wide_stats(w, h_det_split, det_split, P, pairs, L, n_tiles, w.x1p, 64, wts->w[MMMOT_W_PN_WHAT], whp, whs,
-                           wts->w[MMMOT_W_PN_BH], 512, w.ut, st));
-      MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GHW], wts->w[MMMOT_W_PN_GHB], w.cnt, 0, pairs, 512, 1, w.sc, w.sh, st));
-      // recompute + GroupNorm + ReLU + per-detection mean
-      MM_CUDA(cudaMemsetAsync(w.segsum, 0, (size_t)ndet * 512 * sizeof(unsigned long long), st));
-      GemmP p = gemm_defaults();
-      p.bias = wts->w[MMMOT_W_PN_BH]; p.M = 512; p.K = 64;
-      p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
-      p.Y = nullptr; p.y_ms = 512;
-      p.addend = w.ut; p.seg = w.seg; p.ld_add = 512;
-      p.sc = w.sc; p.sh = w.sh;
-      if (timed) mm_timing_begin(st, MM_T_PN_HEADB, 2.0 * 512 * 64 * (double)P, 4.0 * 64 * (double)P);
-      MM_TRY(gemm_tma_launch_mat(p, whp, whs, w.x1p, P * 64, P, 64, tc::OUT_CL, 0, st, w.segsum, nullptr, w.ctab));
+    if (timed) mm_timing_end(st);
+    MM_TRY(stats_reduce(w.part, cout, pairs, 0, w.gstart, w.stats, st, 2));
+    MM_TRY(gn_finalize(w.stats, q[2], q[3], w.cnt, 0, pairs, cout, 1, w.sc, w.sh, st, 0, 0, status));
+    if (!gen_mid || i == 3) {                           // otherwise consumed in place by the next layer's producers
+      if (timed) mm_timing_begin(st, MM_T_PN_NORM, 0.0, 8.0 * cout * cols);
+      MM_TRY(norm_split(ys[i - 1], cout, w.sc, w.sh, cout, P, 0, w.seg, L, w.xp, st, status));
       if (timed) mm_timing_end(st);
-      segsum_mean_cl_kernel<<<mm_cdiv(512L * ndet, 256), 256, 0, st>>>(w.segsum, det_split, 512, ndet, w.hmean);
-      MM_LAUNCH_CHECK();
     }
-    {
-      // conv2 512 -> 512 over the pair's L detections, GroupNorm(16,512), ReLU (point_net.py:40-41), on the tensor cores
-      const int tpg2 = mm_cdiv(L, tc::BN);
-      GemmP p = gemm_defaults();
-      p.bias = wts->w[MMMOT_W_PN_BO]; p.M = 512; p.K = 512;
-      p.S = L; p.tiles_per_group = tpg2; p.num_tiles = tpg2 * pairs;
-      p.x_gs = L;
-      p.Y = w.o; p.y_gs = L; p.y_ms = 512;
-      p.part = w.part;
-      MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WOP], wts->tc_scale[MMMOT_W_PN_WOP], w.hmean, 512,
-                                             nullptr, nullptr, 0, 0, 0, st)));
-      MM_TRY(stats_reduce(w.part, 512, pairs, tpg2, nullptr, w.stats, st, 2));
-      MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GOW], wts->w[MMMOT_W_PN_GOB], nullptr, L, pairs, 512, 32, w.sc, w.sh, st));
-      pointnet_out_cl_kernel<<<dim3(mm_cdiv(L, 32), 16, pairs), dim3(32, 8), 0, st>>>(w.o, w.sc, w.sh, L, feats);
-      MM_LAUNCH_CHECK();
-      return 0;
-    }
-  } else {
+  }
+  const float* const* l5 = &wts->w[MMMOT_W_PN_L1 + 16];
+  MM_TRY(pn_wide_layer(w, h_det_split, det_split, P, pairs, L, n_tiles, w.xp, 128, l5[0],
+                       (const uint4*)wts->w[MMMOT_W_PN_WP1 + 4], wts->tc_scale[MMMOT_W_PN_WP1 + 4], l5[1], 1024, nullptr,
+                       l5[2], l5[3], w.gmean, MM_T_PN_L5B, status, st));
+  {
+    // U[det][512] = gmean[det][1024] Wh[:, 64:]^T  (the per-detection part of point_net.py:27-28's conv1), on the
+    // tensor cores over channels-last rows; its output is directly the [det][512] addend table of the head
+    GemmP p = gemm_defaults();
+    p.M = 512; p.K = 1024;
+    p.S = ndet; p.tiles_per_group = mm_cdiv(ndet, tc::BN); p.num_tiles = p.tiles_per_group;
+    p.x_gs = ndet;
+    p.Y = w.ut; p.y_gs = ndet; p.y_ms = 512;
+    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WHGP], wts->tc_scale[MMMOT_W_PN_WHGP], w.gmean, 1024,
+                                           nullptr, nullptr, 0, 0, 0, st)));
+  }
+  MM_TRY(pn_wide_layer(w, h_det_split, det_split, P, pairs, L, n_tiles, w.x1p, 64, wts->w[MMMOT_W_PN_WHAT],
+                       (const uint4*)wts->w[MMMOT_W_PN_WHAP], wts->tc_scale[MMMOT_W_PN_WHAP], wts->w[MMMOT_W_PN_BH], 512,
+                       w.ut, wts->w[MMMOT_W_PN_GHW], wts->w[MMMOT_W_PN_GHB], w.hmean, MM_T_PN_HEADB, nullptr, st));
+  // conv2 512 -> 512 over the pair's L detections, GroupNorm(16,512), ReLU (point_net.py:40-41), on the tensor cores
+  const int tpg2 = mm_cdiv(L, tc::BN);
+  GemmP p = gemm_defaults();
+  p.bias = wts->w[MMMOT_W_PN_BO]; p.M = 512; p.K = 512;
+  p.S = L; p.tiles_per_group = tpg2; p.num_tiles = tpg2 * pairs;
+  p.x_gs = L;
+  p.Y = w.o; p.y_gs = L; p.y_ms = 512;
+  p.part = w.part;
+  MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WOP], wts->tc_scale[MMMOT_W_PN_WOP], w.hmean, 512,
+                                         nullptr, nullptr, 0, 0, 0, st)));
+  MM_TRY(stats_reduce(w.part, 512, pairs, tpg2, nullptr, w.stats, st, 2));
+  MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GOW], wts->w[MMMOT_W_PN_GOB], nullptr, L, pairs, 512, 32, w.sc, w.sh, st));
+  pointnet_out_cl_kernel<<<dim3(mm_cdiv(L, 32), 16, pairs), dim3(32, 8), 0, st>>>(w.o, w.sc, w.sh, L, feats);
+  MM_LAUNCH_CHECK();
+  return 0;
+}
+
+// FP32 path (also the training forward): channel-major activations [C][P], every layer stored
+int pointnet_fp32(const mmmot_weights* wts, const float* points, const int* det_split, int pairs, int L, long P,
+                  long n_tiles, const PnWs& w, const float* head_mask, float* feats, cudaStream_t st) {
+  const int ndet = pairs * L;
   transpose_points_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(points, w.xt, P);
   MM_LAUNCH_CHECK();
   // trunk: 3 -> 64 -> 64 -> 64 -> 128 -> 1024, each conv + GroupNorm(C,C) over the pair's points + ReLU
+  const int cin[5] = {3, 64, 64, 64, 128}, cout[5] = {64, 64, 64, 128, 1024};
   const float* src[5] = {w.xt, w.y1, w.t0, w.t1, w.t0};
   float* dst[5] = {w.y1, w.t0, w.t1, w.t0, w.big};
   for (int i = 0; i < 5; i++) {
@@ -832,27 +775,87 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
                                                                         512, ndet, L, w.hmean, head_mask);
     MM_LAUNCH_CHECK();
   }
-  }
   // conv2 512 -> 512 over the pair's L detections, GroupNorm(16,512), ReLU (point_net.py:40-41)
-  {
-    GemmP p = gemm_defaults();
-    p.Wt = wts->w[MMMOT_W_PN_WOT]; p.bias = wts->w[MMMOT_W_PN_BO]; p.ldw = 512; p.M = 512; p.K = 512;
-    p.S = L; p.tiles_per_group = mm_cdiv(L, 128); p.num_tiles = p.tiles_per_group * pairs;
-    p.X = w.hmean; p.x_gs = L; p.x_ks = ndet;
-    p.Y = w.o; p.y_gs = L; p.y_ms = ndet;
-    p.part = w.part;
-    MM_TRY(gemm_simt_launch<XM_DIRECT>(p, st));
-    MM_TRY(stats_reduce(w.part, 512, pairs, p.tiles_per_group, nullptr, w.stats, st));
-    MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GOW], wts->w[MMMOT_W_PN_GOB], nullptr, L, pairs, 512, 32,
-                       w.sc, w.sh, st));
-    pointnet_out_kernel<<<mm_cdiv(512L * ndet, 256), 256, 0, st>>>(w.o, w.sc, w.sh, ndet, L, feats);
-    MM_LAUNCH_CHECK();
-  }
+  GemmP p = gemm_defaults();
+  p.Wt = wts->w[MMMOT_W_PN_WOT]; p.bias = wts->w[MMMOT_W_PN_BO]; p.ldw = 512; p.M = 512; p.K = 512;
+  p.S = L; p.tiles_per_group = mm_cdiv(L, 128); p.num_tiles = p.tiles_per_group * pairs;
+  p.X = w.hmean; p.x_gs = L; p.x_ks = ndet;
+  p.Y = w.o; p.y_gs = L; p.y_ms = ndet;
+  p.part = w.part;
+  MM_TRY(gemm_simt_launch<XM_DIRECT>(p, st));
+  MM_TRY(stats_reduce(w.part, 512, pairs, p.tiles_per_group, nullptr, w.stats, st));
+  MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GOW], wts->w[MMMOT_W_PN_GOB], nullptr, L, pairs, 512, 32,
+                     w.sc, w.sh, st));
+  pointnet_out_kernel<<<mm_cdiv(512L * ndet, 256), 256, 0, st>>>(w.o, w.sc, w.sh, ndet, L, feats);
+  MM_LAUNCH_CHECK();
   return 0;
 }
 
+}  // namespace
+
+// engine choice from the per-pair shape only (see appearance.cu)
+static bool pointnet_use_tc(int L) { return mm_engine() == 2 || (mm_engine() == 0 && L >= 16); }
+
+extern "C" size_t mmmot_pointnet_workspace(int pairs, int L, long p_total) {
+  MmArena a(nullptr, 0);
+  carve(a, pairs, L, p_total, pointnet_use_tc(L));
+  return a.off;
+}
+
+extern "C" size_t mmmot_pointnet_train_workspace(int pairs, int L, long p_total) {
+  MmArena a(nullptr, 0);
+  carve(a, pairs, L, p_total, false);
+  return a.off;
+}
+
+// mmmot_debug_stage_layout, stage 2: where mmmot_pointnet_fwd leaves its intermediates (a dry carve; no CUDA call)
+int mm_pointnet_layout(int pairs, int L, long P, size_t* off, int* tensor_cores) {
+  MmArena a(nullptr, 0);
+  const bool use_tc = pointnet_use_tc(L);
+  const PnWs w = carve(a, pairs, L, P, use_tc);
+  const void* const bufs[26] = {w.xt, w.y1, w.t0, w.t1, w.big, w.segsum, w.x1p, w.xp, w.gmean, w.u, w.ut, w.hmean, w.o,
+                                w.sc1, w.sh1, w.sc, w.sh, w.stats, w.mom, w.part, w.gstart, w.sstart, w.seg, w.cnt,
+                                w.tiles, w.ctab};
+  for (int i = 0; i < 26; i++) off[i] = (size_t)reinterpret_cast<uintptr_t>(bufs[i]);
+  off[26] = a.off;
+  if (tensor_cores) *tensor_cores = use_tc ? 1 : 0;
+  return 0;
+}
+
+// train: FP32 engine; head_mask (optional) = the Dropout mask of the head activation, [512][P] with values {0, 1/(1-p)}
+static int pointnet_impl(const mmmot_weights* wts, const float* points, const int* det_split, const int* h_det_split,
+                         int pairs, int L, float* feats, void* workspace, size_t workspace_bytes, void* stream, bool train,
+                         const float* head_mask) {
+  if (!wts || !points || !det_split || !h_det_split || !feats || !workspace || pairs <= 0 || L <= 0)
+    return MMMOT_E_ARG;
+  const bool use_tc = !train && pointnet_use_tc(L);
+  const int tw = use_tc ? tc::BN : 128;
+  PnShape s;
+  MM_TRY(pn_shape(h_det_split, pairs, L, tw, s));
+  MmArena ar(workspace, workspace_bytes);
+  const PnWs w = carve(ar, pairs, L, s.P, use_tc);
+  if (!ar.ok() || s.n_tiles > s.max_tiles) return MMMOT_E_WORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  MM_TRY(pn_tables(det_split, pairs, L, s.P, tw, s.n_tiles, w.cnt, w.gstart, w.tiles, w.seg, use_tc ? w.ctab : nullptr, st));
+  if (use_tc) return pointnet_tc(wts, points, det_split, h_det_split, pairs, L, s.P, s.n_tiles, w, ar.status(), feats, st);
+  return pointnet_fp32(wts, points, det_split, pairs, L, s.P, s.n_tiles, w, head_mask, feats, st);
+}
+
+extern "C" int mmmot_pointnet_fwd(const mmmot_weights* wts, const float* points, const int* det_split,
+                                  const int* h_det_split, int pairs, int L, float* feats,
+                                  void* workspace, size_t workspace_bytes, void* stream) {
+  return pointnet_impl(wts, points, det_split, h_det_split, pairs, L, feats, workspace, workspace_bytes, stream, false, nullptr);
+}
+
+extern "C" int mmmot_pointnet_train_fwd(const mmmot_weights* wts, const float* points, const int* det_split,
+                                        const int* h_det_split, int pairs, int L, const float* head_drop_mask, float* feats,
+                                        void* workspace, size_t workspace_bytes, void* stream) {
+  return pointnet_impl(wts, points, det_split, h_det_split, pairs, L, feats, workspace, workspace_bytes, stream, true,
+                       head_drop_mask);
+}
+
 // PointNet's tables over ragged per-pair point ranges (pn_tables, 256-point tiles as on the tensor-core path), then
-// optionally one matrix-mode contraction on them exactly as pointnet_impl issues it: FP16 planes X[2][P][K], tile
+// optionally one matrix-mode contraction on them exactly as the tensor-core path issues it: FP16 planes X[2][P][K], tile
 // table, and per launch Y / part (statistics), addend (head) or segsum (second passes).
 extern "C" int mmmot_debug_pn_contraction(const int* det_split, const int* h_det_split, int pairs, int L, long max_tiles,
                                           void* tiles, int* cnt, int* gstart, int* seg, void* ctab, long* n_tiles,
@@ -860,31 +863,27 @@ extern "C" int mmmot_debug_pn_contraction(const int* det_split, const int* h_det
                                           float* Y, void* part, const float* addend, int ld_add,
                                           unsigned long long* segsum, const float* sc, const float* sh, void* stream) {
   if (!det_split || !h_det_split || pairs <= 0 || L <= 0 || !tiles || !cnt || !gstart || !seg || !ctab) return MMMOT_E_ARG;
+  PnShape s;
+  MM_TRY(pn_shape(h_det_split, pairs, L, tc::BN, s));
+  if (n_tiles) *n_tiles = s.n_tiles;
+  if (s.n_tiles > max_tiles) return MMMOT_E_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
-  const int ndet = pairs * L;
-  const long P = h_det_split[ndet];
-  if (h_det_split[0] != 0 || P <= 0) return MMMOT_E_SHAPE;
-  for (int d = 0; d < ndet; d++)
-    if (h_det_split[d + 1] <= h_det_split[d]) return MMMOT_E_SHAPE;
-  const long nt = pn_tile_count(h_det_split, pairs, L, tc::BN);
-  if (n_tiles) *n_tiles = nt;
-  if (nt > max_tiles) return MMMOT_E_WORKSPACE;
-  MM_TRY(pn_tables(det_split, pairs, L, P, tc::BN, nt, cnt, gstart, (int4*)tiles, seg, (int4*)ctab, st));
+  MM_TRY(pn_tables(det_split, pairs, L, s.P, tc::BN, s.n_tiles, cnt, gstart, (int4*)tiles, seg, (int4*)ctab, st));
   if (!Wp) return 0;
   if (!Xhi) return MMMOT_E_ARG;
   GemmP p = gemm_defaults();
   p.bias = bias; p.M = M; p.K = K;
-  p.tile_tab = (const int4*)tiles; p.num_tiles = (int)nt;
+  p.tile_tab = (const int4*)tiles; p.num_tiles = (int)s.n_tiles;
   p.Y = Y; p.y_ms = M;
   p.part = (double2*)part;
   p.addend = addend; p.ld_add = ld_add;
   p.sc = sc; p.sh = sh;
   if (addend || segsum) p.seg = seg;
-  return gemm_tma_launch_mat(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, P * K, P, K, tc::OUT_CL, 0, st, segsum, nullptr,
-                             (const int4*)ctab);
+  return gemm_tma_launch_mat(p, (const uint4*)Wp, wp_scale, (const __half*)Xhi, s.P * K, s.P, K, tc::OUT_CL, 0, st, segsum,
+                             nullptr, (const int4*)ctab);
 }
 
-// The GroupNorm statistics of PointNet's widest layers exactly as pointnet_impl computes them (pn_wide_stats under the
+// The GroupNorm statistics of PointNet's widest layers exactly as the tensor-core path computes them (pn_wide_stats under the
 // current debug bits), then gn_finalize.  The workspace is a PointNet one (mmmot_pointnet_workspace(pairs, L, P)).
 extern "C" int mmmot_debug_pn_stats(const int* det_split, const int* h_det_split, int pairs, int L, const void* Xhi, int K,
                                     const float* Wt, const void* Wp, float wp_scale, const float* bias, int M,
@@ -898,18 +897,14 @@ extern "C" int mmmot_debug_pn_stats(const int* det_split, const int* h_det_split
   if (two_pass ? !Wp : !Wt) return MMMOT_E_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   const int ndet = pairs * L;
-  const long P = h_det_split[ndet];
-  if (h_det_split[0] != 0 || P <= 0) return MMMOT_E_SHAPE;
-  for (int d = 0; d < ndet; d++)
-    if (h_det_split[d + 1] <= h_det_split[d]) return MMMOT_E_SHAPE;
-  const long n_tiles = pn_tile_count(h_det_split, pairs, L, tc::BN);
-  const long max_tiles = P / 128 + 2 * pairs + 2;
+  PnShape s;
+  MM_TRY(pn_shape(h_det_split, pairs, L, tc::BN, s));
   MmArena ar(workspace, workspace_bytes);
-  PnWs w = carve(ar, pairs, L, P, max_tiles, true);
-  if (!ar.ok() || n_tiles > max_tiles) return MMMOT_E_WORKSPACE;
-  MM_TRY(pn_tables(det_split, pairs, L, P, tc::BN, n_tiles, w.cnt, w.gstart, w.tiles, w.seg, w.ctab, st));
-  MM_TRY(pn_wide_stats(w, h_det_split, det_split, P, pairs, L, n_tiles, (const __half*)Xhi, K, Wt, (const uint4*)Wp, wp_scale,
-                       bias, M, addend, st));
+  const PnWs w = carve(ar, pairs, L, s.P, true);
+  if (!ar.ok() || s.n_tiles > s.max_tiles) return MMMOT_E_WORKSPACE;
+  MM_TRY(pn_tables(det_split, pairs, L, s.P, tc::BN, s.n_tiles, w.cnt, w.gstart, w.tiles, w.seg, w.ctab, st));
+  MM_TRY(pn_wide_stats(w, h_det_split, det_split, s.P, pairs, L, s.n_tiles, (const __half*)Xhi, K, Wt, (const uint4*)Wp,
+                       wp_scale, bias, M, addend, st));
   MM_TRY(gn_finalize(w.stats, gamma, beta, w.cnt, 0, pairs, M, 1, sc, sh, st));
   if (stats) MM_CUDA(cudaMemcpyAsync(stats, w.stats, (size_t)pairs * M * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
   if (mom && !two_pass)

@@ -53,7 +53,7 @@ recomputed; t0 from t1; big (the head) from y1, sc1 / sh1 and the addend u; gmea
 (its output is overwritten by the head), its statistics carrying the contraction bound, and segment_mean's fp32 lane
 sums (cnt + 2) u mean|r|; u from gmean; hmean from big with the head's statistics recomputed; o, conv2 and feats as above.
 
-CPU tests: the layout query without a device, a coverage guard over every launch in pointnet_impl, and planted
+CPU tests: the layout query without a device, a coverage guard over every launch of the stage, and planted
 defects: each bound accepts a plain fp32 evaluation and rejects pn_l1_apply taking the next pair's sc / sh, a
 per-detection mean divided by n_d + 1, the head taking the neighbouring detection's U row, conv2's GroupNorm taken
 over 16 channels per group instead of 32, and pointnet_out_cl with l and c swapped inside a 32 x 32 tile.
@@ -532,62 +532,73 @@ def test_pointnet_layout_without_device():
         assert lib.mmmot_debug_stage_layout(*args, off, None) == -1, args
 
 
-# Every kernel launch and helper call inside pointnet_impl, in source order, and the checks above that hold its output.
-LAUNCH_SITES = [
-    ("pn_tables", ("tables",)),
-    ("pn_l1_stats_kernel", ("x1p",)),
-    ("pn_wide_stats", ("gmean",)),                      # layer 5 statistics from the moments
-    ("gemm_gen_launch", ("t1", "t0")),                  # layers 3, 4 (GEN_NORM)
-    ("gemm_tma_launch_mat", ("t1",)),                   # layer 2 from x1p
-    ("stats_reduce", ("x1p", "t1", "t0", "xp")),
-    ("gn_finalize", ("x1p", "t1", "t0", "xp", "gmean")),
-    ("pn_l1_apply_kernel", ("x1p",)),
-    ("norm_split", ("xp",)),
-    ("gemm_tma_launch_mat", ("gmean",)),                # layer 5 recompute + per-detection sums
-    ("segsum_mean_cl_kernel", ("gmean",)),
-    ("gemm_gen_launch", ("ut",)),
-    ("pn_wide_stats", ("hmean",)),
-    ("gn_finalize", ("hmean",)),
-    ("gemm_tma_launch_mat", ("hmean",)),
-    ("segsum_mean_cl_kernel", ("hmean",)),
-    ("gemm_gen_launch", ("o",)),
-    ("stats_reduce", ("conv2_stats",)),
-    ("gn_finalize", ("conv2_affine",)),
-    ("pointnet_out_cl_kernel", ("feats",)),
-    ("transpose_points_kernel", ("xt",)),
-    ("gemm_simt_launch", ("y1",)),
-    ("gemm_simt_launch", ("t1", "t0", "gmean")),
-    ("stats_reduce", ("sc1_sh1", "t1", "t0", "gmean")),
-    ("gn_finalize", ("sc1_sh1", "t1", "t0", "gmean")),
-    ("segment_mean_kernel", ("gmean",)),
-    ("gemm_simt_launch", ("u",)),
-    ("gemm_simt_launch", ("big",)),
-    ("stats_reduce", ("hmean",)),
-    ("gn_finalize", ("hmean",)),
-    ("segment_mean_kernel", ("hmean",)),
-    ("gemm_simt_launch", ("o",)),
-    ("stats_reduce", ("conv2_stats",)),
-    ("gn_finalize", ("conv2_affine",)),
-    ("pointnet_out_kernel", ("feats",)),
-]
+# The functions the stage runs and, per function, every kernel launch and helper call in its body, in source order, with
+# the checks above that hold its output.  A call of pn_wide_layer counts as a site of the layer it runs.
+LAUNCH_SITES = {
+    "pointnet_impl": [("pn_tables", ("tables",))],
+    "pointnet_tc": [
+        ("pn_l1_stats_kernel", ("x1p",)),
+        ("stats_reduce", ("x1p",)),
+        ("gn_finalize", ("x1p",)),
+        ("pn_l1_apply_kernel", ("x1p",)),
+        ("gemm_gen_launch", ("t1", "t0")),              # layers 3, 4 (GEN_NORM)
+        ("gemm_tma_launch_mat", ("t1",)),               # layer 2 from x1p
+        ("stats_reduce", ("t1", "t0", "xp")),
+        ("gn_finalize", ("t1", "t0", "xp")),
+        ("norm_split", ("xp",)),
+        ("pn_wide_layer", ("gmean",)),                  # layer 5
+        ("gemm_gen_launch", ("ut",)),
+        ("pn_wide_layer", ("hmean",)),                  # head
+        ("gemm_gen_launch", ("o",)),
+        ("stats_reduce", ("conv2_stats",)),
+        ("gn_finalize", ("conv2_affine",)),
+        ("pointnet_out_cl_kernel", ("feats",)),
+    ],
+    "pn_wide_layer": [
+        ("pn_wide_stats", ("gmean", "hmean")),          # statistics from the moments
+        ("gn_finalize", ("gmean", "hmean")),
+        ("gemm_tma_launch_mat", ("gmean", "hmean")),    # recompute + per-detection sums
+        ("segsum_mean_cl_kernel", ("gmean", "hmean")),
+    ],
+    "pointnet_fp32": [
+        ("transpose_points_kernel", ("xt",)),
+        ("gemm_simt_launch", ("y1",)),
+        ("gemm_simt_launch", ("t1", "t0", "gmean")),
+        ("stats_reduce", ("sc1_sh1", "t1", "t0", "gmean")),
+        ("gn_finalize", ("sc1_sh1", "t1", "t0", "gmean")),
+        ("segment_mean_kernel", ("gmean",)),
+        ("gemm_simt_launch", ("u",)),
+        ("gemm_simt_launch", ("big",)),
+        ("stats_reduce", ("hmean",)),
+        ("gn_finalize", ("hmean",)),
+        ("segment_mean_kernel", ("hmean",)),
+        ("gemm_simt_launch", ("o",)),
+        ("stats_reduce", ("conv2_stats",)),
+        ("gn_finalize", ("conv2_affine",)),
+        ("pointnet_out_kernel", ("feats",)),
+    ],
+}
 
 
-def impl_launches():
+def impl_launches(func):
     """(name) of every `kernel<<<` launch and every gemm_*_launch*, norm_split, stats_reduce, gn_finalize,
-    pn_wide_stats and pn_tables call in the body of pointnet_impl, in source order."""
+    pn_wide_stats, pn_wide_layer and pn_tables call in the body of the function func of pointnet.cu, in source order."""
     src = open(os.path.join(CSRC, "pointnet.cu")).read()
-    start = src.index("{", src.index("static int pointnet_impl(", src.index("static int pointnet_impl(") + 1))
-    body = src[start:src.index("\n}\n", start)]
+    defs = list(re.finditer(rf"^(?:static )?int {func}\([^;{{]*\)\s*{{", src, re.M))
+    assert len(defs) == 1, (func, len(defs))
+    body = src[defs[0].end():src.index("\n}\n", defs[0].end())]
     body = re.sub(r"//[^\n]*", "", body)
-    pat = r"\b(\w+)(?:<[^<>;()]*>)?<<<|\b(gemm_\w+_launch\w*|norm_split|stats_reduce|gn_finalize|pn_wide_stats|pn_tables)\s*[<(]"
+    pat = (r"\b(\w+)(?:<[^<>;()]*>)?<<<"
+           r"|\b(gemm_\w+_launch\w*|norm_split|stats_reduce|gn_finalize|pn_wide_stats|pn_wide_layer|pn_tables)\s*[<(]")
     return [m.group(1) or m.group(2) for m in re.finditer(pat, body)]
 
 
-def test_launch_coverage_guard():
-    """Every launch in pointnet_impl maps to a check of this file: a launch added, removed or reordered without its
-    entry in LAUNCH_SITES fails here, and every check named there is one the GPU test fills."""
-    assert impl_launches() == [s[0] for s in LAUNCH_SITES]
-    named = {c for _, cs in LAUNCH_SITES for c in cs}
+def test_stage_launch_coverage_guard():
+    """Every launch in the functions the stage runs maps to a check of this file: a launch added, removed or reordered
+    without its entry in LAUNCH_SITES fails here, and every check named there is one the GPU test fills."""
+    for func, sites in LAUNCH_SITES.items():
+        assert impl_launches(func) == [s[0] for s in sites], func
+    named = {c for sites in LAUNCH_SITES.values() for _, cs in sites for c in cs}
     assert named <= set(TC_CHECKS) | set(FP32_CHECKS), named - set(TC_CHECKS) - set(FP32_CHECKS)
     assert (set(TC_CHECKS) | set(FP32_CHECKS)) - {"tables"} <= named
 
