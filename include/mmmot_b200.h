@@ -455,10 +455,10 @@ int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const flo
  * stage_layout: where one run of a stage leaves its intermediates in the caller's workspace, computed on the host without
  *   any CUDA call from the same carve of the workspace the stage runs.  stage 0 = mmmot_affinity_fwd of shape
  *   (pairs, n, m), stage 1 = mmmot_fusion_det_fwd of shape (pairs, L = n; m ignored), stage 2 = mmmot_pointnet_fwd of
- *   shape (pairs, L = n, P = m points in all).  offsets (host) receives byte
+ *   shape (pairs, L = n, P = m points in all).  offsets (host, room for 32 entries whatever the stage) receives byte
  *   offsets from the start of the workspace, G = 3 pairs groups g = pair*3 + stack, NM = n*m, ldv = G*(n + m),
  *   "TC" the tensor-core path, "FP32" the FP32-engine path:
- *     stage 0, 16 offsets:
+ *     stage 0, 31 offsets (entries [16].. are scratch the stage reuses; each holds what its last writer left):
  *       [0] y01   first layer [conv1.0 ; new/end conv0]: TC [g*NM + i*m + j][1024], FP32 [g][1024][NM]
  *       [1] y3    third affinity layer: TC [g*NM + s][128], FP32 [g][128][NM]
  *       [2] z     link logits [g][NM] (softmax_mode != NONE; with NONE they go straight to link)
@@ -470,6 +470,24 @@ int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const flo
  *       [9] h2    second new/end MLP layer: TC [col][128], FP32 [128][ldv]
  *       [10] nsc2 [11] nsh2  its GroupNorm affine [2g + (0 new | 1 end)][128]
  *       [12] rmax [13] rsum  softmax over j per row [g][n];  [14] cmax [15] csum  over i per column [g][m]
+ *       [16] y2   second affinity layer (before its GroupNorm): TC [g*NM + s][512], FP32 [g][512][NM]
+ *       [17] sc1 [18] sh1   GroupNorm(512, 512) affine of the first affinity layer (channels 0..511 of y01) [g][512]
+ *       [19] sc2 [20] sh2   GroupNorm(512, 512) affine of the second affinity layer [g][512]
+ *       [21] h1   first new/end MLP layer (before its GroupNorm): TC [col][512], FP32 [512][ldv]
+ *       [22] nsc1 [23] nsh1  its GroupNorm(1, 512) affine [2g + (0 new | 1 end)][512]
+ *       [24] stats  fp64 (sum, sum of squares) [G][1024][2], written by layers 1, 2 and 3 in turn: at the end the
+ *                 first [g][128][2] hold the third layer's
+ *       [25] nstats fp64 [2G][512][2], written by both new/end layers: at the end the first [2g + e][128][2] hold
+ *                 the second layer's
+ *       [26] part  fp64 (sum, sum of squares) per column-tile partial, [tile*k + half][channel] with k = 2 on TC
+ *                 (256-column tiles, two halves) and 1 on FP32 (128-column tiles), tiles g*tpg .. (g+1)*tpg - 1 of
+ *                 group g; at the end the third layer's [G*tpg*k][128]
+ *       [27] npart  the same for the new/end tiles of the table: at the end the second new/end layer's
+ *                 [ne_tiles*k][128]
+ *       [28] tiles  int4 {group 2g + e, first column col, length, 0}: per g, the new columns in tiles of 256 (TC) or
+ *                 128 (FP32), then the end columns
+ *       [29] cnt  int [2G] columns per new/end group (m new, n end)   [30] gstart  int [2G + 1] first tile per group
+ *       The statistics of the first affinity layer, the second and the first new/end layer do not survive the stage.
  *     stage 1, 2 offsets:
  *       [0] f3    TC only: detection-major rows [(pair*L + l)*3 + stack][512]
  *       [1] h2    second w_det layer (after its ReLU): TC [(pair*L + l)*3 + stack][256], FP32 [g][256][L]

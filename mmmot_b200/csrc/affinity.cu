@@ -311,9 +311,11 @@ extern "C" size_t mmmot_affinity_workspace(int pairs, int n, int m) {
 int mm_affinity_layout(int pairs, int n, int m, size_t* off, int* tensor_cores) {
   MmArena a(nullptr, 0);
   const AfWs w = carve(a, pairs, n, m);
-  const void* const bufs[16] = {w.y01, w.y3, w.z, w.fcl, w.sc0, w.sh0, w.sc3, w.sh3,
-                                w.v, w.h2, w.nsc2, w.nsh2, w.rmax, w.rsum, w.cmax, w.csum};
-  for (int i = 0; i < 16; i++) off[i] = (size_t)reinterpret_cast<uintptr_t>(bufs[i]);
+  const void* const bufs[31] = {w.y01, w.y3, w.z, w.fcl, w.sc0, w.sh0, w.sc3, w.sh3,
+                                w.v, w.h2, w.nsc2, w.nsh2, w.rmax, w.rsum, w.cmax, w.csum,
+                                w.y2, w.sc1, w.sh1, w.sc2, w.sh2, w.h1, w.nsc1, w.nsh1,
+                                w.stats, w.nstats, w.part, w.npart, w.tiles, w.cnt, w.gstart};
+  for (int i = 0; i < 31; i++) off[i] = (size_t)reinterpret_cast<uintptr_t>(bufs[i]);
   if (tensor_cores) *tensor_cores = affinity_use_tc(n, m) ? 1 : 0;
   return 0;
 }

@@ -9,6 +9,7 @@ import contextlib
 import ctypes
 import math
 import os
+import re
 import zlib
 
 import numpy as np
@@ -26,6 +27,7 @@ EPS = 1e-5                         # GroupNorm / BatchNorm epsilon
 # plans.
 TAU = 2.0 ** -18
 KAPPA, KAPPA1 = 64, 40             # the GroupNorm statistics bound of stats_ratios
+FP64 = 2.0 ** -40                  # fp64 summation and cancellation, far below every other term of a bound
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "mmmot_b200", "csrc")
 KSEG_DEFAULT = 36                  # mmmot_set_kseg default (api.cu)
 ENGINE = {"auto": 0, "fp32": 1, "tc": 2}
@@ -124,7 +126,9 @@ def nan_workspace(lib, nbytes):
 
 # Buffers of mmmot_debug_stage_layout, in the header's order: stage 0 = mmmot_affinity_fwd, 1 = mmmot_fusion_det_fwd,
 # 2 = mmmot_pointnet_fwd (its last entry, `end`, is the workspace size).
-AF_BUFS = ("y01", "y3", "z", "fcl", "sc0", "sh0", "sc3", "sh3", "v", "h2", "nsc2", "nsh2", "rmax", "rsum", "cmax", "csum")
+AF_BUFS = ("y01", "y3", "z", "fcl", "sc0", "sh0", "sc3", "sh3", "v", "h2", "nsc2", "nsh2", "rmax", "rsum", "cmax", "csum",
+           "y2", "sc1", "sh1", "sc2", "sh2", "h1", "nsc1", "nsh1", "stats", "nstats", "part", "npart", "tiles", "cnt",
+           "gstart")
 FD_BUFS = ("f3", "h2")
 PN_BUFS = ("xt", "y1", "t0", "t1", "big", "segsum", "x1p", "xp", "gmean", "u", "ut", "hmean", "o", "sc1", "sh1", "sc",
            "sh", "stats", "mom", "part", "gstart", "sstart", "seg", "cnt", "tiles", "ctab", "end")
@@ -213,10 +217,22 @@ def norm_operand(v, sc, sh):
     return (v.double() * sc.double() + sh.double()).float().clamp_min(0)
 
 
+def pair_operand(f, op, n, m):
+    """f [G][K][Lf] fp32 -> the FP32 engine's pairwise operand [K][G*n*m] (XM.MUL / ABS / SUB), column g*n*m + i*m + j
+    from object i and detection n + j, formed in fp32 as the engine's loader forms it."""
+    s = torch.arange(n * m, device=f.device)
+    a, b = f[:, :, s // m], f[:, :, n + s % m]
+    x = a * b if op == XM.MUL else (a - b) * 0.5
+    if op == XM.ABS:
+        x = x.abs()
+    return x.permute(1, 0, 2).reshape(f.shape[1], -1)
+
+
 def ref_linear(X, A, wt, b):
-    """fp64 X W^T + b and S = A |W|^T + |b| (X, A [cols][K] fp64 cuda): the reference and scale of the TAU bound."""
-    w = wt.double().cuda()
-    bb = b.double().cuda()
+    """fp64 X W^T + b and S = A |W|^T + |b| (X, A [cols][K] fp64, on their device): the reference and scale of the TAU
+    bound."""
+    w = wt.double().to(X.device)
+    bb = b.double().to(X.device)
     return X @ w + bb, A @ w.abs() + bb.abs()
 
 
@@ -263,6 +279,97 @@ def stats_ratios(S1, S2, y, grp, G):
     rm = ((m - mean).abs() / tm.clamp_min(1e-300))[keep]
     cond = (mean.abs() / var.clamp_min(1e-300).sqrt())[keep]
     return float(rv.max()), float(rm.max()), float(cond.max())
+
+
+def group_sum(v, idx, G):
+    """Rows of v [n][C] summed in fp64 into their groups idx [n] -> [G][C]."""
+    return torch.zeros(G, v.shape[1], dtype=torch.float64, device=v.device).index_add_(0, idx, v)
+
+
+def gn_stats(y, grp, G, T=None, kappa=True, cpg=1):
+    """GroupNorm statistics per group of y [n][C] (fp64 reference of the values the kernel summed, which err by at most
+    T), normalisation groups of cpg adjacent channels -> (mean, var, tm, tv) [G][C], each channel carrying its
+    normalisation group's values.
+
+    Per channel the kernel's mean and variance differ from the two-pass fp64 values by at most
+        tm = mean(T) + [KAPPA1 u mean|y|] + FP64 mean|y|,
+        tv = 2 mean(|y - mean| T) + mean(T^2) + [KAPPA u (|mean| mean|y - mean| + var)] + FP64 (mean^2 + var),
+    the bracketed terms (kappa) only where the sums come from a contraction epilogue's fp32 runs (stats_ratios).
+    gn_finalize adds the cpg channel sums of a normalisation group in fp64.  Every channel has the same count, so the
+    group's mean M is the mean over its channels of the channel means m_c and its variance is
+    mean_c [v_c + (m_c - M)^2].  With the channel errors dm_c, dv_c:
+        dM = mean_c dm_c,    dV = mean_c [dv_c + 2 (m_c - M) dm_c] + (mean_c dm_c^2 - (mean_c dm_c)^2),
+    the last bracket in [0, mean_c dm_c^2], so
+        tm_G = mean_c tm_c,  tv_G = mean_c [tv_c + 2 |m_c - M| tm_c + tm_c^2].
+    The channels' FP64 (m_c^2 + v_c) average to FP64 (M^2 + V), which also covers the fp64 sums over the cpg channels."""
+    n, mean, var, mad, may = group_moments(y, grp, G)
+    tm = FP64 * may
+    tv = FP64 * (mean * mean + var)
+    if kappa:
+        tm = tm + KAPPA1 * U * may
+        tv = tv + KAPPA * U * (mean.abs() * mad + var)
+    if T is not None:
+        dev = y - mean[grp]
+        tm = tm + group_sum(T, grp, G) / n
+        tv = tv + (2 * group_sum(dev.abs() * T, grp, G) + group_sum(T * T, grp, G)) / n
+    if cpg == 1:
+        return mean, var, tm, tv
+    C = y.shape[1]
+    per = lambda v: v.view(G, C // cpg, cpg)
+    wide = lambda v: v.repeat_interleave(cpg, 1)
+    M = per(mean).mean(2, keepdim=True)
+    V = (per(var) + (per(mean) - M) ** 2).mean(2)
+    TV = (per(tv) + 2 * (per(mean) - M).abs() * per(tm) + per(tm) ** 2).mean(2)
+    return wide(M[..., 0]), wide(V), wide(per(tm).mean(2)), wide(TV)
+
+
+def gn_apply(y, T, grp, st, gamma, beta):
+    """fmaf(y, sc, sh) of a kernel's GroupNorm before the ReLU, from y [n][C] that errs by at most T (None: exact) and
+    the statistics st of gn_stats -> (z [n][C], Tz, |y a| + |sh|).
+
+    With a = gamma / sqrt(var + eps), sh = beta - mean a, sc_k = fl(a_k), sh_k = fl(beta - mean_k a_k) and
+    |a_k - a| <= |a| er, er = tv / (2 (var + eps)) + FP64, the value errs before the ReLU (1-Lipschitz) by
+        Tz = |a| (T + tm + |y - mean| er) + 8u (|y a| + |sh| + |z|),
+    the last term the fp32 roundings of sc, sh and the fma; |y a| ~ |mean| / std is GroupNorm's own conditioning."""
+    mean, var, tm, tv = st
+    a = gamma / torch.sqrt(var + EPS)
+    sh = beta - mean * a
+    er = tv / (2 * (var + EPS)) + FP64
+    A, SH = a[grp], sh[grp]
+    z = y * A + SH
+    Tz = A.abs() * ((0.0 if T is None else T) + tm[grp] + (y - mean[grp]).abs() * er[grp])
+    mag = (y * A).abs() + SH.abs()
+    return z, Tz + 8 * U * (mag + z.abs()), mag
+
+
+def affine_bound(st, gamma, beta):
+    """gn_finalize's fp32 sc / sh from statistics whose mean and variance err by at most (tm, tv) of st = gn_stats(...)
+    -> (a, sh, Ta, Tsh) [G][C]: the fp64 affine of the reference statistics and the bounds
+        |sc - a| <= |a| (er + u),   |sh - sh_ref| <= |a| tm + |mean a| er + u (|sh| + |mean a|),
+    er = tv / (2 (var + eps)) + FP64 (the relative error of 1 / sqrt(var + eps)), u the final fp32 rounding."""
+    mean, var, tm, tv = st
+    a = gamma / torch.sqrt(var + EPS)
+    er = tv / (2 * (var + EPS)) + FP64
+    sh = beta - mean * a
+    ma = (mean * a).abs()
+    return a, sh, a.abs() * (er + U), a.abs() * tm + ma * er + U * (sh.abs() + ma)
+
+
+def gn_affine(stats, gamma, beta, count, cpg=1):
+    """gn_finalize of GroupNorm(C / cpg, C) from the stored fp64 stats [G][C][2] (sum, sum of squares) over `count`
+    columns per group (a number, or a tensor [G]) -> (sc, sh, Tsc, Tsh) [G][C]: fp64 from the stored sums, the kernel
+    then rounds each once to fp32 (u |sc|, u |sh|); its fp64 arithmetic adds FP64 |a| (mean^2 + var) / (var + eps) and
+    likewise for sh."""
+    G, C = stats.shape[:2]
+    s = stats.view(G, C // cpg, cpg, 2).sum(2)
+    n = (count.double().view(G, 1) if torch.is_tensor(count) else float(count)) * cpg
+    mean = s[..., 0] / n
+    var = (s[..., 1] / n - mean * mean).clamp_min(0)
+    mean, var = mean.repeat_interleave(cpg, 1), var.repeat_interleave(cpg, 1)
+    a = gamma / torch.sqrt(var + EPS)
+    sh = beta - mean * a
+    cond = (mean * mean + var) / (var + EPS)
+    return a, sh, U * a.abs() + FP64 * a.abs() * cond, U * sh.abs() + FP64 * (mean * a).abs() * (1 + cond)
 
 
 def reduce_parts(part, slot_group, G):
@@ -333,14 +440,15 @@ def pn_host_tables(split, pairs, L):
     return tiles, seg, ctab, cnt, gstart
 
 
-def ne_tiles_host(G, n, m, gap):
-    """The new/end MLP's table (affinity.cu ne_tiles_kernel): group 2g = the m new columns, 2g+1 = the n end columns
-    of pair-stack g, here with `gap` unused rows after every g."""
+def ne_tiles_host(G, n, m, gap, tw=BN):
+    """The new/end MLP's table (affinity.cu ne_tiles_kernel) in tiles of tw columns (BN on the tensor cores, 128 on the
+    FP32 engine): group 2g = the m new columns, 2g+1 = the n end columns of pair-stack g, here with `gap` unused rows
+    after every g."""
     tiles = []
     for g in range(G):
         base = g * (n + m + gap)
-        tiles += [(2 * g, base + c, min(BN, m - c)) for c in range(0, m, BN)]
-        tiles += [(2 * g + 1, base + m + c, min(BN, n - c)) for c in range(0, n, BN)]
+        tiles += [(2 * g, base + c, min(tw, m - c)) for c in range(0, m, tw)]
+        tiles += [(2 * g + 1, base + m + c, min(tw, n - c)) for c in range(0, n, tw)]
     return tiles, G * (n + m + gap)
 
 
@@ -382,6 +490,19 @@ def bench_n_imgs(pairs, L):
         if pairs % c:
             chunks.add(pairs % c)
     return sorted(k * L for k in chunks)
+
+
+# ------------------------------------------------------------------------------------------------ launch sites
+def impl_launches(src_file, func, helpers):
+    """(name) of every `kernel<<<` launch and every call of one of `helpers` (regular expressions of function names) in
+    the body of the function func of csrc/src_file, in source order, comments skipped."""
+    src = open(os.path.join(CSRC, src_file)).read()
+    defs = list(re.finditer(rf'^(?:static |extern "C" )?int {func}\([^;{{]*\)\s*{{', src, re.M))
+    assert len(defs) == 1, (func, len(defs))
+    body = src[defs[0].end():src.index("\n}\n", defs[0].end())]
+    body = re.sub(r"//[^\n]*", "", body)
+    pat = rf"\b(\w+)(?:<[^<>;()]*>)?<<<|\b({'|'.join(helpers)})\s*[<(]"
+    return [m.group(1) or m.group(2) for m in re.finditer(pat, body)]
 
 
 # ------------------------------------------------------------------------------------------------ generated-operand engine

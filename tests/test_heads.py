@@ -83,15 +83,23 @@ CFG_N = {"cfg2": 32, "cfg3": 64, "cfg4": 128, "cfg5": 256}
 
 # ------------------------------------------------------------------------------------------------ layout
 def af_sizes(pairs, n, m):
-    """Floats in each affinity intermediate (the shapes the header documents)."""
+    """Bytes of each affinity intermediate (the shapes and types the header documents; part, npart and tiles sized for
+    the larger of the two paths' tilings)."""
     G, NM, ldv = 3 * pairs, n * m, 3 * pairs * (n + m)
-    return dict(y01=G * 1024 * NM, y3=G * 128 * NM, z=G * NM, fcl=G * (n + m) * 512, sc0=G * 512, sh0=G * 512,
-                sc3=G * 128, sh3=G * 128, v=512 * ldv, h2=128 * ldv, nsc2=2 * G * 128, nsh2=2 * G * 128,
-                rmax=G * n, rsum=G * n, cmax=G * m, csum=G * m)
+    cd = lambda a, b: -(-a // b)
+    ntile = G * (cd(n, 128) + cd(m, 128))
+    f32 = dict(y01=G * 1024 * NM, y3=G * 128 * NM, z=G * NM, fcl=G * (n + m) * 512, sc0=G * 512, sh0=G * 512,
+               sc3=G * 128, sh3=G * 128, v=512 * ldv, h2=128 * ldv, nsc2=2 * G * 128, nsh2=2 * G * 128,
+               rmax=G * n, rsum=G * n, cmax=G * m, csum=G * m, y2=G * 512 * NM, sc1=G * 512, sh1=G * 512, sc2=G * 512,
+               sh2=G * 512, h1=512 * ldv, nsc1=2 * G * 512, nsh1=2 * G * 512)
+    size = {k: 4 * v for k, v in f32.items()}
+    size.update(stats=8 * G * 1024 * 2, nstats=8 * 2 * G * 512 * 2, part=16 * G * 2 * cd(NM, 256) * 1024,
+                npart=16 * 2 * ntile * 512, tiles=16 * ntile, cnt=4 * 2 * G, gstart=4 * (2 * G + 1))
+    return size
 
 
 def fd_sizes(pairs, L):
-    return dict(f3=3 * pairs * 512 * L, h2=3 * pairs * 256 * L)
+    return dict(f3=4 * 3 * pairs * 512 * L, h2=4 * 3 * pairs * 256 * L)
 
 
 # ------------------------------------------------------------------------------------------------ fp64 bounds
@@ -247,7 +255,7 @@ def test_stage_layout_without_device():
                 lay, tc = stage_layout(lib, 1, pairs, L)
                 assert tc == (det_path(L, engine) == "tc"), (engine, L)
                 _disjoint_inside(lay, fd_sizes(pairs, L), int(lib.mmmot_fusion_det_workspace(pairs, L)))
-    off = (ctypes.c_size_t * 16)()
+    off = (ctypes.c_size_t * 32)()
     for args in ((3, 1, 4, 4), (0, 0, 4, 4), (0, 1, 0, 4), (0, 1, 4, 0), (1, 1, 0, 0), (-1, 1, 4, 4)):
         assert lib.mmmot_debug_stage_layout(*args, off, None) == -1, args
     assert lib.mmmot_debug_stage_layout(0, 1, 4, 4, None, None) == -1
@@ -259,7 +267,7 @@ def test_stage_layout_without_device():
 
 
 def _disjoint_inside(lay, sizes, ws_bytes):
-    spans = sorted((lay[k], lay[k] + 4 * sizes[k], k) for k in lay)
+    spans = sorted((lay[k], lay[k] + sizes[k], k) for k in lay)
     assert spans[0][0] >= 256, spans[0]
     assert spans[-1][1] <= ws_bytes, (spans[-1], ws_bytes)
     for (a0, a1, ka), (b0, b1, kb) in zip(spans, spans[1:]):
@@ -370,7 +378,7 @@ def test_affinity_tail_vs_fp64(n, m, pairs, engine, op, sm, end, peaky):
         assert_written(buf, cnt, what)
     size = af_sizes(pairs, n, m)
     wsv = Workspace(ws, lay)
-    B = {k: wsv.view(k, size[k]) for k in AF_BUFS}
+    B = {k: wsv.view(k, size[k] // 4) for k in AF_BUFS[:16]}     # the fp32 buffers this test reads
     r = {}
     # fcl: the channels-last copy of the feature stacks on the tensor-core path, untouched on the FP32 path
     if tc:
@@ -458,7 +466,7 @@ def test_det_score_vs_fp64(L, pairs, engine, flags, fusion):
     assert bool(torch.isfinite(feats[:, 2]).all()), "stack 2 not written"
     size = fd_sizes(pairs, L)
     wsv = Workspace(ws, lay)
-    f3, h2 = wsv.view("f3", size["f3"]), wsv.view("h2", size["h2"])
+    f3, h2 = wsv.view("f3", size["f3"] // 4), wsv.view("h2", size["h2"] // 4)
     if tc:
         f3 = f3.view(pairs, L, 3, 512)
         for s in range(3):

@@ -60,22 +60,20 @@ over 16 channels per group instead of 32, and pointnet_out_cl with l and c swapp
 """
 import ctypes
 import functools
-import os
-import re
 
 import numpy as np
 import pytest
 import torch
 
-from kernel_kit import (CSRC, ENGINE, EPS, KAPPA, KAPPA1, PN_BUFS, TAU, TINY, U, Workspace, case_seed, contraction_bound,
-                        eval_net, group_moments, lib_state, nan_output, nan_workspace, norm_operand, pn_host_tables,
-                        ref_linear, report, stage_layout, stats_ratios, vp, worst_ratio)
+from kernel_kit import (ENGINE, EPS, FP64, PN_BUFS, TAU, TINY, U, Workspace, affine_bound, case_seed,
+                        contraction_bound, eval_net, gn_affine, gn_apply, gn_stats, group_moments, group_sum, impl_launches,
+                        lib_state, nan_output, nan_workspace, norm_operand, pn_host_tables, ref_linear, report,
+                        stage_layout, stats_ratios, vp, worst_ratio)
 from mmmot_b200 import _lib
 from mmmot_b200.synthetic import synthetic_state_dict
 from mmmot_b200.weights import prepare
 
 gpu = pytest.mark.gpu
-FP64 = 2.0 ** -40
 MOM = 2.0 ** -18                   # S2 of the moments kernel (test_pn_moments.py)
 FIX = 2.0 ** -33                   # one rounding to 2^-32 fixed point
 W = _lib.W
@@ -103,46 +101,13 @@ def _align(n):
 
 
 # ------------------------------------------------------------------------------------------------ fp64 bounds
-def _acc(v, idx, G):
-    return torch.zeros(G, v.shape[1], dtype=torch.float64, device=v.device).index_add_(0, idx, v)
-
-
-def gn_stats(y, grp, G, T=None, kappa=True):
-    """GroupNorm(C, C) statistics per group of y [n][C] (fp64 reference of the values the kernel summed, which err by at
-    most T) -> (mean, var, tm, tv) [G][C] (module docstring)."""
-    n, mean, var, mad, may = group_moments(y, grp, G)
-    tm = FP64 * may
-    tv = FP64 * (mean * mean + var)
-    if kappa:
-        tm = tm + KAPPA1 * U * may
-        tv = tv + KAPPA * U * (mean.abs() * mad + var)
-    if T is not None:
-        dev = y - mean[grp]
-        tm = tm + _acc(T, grp, G) / n
-        tv = tv + (2 * _acc(dev.abs() * T, grp, G) + _acc(T * T, grp, G)) / n
-    return mean, var, tm, tv
-
-
 def mom_stats(y, XW, grp, G, cross=None):
     """Statistics from the input moments: y [n][C] the fp64 reference, XW = |x| @ |W| -> (mean, var, tm, tv)."""
     n, mean, var, _, may = group_moments(y, grp, G)
-    tv = 1.01 * MOM * _acc(XW * XW, grp, G) / n + FP64 * (mean * mean + var)
+    tv = 1.01 * MOM * group_sum(XW * XW, grp, G) / n + FP64 * (mean * mean + var)
     if cross is not None:
         tv = tv + cross
-    return mean, var, FP64 * (_acc(XW, grp, G) / n + may), tv
-
-
-def gn_apply(y, T, grp, st, gamma, beta):
-    """fmaf(y, sc, sh) of the kernel's GroupNorm before the ReLU -> (z [n][C], Tz, |y a| + |sh|)."""
-    mean, var, tm, tv = st
-    a = gamma / torch.sqrt(var + EPS)
-    sh = beta - mean * a
-    er = tv / (2 * (var + EPS)) + FP64
-    A, SH = a[grp], sh[grp]
-    z = y * A + SH
-    Tz = A.abs() * ((0.0 if T is None else T) + tm[grp] + (y - mean[grp]).abs() * er[grp])
-    mag = (y * A).abs() + SH.abs()
-    return z, Tz + 8 * U * (mag + z.abs()), mag
+    return mean, var, FP64 * (group_sum(XW, grp, G) / n + may), tv
 
 
 def split_bound(z):
@@ -152,30 +117,16 @@ def split_bound(z):
 def seg_mean_tc(z, Tz, mag, seg, cnt):
     """Per-detection mean of relu(z) through the 2^-32 fixed-point segment sums -> (ref [ndet][C], bound)."""
     nd = cnt.shape[0]
-    ref = _acc(z.clamp_min(0), seg, nd) / cnt
-    return ref, (_acc(Tz, seg, nd) + 40 * U * _acc(mag, seg, nd)) / cnt + FIX + U * ref.abs()
+    ref = group_sum(z.clamp_min(0), seg, nd) / cnt
+    return ref, (group_sum(Tz, seg, nd) + 40 * U * group_sum(mag, seg, nd)) / cnt + FIX + U * ref.abs()
 
 
 def seg_mean_fp32(z, Tz, seg, cnt):
     """segment_mean_kernel: fp32 lane sums of relu(z) over the detection, then the division."""
     nd = cnt.shape[0]
     r = z.clamp_min(0)
-    ref = _acc(r, seg, nd) / cnt
-    return ref, _acc(Tz, seg, nd) / cnt + (cnt + 2) * U * _acc(r, seg, nd) / cnt + U * ref.abs()
-
-
-def conv2_affine(stats, gamma, beta, L, cpg=32):
-    """gn_finalize of GroupNorm(512 / cpg, 512) over L detections from stats [pairs][512][2] -> (sc, sh, Tsc, Tsh)."""
-    pairs = stats.shape[0]
-    s = stats.view(pairs, 512 // cpg, cpg, 2).sum(2)
-    n = float(L * cpg)
-    mean = s[..., 0] / n
-    var = (s[..., 1] / n - mean * mean).clamp_min(0)
-    mean, var = mean.repeat_interleave(cpg, 1), var.repeat_interleave(cpg, 1)
-    a = gamma / torch.sqrt(var + EPS)
-    sh = beta - mean * a
-    cond = (mean * mean + var) / (var + EPS)
-    return a, sh, U * a.abs() + FP64 * a.abs() * cond, U * sh.abs() + FP64 * (mean * a).abs() * (1 + cond)
+    ref = group_sum(r, seg, nd) / cnt
+    return ref, group_sum(Tz, seg, nd) / cnt + (cnt + 2) * U * group_sum(r, seg, nd) / cnt + U * ref.abs()
 
 
 def out_ref(o, sc, sh):
@@ -320,7 +271,7 @@ def _check_conv2(d, o, r):
     r["conv2_stats"] = max(rv, rm)
     sc = W.view("sc", pairs * 1024)[:pairs * 512].view(pairs, 512)
     sh = W.view("sh", pairs * 1024)[:pairs * 512].view(pairs, 512)
-    a, b, Ta, Tb = conv2_affine(stats, wt["PN_GOW"], wt["PN_GOB"], L)
+    a, b, Ta, Tb = gn_affine(stats, wt["PN_GOW"], wt["PN_GOB"], L, 32)
     r["conv2_affine"] = max(worst_ratio(sc, a, Ta), worst_ratio(sh, b, Tb))
     ref, T = out_ref(o.view(pairs, L, 512), sc, sh)
     r["feats"] = worst_ratio(d["f"][:, 1], ref, T)
@@ -386,9 +337,9 @@ def check_tc(d):
     hm = W.owned("hmean", nd * 512).view(nd, 512)
     WhA, bh = wt["PN_WHAT"], wt["PN_BH"]
     ad = ut.double() + bh                                             # a_d of the moments kernel
-    n_p = _acc(cnt, torch.arange(nd, device="cuda") // L, pairs)
-    abar = _acc(cnt * ad, torch.arange(nd, device="cuda") // L, pairs) / n_p
-    cross = 2 * _acc(cnt * (ad - abar[torch.arange(nd, device="cuda") // L]).abs(), torch.arange(nd, device="cuda") // L,
+    n_p = group_sum(cnt, torch.arange(nd, device="cuda") // L, pairs)
+    abar = group_sum(cnt * ad, torch.arange(nd, device="cuda") // L, pairs) / n_p
+    cross = 2 * group_sum(cnt * (ad - abar[torch.arange(nd, device="cuda") // L]).abs(), torch.arange(nd, device="cuda") // L,
                      pairs) / n_p * FIX * WhA.abs().sum(0)
     r["hmean"] = 0.0
     for c0 in range(0, 512, 128):
@@ -428,14 +379,10 @@ def check_fp32(d):
     ref, T = contraction_bound(W1, d["pts"].T.contiguous(), b1)
     r["y1"] = worst_ratio(y1, ref, T)
     y = y1.double().T
-    mean, var, tm, tv = gn_stats(y, grp, pairs)
-    a = g1 / torch.sqrt(var + EPS)
-    er = tv / (2 * (var + EPS)) + FP64
+    a, sh, Ta, Tsh = affine_bound(gn_stats(y, grp, pairs), g1, be1)
     sc1 = W.owned("sc1", pairs * 64).view(pairs, 64)
     sh1 = W.owned("sh1", pairs * 64).view(pairs, 64)
-    r["sc1_sh1"] = max(worst_ratio(sc1, a, a.abs() * er + U * a.abs()),
-                       worst_ratio(sh1, be1 - mean * a, a.abs() * tm + (mean * a).abs() * er
-                                   + U * ((be1 - mean * a).abs() + (mean * a).abs())))
+    r["sc1_sh1"] = max(worst_ratio(sc1, a, Ta), worst_ratio(sh1, sh, Tsh))
     # t1: layers 2 (recomputed from the stored y1, sc1, sh1) and 3
     W2, b2, g2, be2 = lyr[1]
     W3, b3, g3, be3 = lyr[2]
@@ -580,24 +527,15 @@ LAUNCH_SITES = {
 }
 
 
-def impl_launches(func):
-    """(name) of every `kernel<<<` launch and every gemm_*_launch*, norm_split, stats_reduce, gn_finalize,
-    pn_wide_stats, pn_wide_layer and pn_tables call in the body of the function func of pointnet.cu, in source order."""
-    src = open(os.path.join(CSRC, "pointnet.cu")).read()
-    defs = list(re.finditer(rf"^(?:static )?int {func}\([^;{{]*\)\s*{{", src, re.M))
-    assert len(defs) == 1, (func, len(defs))
-    body = src[defs[0].end():src.index("\n}\n", defs[0].end())]
-    body = re.sub(r"//[^\n]*", "", body)
-    pat = (r"\b(\w+)(?:<[^<>;()]*>)?<<<"
-           r"|\b(gemm_\w+_launch\w*|norm_split|stats_reduce|gn_finalize|pn_wide_stats|pn_wide_layer|pn_tables)\s*[<(]")
-    return [m.group(1) or m.group(2) for m in re.finditer(pat, body)]
+PN_HELPERS = (r"gemm_\w+_launch\w*", "norm_split", "stats_reduce", "gn_finalize", "pn_wide_stats", "pn_wide_layer",
+              "pn_tables")
 
 
 def test_stage_launch_coverage_guard():
     """Every launch in the functions the stage runs maps to a check of this file: a launch added, removed or reordered
     without its entry in LAUNCH_SITES fails here, and every check named there is one the GPU test fills."""
     for func, sites in LAUNCH_SITES.items():
-        assert impl_launches(func) == [s[0] for s in sites], func
+        assert impl_launches("pointnet.cu", func, PN_HELPERS) == [s[0] for s in sites], func
     named = {c for sites in LAUNCH_SITES.values() for _, cs in sites for c in cs}
     assert named <= set(TC_CHECKS) | set(FP32_CHECKS), named - set(TC_CHECKS) - set(FP32_CHECKS)
     assert (set(TC_CHECKS) | set(FP32_CHECKS)) - {"tables"} <= named
@@ -698,10 +636,10 @@ def test_bounds_reject_planted_defects():
     # conv2's GroupNorm over 16 channels per group instead of 32
     L2 = 40
     o = torch.randn(pairs * L2, 512, generator=g) * 0.7 + torch.randn(512, generator=g) * 0.3
-    stats = torch.stack([_acc(o.double(), torch.arange(pairs * L2) // L2, pairs),
-                         _acc(o.double() ** 2, torch.arange(pairs * L2) // L2, pairs)], -1)
-    a, b, Ta, Tb = conv2_affine(stats, w("PN_GOW"), w("PN_GOB"), L2)
-    a16, b16, _, _ = conv2_affine(stats, w("PN_GOW"), w("PN_GOB"), L2, cpg=16)
+    stats = torch.stack([group_sum(o.double(), torch.arange(pairs * L2) // L2, pairs),
+                         group_sum(o.double() ** 2, torch.arange(pairs * L2) // L2, pairs)], -1)
+    a, b, Ta, Tb = gn_affine(stats, w("PN_GOW"), w("PN_GOB"), L2, 32)
+    a16, b16, _, _ = gn_affine(stats, w("PN_GOW"), w("PN_GOB"), L2, 16)
     out["conv2 fp32"] = max(worst_ratio(a.float(), a, Ta), worst_ratio(b.float(), b, Tb))
     out["conv2 16 per group"] = max(worst_ratio(a16.float(), a, Ta), worst_ratio(b16.float(), b, Tb))
     # pointnet_out_cl with l and c swapped inside each 32 x 32 tile (L = 40: one full tile and an 8-column tail)

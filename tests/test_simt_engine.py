@@ -32,8 +32,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from kernel_kit import (CSRC, XM, case_seed, contraction_bound, nan_output, norm_operand, reduce_parts, report,
-                        stats_ratios, vp, worst_ratio)
+from kernel_kit import (CSRC, XM, case_seed, contraction_bound, nan_output, norm_operand, pair_operand, reduce_parts,
+                        report, stats_ratios, vp, worst_ratio)
 from mmmot_b200 import _lib
 
 gpu = pytest.mark.gpu
@@ -42,16 +42,6 @@ GUARD = 512     # NaN floats past the end of every output buffer
 
 
 # ------------------------------------------------------------------------------------------------ reference
-def pair_operand(f, op, n, m):
-    """f [G][K][Lf] fp32 -> the pairwise operand [K][G*n*m], column g*n*m + i*m + j from object i and detection n + j."""
-    s = torch.arange(n * m, device=f.device)
-    a, b = f[:, :, s // m], f[:, :, n + s % m]
-    x = a * b if op == XM.MUL else (a - b) * 0.5
-    if op == XM.ABS:
-        x = x.abs()
-    return x.permute(1, 0, 2).reshape(f.shape[1], -1)
-
-
 def im2col(x):
     """x [n_img][Cin][H][W] -> the zero-padded 3x3 operand [9*Cin][n_img*H*W], row (ky*3 + kx)*Cin + ci."""
     n_img, cin, h, w = x.shape
