@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define MMMOT_ABI_VERSION 2
+#define MMMOT_ABI_VERSION 3
 
 enum {
   MMMOT_E_ARG = -1,        /* null pointer / non-positive size / unsupported enum */
@@ -118,6 +118,9 @@ typedef struct mmmot_weights {
   /* for the packed tensor-core operands (ids >= MMMOT_W_VGG_WP0): 2^-s, where the packed FP16 tiles
      hold W * 2^s (power-of-two pre-scaling keeps the lo terms in FP16's normal range) */
   float tc_scale[MMMOT_W_COUNT];
+  /* width of PointNet's input points, a property of the checkpoint (point_net.feat.conv1.weight.shape[1]): 3 = xyz,
+     4 = xyz + LiDAR reflectance (reference without_reflectivity: False, modules/tracking_net.py:41) */
+  int point_channels;
 } mmmot_weights;
 
 int mmmot_abi_version(void);
@@ -150,7 +153,9 @@ int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops, int n_img
 /* ---------------------------------------------------------------------------------------------
  * PointNet encoder over ragged per-detection point sets -> stack 1 of feats.
  * Replaces PointNet_v1.forward, reference modules/point_net.py:25-44,115-153.
- *   points     [P_total][3]  xyz, detections concatenated in order
+ *   points     [P_total][C]  C = wts->point_channels: xyz, or xyz + reflectance (16-byte aligned rows), detections
+ *                            concatenated in order; any other point_channels (or misaligned 4-channel points) returns
+ *                            MMMOT_E_ARG before any CUDA call
  *   det_split  [pairs*L + 1] int32 CSR offsets into points (device)
  *   h_det_split same array on the HOST (used only to size the launch; the reference reads it
  *               with .item() per detection, point_net.py:33-35,140-142)
@@ -493,8 +498,9 @@ int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const flo
  *       [1] h2    second w_det layer (after its ReLU): TC [(pair*L + l)*3 + stack][256], FP32 [g][256][L]
  *     stage 2, 27 offsets (carve order; ndet = pairs*L detections, d = pair*L + l; a buffer a path does not use has
  *     size 0 there; sc / sh / stats / part are reused layer after layer and end as conv2's):
- *       [0] xt    FP32: the points channel-major [3][P]
- *       [1] y1    FP32: layer 1 (3 -> 64, before its GroupNorm) [64][P]
+ *       [0] xt    FP32: 3-channel points channel-major [3][P] (4-channel points are transposed into t1 instead, which
+ *                 layer 3 then overwrites; xt stays untouched)
+ *       [1] y1    FP32: layer 1 (C -> 64, before its GroupNorm) [64][P]
  *       [2] t0    TC: layer 4 [P][128];  FP32: layer 4 [128][P]
  *       [3] t1    TC: layer 3 [P][64];   FP32: layer 3 [64][P]
  *       [4] big   FP32: [1024][P], layer 5, whose first 512 rows the head (64 -> 512 + U addend, before its GroupNorm)

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmmmot_sm90a.so")
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "mmmot_b200.h")
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 SCORE_SIGMOID, SCORE_THRESHOLD = 1, 2
 FUSION = {"A": 0, "B": 1, "C": 2}
 AFFINITY = {"multiply": 0, "minus_abs": 1, "minus": 2}
@@ -37,7 +37,7 @@ W = dict(
 
 
 class Weights(ctypes.Structure):
-    _fields_ = [("w", ctypes.c_void_p * W["COUNT"]), ("tc_scale", ctypes.c_float * W["COUNT"])]
+    _fields_ = [("w", ctypes.c_void_p * W["COUNT"]), ("tc_scale", ctypes.c_float * W["COUNT"]), ("point_channels", ctypes.c_int)]
 
 
 class MmmotError(RuntimeError):

@@ -16,33 +16,44 @@
 
 namespace {
 
-__global__ void transpose_points_kernel(const float* __restrict__ pts, float* __restrict__ xt, long P) {
+// xt [C][P] = pts [P][C] transposed (C = 3 or 4 point channels)
+__global__ void transpose_points_kernel(const float* __restrict__ pts, int C, float* __restrict__ xt, long P) {
   long p = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P) return;
-  xt[p] = pts[p * 3];
-  xt[P + p] = pts[p * 3 + 1];
-  xt[2 * P + p] = pts[p * 3 + 2];
+  for (int k = 0; k < C; k++) xt[k * P + p] = pts[p * C + k];
 }
 
-// First trunk layer (3 -> 64) on the tensor-core path.  With K = 3 a contraction kernel is all epilogue, so the
-// layer is never materialised in fp32: one kernel accumulates its GroupNorm statistics, a second recomputes it,
-// applies GroupNorm + ReLU and writes the FP16 hi/lo planes layer 2's TMA loads read.  Both evaluate
-//   y = fma(w2, z, fma(w1, y, fma(w0, x, b)))  in this order, so the statistics describe exactly the values normalised.
-// pts [P][3], wt [3][64], part[(tile*2 + h)*64 + c] (h = first / second half of the tile's points, fp64 sums).
-__global__ void __launch_bounds__(256) pn_l1_stats_kernel(const float* __restrict__ pts, const int4* __restrict__ tiles,
+// First trunk layer (C -> 64, C = 3 xyz or 4 xyz + reflectance) on the tensor-core path.  With K = C a contraction
+// kernel is all epilogue, so the layer is never materialised in fp32: one kernel accumulates its GroupNorm statistics, a
+// second recomputes it, applies GroupNorm + ReLU and writes the FP16 hi/lo planes layer 2's TMA loads read.  Both evaluate
+//   y = fma(w2, z, fma(w1, y, fma(w0, x, b)))  and, with C = 4, then  y = fma(w3, r, y)
+// in this order, so the statistics describe exactly the values normalised and 3-channel points take the same arithmetic
+// as before the reflectance channel existed.  C is a runtime argument, uniform per launch.
+// pts [P][C] (16-byte rows when C = 4), wt [C][64], part[(tile*2 + h)*64 + c] (h = first / second half of the tile's
+// points, fp64 sums).  The stats kernel stages the tile's points as 16-byte rows whatever C (3-channel rows padded with
+// r = 0, w3 = 0) and runs one loop for both widths: fma(0, 0, y) = y exactly (up to the sign of a zero, which no sum or
+// square sees), so the statistics of 3-channel points are the ones the 3-term chain gives.  The apply kernel, whose
+// outputs carry the sign of a zero into the FP16 planes, takes the fourth fma only when C = 4.  The fp64 sums are
+// latency-bound: the stats kernel is held to 32 registers, eight CTAs per SM.
+__global__ void __launch_bounds__(256, 8) pn_l1_stats_kernel(const float* __restrict__ pts, int C, const int4* __restrict__ tiles,
                                                           const float* __restrict__ wt, const float* __restrict__ bias,
                                                           double2* __restrict__ part) {
-  __shared__ float sp[256 * 3];
+  __shared__ float4 sp[256];
   __shared__ double2 red[4][64];
   const int4 tt = tiles[blockIdx.x];          // (pair, first point, length <= 256, -)
-  for (int i = threadIdx.x; i < tt.z * 3; i += 256) sp[i] = pts[(long)tt.y * 3 + i];
+  if (threadIdx.x < tt.z) {                   // one point per thread (a tile holds at most 256)
+    const long r = (long)tt.y + threadIdx.x;
+    sp[threadIdx.x] = C == 4 ? __ldg(reinterpret_cast<const float4*>(pts) + r)
+                             : make_float4(__ldg(pts + r * 3), __ldg(pts + r * 3 + 1), __ldg(pts + r * 3 + 2), 0.f);
+  }
   __syncthreads();
   const int c = threadIdx.x & 63, qd = threadIdx.x >> 6;
-  const float w0 = wt[c], w1 = wt[64 + c], w2 = wt[128 + c], b = bias[c];
+  const float w0 = wt[c], w1 = wt[64 + c], w2 = wt[128 + c], w3 = C == 4 ? wt[192 + c] : 0.f, b = bias[c];
   double s1 = 0.0, s2 = 0.0;
   const int p1 = min(tt.z, (qd + 1) * 64);
   for (int p = qd * 64; p < p1; p++) {
-    const float y = fmaf(w2, sp[3 * p + 2], fmaf(w1, sp[3 * p + 1], fmaf(w0, sp[3 * p], b)));
+    const float4 q = sp[p];
+    const float y = fmaf(w3, q.w, fmaf(w2, q.z, fmaf(w1, q.y, fmaf(w0, q.x, b))));
     s1 += (double)y;
     s2 += (double)y * (double)y;
   }
@@ -55,7 +66,7 @@ __global__ void __launch_bounds__(256) pn_l1_stats_kernel(const float* __restric
   }
 }
 // x1p planes [2][P][64] = split(relu(GN(y)))  ;  thread = (point, 4 channels)
-__global__ void __launch_bounds__(256) pn_l1_apply_kernel(const float* __restrict__ pts, const float* __restrict__ wt,
+__global__ void __launch_bounds__(256) pn_l1_apply_kernel(const float* __restrict__ pts, int C, const float* __restrict__ wt,
                                                           const float* __restrict__ bias, const float* __restrict__ sc,
                                                           const float* __restrict__ sh, const int* __restrict__ seg,
                                                           int L, long P, __half* __restrict__ out, int* status) {
@@ -64,16 +75,27 @@ __global__ void __launch_bounds__(256) pn_l1_apply_kernel(const float* __restric
   const long row = idx >> 4;
   const int c = (int)(idx & 15) * 4;
   const int g = seg[row] / L;
-  const float x = __ldg(pts + row * 3), y = __ldg(pts + row * 3 + 1), z = __ldg(pts + row * 3 + 2);
+  float4 q;
+  if (C == 4) q = __ldg(reinterpret_cast<const float4*>(pts) + row);
+  else q = make_float4(__ldg(pts + row * 3), __ldg(pts + row * 3 + 1), __ldg(pts + row * 3 + 2), 0.f);
   const float4 w0 = *reinterpret_cast<const float4*>(wt + c), w1 = *reinterpret_cast<const float4*>(wt + 64 + c),
                w2 = *reinterpret_cast<const float4*>(wt + 128 + c), b = *reinterpret_cast<const float4*>(bias + c);
+  float4 v;
+  v.x = fmaf(w2.x, q.z, fmaf(w1.x, q.y, fmaf(w0.x, q.x, b.x)));
+  v.y = fmaf(w2.y, q.z, fmaf(w1.y, q.y, fmaf(w0.y, q.x, b.y)));
+  v.z = fmaf(w2.z, q.z, fmaf(w1.z, q.y, fmaf(w0.z, q.x, b.z)));
+  v.w = fmaf(w2.w, q.z, fmaf(w1.w, q.y, fmaf(w0.w, q.x, b.w)));
+  if (C == 4) {
+    const float4 w3 = *reinterpret_cast<const float4*>(wt + 192 + c);
+    v.x = fmaf(w3.x, q.w, v.x); v.y = fmaf(w3.y, q.w, v.y); v.z = fmaf(w3.z, q.w, v.z); v.w = fmaf(w3.w, q.w, v.w);
+  }
   const float4 a = *reinterpret_cast<const float4*>(sc + (long)g * 64 + c);
   const float4 s = *reinterpret_cast<const float4*>(sh + (long)g * 64 + c);
   float4 r;
-  r.x = fmaxf(fmaf(fmaf(w2.x, z, fmaf(w1.x, y, fmaf(w0.x, x, b.x))), a.x, s.x), 0.f);
-  r.y = fmaxf(fmaf(fmaf(w2.y, z, fmaf(w1.y, y, fmaf(w0.y, x, b.y))), a.y, s.y), 0.f);
-  r.z = fmaxf(fmaf(fmaf(w2.z, z, fmaf(w1.z, y, fmaf(w0.z, x, b.z))), a.z, s.z), 0.f);
-  r.w = fmaxf(fmaf(fmaf(w2.w, z, fmaf(w1.w, y, fmaf(w0.w, x, b.w))), a.w, s.w), 0.f);
+  r.x = fmaxf(fmaf(v.x, a.x, s.x), 0.f);
+  r.y = fmaxf(fmaf(v.y, a.y, s.y), 0.f);
+  r.z = fmaxf(fmaf(v.z, a.z, s.z), 0.f);
+  r.w = fmaxf(fmaf(v.w, a.w, s.w), 0.f);
   split4_store(r, out + row * 64 + c, out + P * 64 + row * 64 + c, status);
 }
 
@@ -477,7 +499,7 @@ PnWs carve(MmArena& a, int pairs, int L, long P, bool use_tc) {
   const long max_tiles = pn_max_tiles(P, pairs);
   PnWs w;
   long nd = (long)pairs * L;
-  w.xt = a.take<float>(use_tc ? 0 : 3 * P);
+  w.xt = a.take<float>(use_tc ? 0 : 3 * P);   // 3-channel points only: pointnet_fp32 transposes 4-channel ones into t1
   w.y1 = a.take<float>(use_tc ? 0 : 64 * P);
   w.t0 = a.take<float>(128 * P);
   w.t1 = a.take<float>(64 * P);
@@ -639,16 +661,17 @@ int pointnet_tc(const mmmot_weights* wts, const float* points, const int* det_sp
   const int ndet = pairs * L;
   const bool timed = mm_timing_on();
   const double cols = (double)P;
-  // layer 1 (3 -> 64): its statistics, then the layer recomputed, normalised and split into x1p
+  // layer 1 (C -> 64): its statistics, then the layer recomputed, normalised and split into x1p
+  const int C = wts->point_channels;
   const float* const* l1 = &wts->w[MMMOT_W_PN_L1];
-  if (timed) mm_timing_begin(st, MM_T_PN_L1, 2.0 * 64 * 3 * cols, 12.0 * cols);
-  pn_l1_stats_kernel<<<(int)n_tiles, 256, 0, st>>>(points, w.tiles, l1[0], l1[1], w.part);
+  if (timed) mm_timing_begin(st, MM_T_PN_L1, 2.0 * 64 * C * cols, 4.0 * C * cols);
+  pn_l1_stats_kernel<<<(int)n_tiles, 256, 0, st>>>(points, C, w.tiles, l1[0], l1[1], w.part);
   MM_LAUNCH_CHECK();
   if (timed) mm_timing_end(st);
   MM_TRY(stats_reduce(w.part, 64, pairs, 0, w.gstart, w.stats, st, 2));
   MM_TRY(gn_finalize(w.stats, l1[2], l1[3], w.cnt, 0, pairs, 64, 1, w.sc, w.sh, st, 0, 0, status));
-  if (timed) mm_timing_begin(st, MM_T_PN_L1, 0.0, (12.0 + 4.0 * 64) * cols);
-  pn_l1_apply_kernel<<<mm_cdiv(P * 16, 256), 256, 0, st>>>(points, l1[0], l1[1], w.sc, w.sh, w.seg, L, P, w.x1p, status);
+  if (timed) mm_timing_begin(st, MM_T_PN_L1, 0.0, (4.0 * C + 4.0 * 64) * cols);
+  pn_l1_apply_kernel<<<mm_cdiv(P * 16, 256), 256, 0, st>>>(points, C, l1[0], l1[1], w.sc, w.sh, w.seg, L, P, w.x1p, status);
   MM_LAUNCH_CHECK();
   if (timed) mm_timing_end(st);
   float* const ys[3] = {w.t0, w.t1, w.t0};             // outputs of layers 2, 3, 4
@@ -720,11 +743,15 @@ int pointnet_tc(const mmmot_weights* wts, const float* points, const int* det_sp
 int pointnet_fp32(const mmmot_weights* wts, const float* points, const int* det_split, int pairs, int L, long P,
                   long n_tiles, const PnWs& w, const float* head_mask, float* feats, cudaStream_t st) {
   const int ndet = pairs * L;
-  transpose_points_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(points, w.xt, P);
+  const int C = wts->point_channels;
+  // the carve holds 3P floats for xt; 4-channel points are transposed into t1 (64P floats), which nothing reads before
+  // layer 3 writes it
+  float* const xt = C == 4 ? w.t1 : w.xt;
+  transpose_points_kernel<<<mm_cdiv(P, 256), 256, 0, st>>>(points, C, xt, P);
   MM_LAUNCH_CHECK();
-  // trunk: 3 -> 64 -> 64 -> 64 -> 128 -> 1024, each conv + GroupNorm(C,C) over the pair's points + ReLU
-  const int cin[5] = {3, 64, 64, 64, 128}, cout[5] = {64, 64, 64, 128, 1024};
-  const float* src[5] = {w.xt, w.y1, w.t0, w.t1, w.t0};
+  // trunk: C -> 64 -> 64 -> 64 -> 128 -> 1024, each conv + GroupNorm(cout, cout) over the pair's points + ReLU
+  const int cin[5] = {C, 64, 64, 64, 128}, cout[5] = {64, 64, 64, 128, 1024};
+  const float* src[5] = {xt, w.y1, w.t0, w.t1, w.t0};
   float* dst[5] = {w.y1, w.t0, w.t1, w.t0, w.big};
   for (int i = 0; i < 5; i++) {
     const float* const* q = &wts->w[MMMOT_W_PN_L1 + 4 * i];
@@ -827,6 +854,9 @@ static int pointnet_impl(const mmmot_weights* wts, const float* points, const in
                          int pairs, int L, float* feats, void* workspace, size_t workspace_bytes, void* stream, bool train,
                          const float* head_mask) {
   if (!wts || !points || !det_split || !h_det_split || !feats || !workspace || pairs <= 0 || L <= 0)
+    return MMMOT_E_ARG;
+  // points [P][point_channels]: xyz, or xyz + reflectance in 16-byte rows
+  if (wts->point_channels != 3 && !(wts->point_channels == 4 && (reinterpret_cast<uintptr_t>(points) & 15) == 0))
     return MMMOT_E_ARG;
   const bool use_tc = !train && pointnet_use_tc(L);
   const int tw = use_tc ? tc::BN : 128;

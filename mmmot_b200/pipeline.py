@@ -43,11 +43,13 @@ class HostPipeline:
         self._shape = key
 
     def run(self, h_crops, h_points, points_split, sync=True):
-        """h_crops (B*L) x 3 x H x W, h_points P x 3: pinned host tensors; points_split (B*L + 1,) CPU int CSR offsets.
+        """h_crops (B*L) x 3 x H x W, h_points P x C (C the net's point width, else MmmotError): pinned host tensors;
+        points_split (B*L + 1,) CPU int CSR offsets.
         Returns {"match": B x n int32, "assign_det" / "assign_new" / "assign_end": B x L} as pinned host tensors (valid
         after the synchronisation this call performs unless sync=False) and "match_device", the same B x n matches on the
         device (for a gather across ranks).  Raises MmmotError (MMMOT_E_RANGE) if the library flagged an FP16 range overflow."""
         n, m, L = self.n, self.m, self.n + self.m
+        self.net._check_points(h_points)
         pairs = h_crops.shape[0] // L
         self._prepare(h_crops, h_points, pairs)
         split = points_split.detach().to("cpu", torch.int64)

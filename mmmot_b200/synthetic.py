@@ -11,15 +11,16 @@ import torch
 from .schema import state_schema
 
 
-def synthetic_state_dict(fusion="C", seed=0):
-    """A non-degenerate ``state_dict`` for ``TrackingNet`` with the reference's key names.
+def synthetic_state_dict(fusion="C", seed=0, point_in=3):
+    """A non-degenerate ``state_dict`` for ``TrackingNet`` with the reference's key names; point_in = 4 for a net on
+    xyz + reflectance points (``without_reflectivity=False``).
 
     Default inits make every GroupNorm the identity affine and both STN output layers zero
     (reference: modules/point_net.py:69-70), which hides bugs; so norm affines, BN running
     statistics and the STN output layers are all randomised."""
     g = torch.Generator().manual_seed(1000 + seed)
     sd = {}
-    for key, (shape, kind) in state_schema(fusion).items():
+    for key, (shape, kind) in state_schema(fusion, point_in).items():
         if kind == "conv":
             fan_in = 1
             for s in shape[1:]:
@@ -62,12 +63,16 @@ def structured_crops(noise, gen):
     return noise * contrast + 1.5 * lf + bright
 
 
-def synthetic_pair(n, m=None, pts=128, hw=64, seed=0, ragged=False):
+def synthetic_pair(n, m=None, pts=128, hw=64, seed=0, ragged=False, reflectance=False):
     """One frame-pair in the exact layout ``TestSequence.__getitem__`` + the DataLoader hand to
     ``TrackingNet.forward`` (reference: dataset/test_seq_dataset.py:227-246, eval_seq.py:144-153):
 
-    dets ``L x 3 x H x W``; det_info['points'] ``1 x P_t x 3``; det_info['points_split']
-    ``1 x (L+1)`` **float**; dets_split = list of shape-(1,) int tensors.
+    dets ``L x 3 x H x W``; det_info['points'] ``1 x P_t x 3`` (``1 x P_t x 4`` with reflectance);
+    det_info['points_split'] ``1 x (L+1)`` **float**; dets_split = list of shape-(1,) int tensors.
+
+    reflectance: a fourth column in [0, 1], a per-detection base (surfaces differ between objects) plus per-point
+    noise, drawn after every other value so the xyz outputs of a seed are the same with or without it.  A column
+    without detection-level structure would be a degenerate GroupNorm input (see ``structured_crops``).
     """
     m = n if m is None else m
     L = n + m
@@ -84,6 +89,10 @@ def synthetic_pair(n, m=None, pts=128, hw=64, seed=0, ragged=False):
         [0.0, -20.0, -2.0])
     which = torch.repeat_interleave(torch.arange(L), cnt)
     points = torch.randn(pt, 3, generator=g) * torch.tensor([2.0, 1.0, 0.8]) + centre[which]
+    if reflectance:
+        base = torch.rand(L, generator=g) * 0.8 + 0.1
+        refl = (base[which] + torch.randn(pt, generator=g) * 0.05).clamp(0.0, 1.0)
+        points = torch.cat([points, refl[:, None]], 1)
     det_info = {
         "points": points.unsqueeze(0).contiguous(),
         "points_split": split.float().unsqueeze(0),
@@ -92,13 +101,14 @@ def synthetic_pair(n, m=None, pts=128, hw=64, seed=0, ragged=False):
     return dets, det_info, dets_split
 
 
-def synthetic_batch(b, n, pts=128, hw=64, seed=0):
+def synthetic_batch(b, n, pts=128, hw=64, seed=0, reflectance=False):
     """``b`` frame-pairs with equal ``n`` detections per frame, packed for ``forward_batch``:
-    dets ``(b*2n) x 3 x H x W``, points ``P_total x 3``, points_split ``(b*2n+1,)`` int64."""
+    dets ``(b*2n) x 3 x H x W``, points ``P_total x 3`` (``x 4`` with reflectance), points_split ``(b*2n+1,)``
+    int64."""
     ds, ps, sp = [], [], [torch.zeros(1, dtype=torch.int64)]
     off = 0
     for p in range(b):
-        d, info, _ = synthetic_pair(n, n, pts, hw, seed=seed + p)
+        d, info, _ = synthetic_pair(n, n, pts, hw, seed=seed + p, reflectance=reflectance)
         ds.append(d)
         ps.append(info["points"][0])
         s = info["points_split"][0].long()

@@ -29,6 +29,12 @@ def _vp(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
+def _aligned_rows(points):
+    """4-channel points are read as 16-byte rows (one float4 per point): a tensor that does not start on a 16-byte
+    boundary (a view at an odd storage offset) is copied."""
+    return points.clone() if points.shape[1] == 4 and points.data_ptr() % 16 else points
+
+
 class _Holder(nn.Module):
     """Empty module used to build the reference's parameter tree (names only)."""
 
@@ -74,7 +80,7 @@ class TrackingNet(nn.Module):
         unsupported = []
         if appear_len != 512 or point_len != 512: unsupported.append("appear_len/point_len != 512")
         if appear_arch != 'vgg' or not appear_skippool or appear_fpn: unsupported.append("appearance must be vgg + skippool")
-        if point_arch != 'v1' or not without_reflectivity: unsupported.append("point_arch must be v1 on xyz points")
+        if point_arch != 'v1': unsupported.append("point_arch must be v1")
         if end_arch != 'v2' or end_mode not in _lib.END_MODE: unsupported.append("end_arch must be v2, end_mode avg or max")
         if score_arch not in ('branch_cls', 'branch_reg'): unsupported.append("score_arch must be branch_cls/branch_reg")
         if score_fusion_arch not in _lib.FUSION: unsupported.append(f"score_fusion_arch {score_fusion_arch!r}")
@@ -91,8 +97,10 @@ class TrackingNet(nn.Module):
         self.score_fusion_arch = score_fusion_arch
         # dropblock / use_dropout are identity in eval mode; accepted for config compatibility
         self.dropblock, self.use_dropout = dropblock, use_dropout
+        # PointNet's input width (tracking_net.py:41): xyz, or xyz + LiDAR reflectance
+        self.point_channels = 4 - int(bool(without_reflectivity))
         gen = torch.Generator().manual_seed(0)
-        for key, (shape, kind) in state_schema(score_fusion_arch).items():
+        for key, (shape, kind) in state_schema(score_fusion_arch, self.point_channels).items():
             _register(self, key, _default_init(shape, kind, gen), kind in BUFFER_KINDS)
         for name, prm in self.named_parameters():
             if name.endswith(".idt"):           # reference point_net.py:62: requires_grad=False
@@ -229,6 +237,13 @@ class TrackingNet(nn.Module):
         the eval branch."""
         return (_lib.SCORE_SIGMOID if "cls" in self.score_arch else 0) | _lib.SCORE_THRESHOLD
 
+    def _check_points(self, points):
+        """points [P][C] with C the net's point width (point_channels); raises MmmotError otherwise.  Any other width
+        would be read as rows of C floats and silently regrouped."""
+        if points.dim() != 2 or points.shape[1] != self.point_channels:
+            raise _lib.MmmotError(f"points must be [P][{self.point_channels}] for this net "
+                                  f"(without_reflectivity={self.point_channels == 3}), got {list(points.shape)}")
+
     @staticmethod
     def _raise_on_status(status):
         """`status`: the int32 word forward_batch returns (device tensor or int)."""
@@ -250,11 +265,12 @@ class TrackingNet(nn.Module):
         """B independent frame-pairs, each with n previous and m next detections.
 
         crops         (B*(n+m)) x 3 x H x W  fp32, CUDA
-        points        P_total x 3            fp32, CUDA (detections concatenated in order)
+        points        P_total x C            fp32, CUDA (detections concatenated in order); C = point_channels:
+                                             xyz, or xyz + reflectance (without_reflectivity=False)
         points_split  (B*(n+m) + 1,) int     CSR offsets, CPU tensor (the reference reads it with
                                              .item() per detection: modules/point_net.py:33-35)
         returns dict: det B x 3 x L, link B x 3 x n x m, new B x 3 x m, end B x 3 x n (un-padded),
-                      trans [1x3x3, 1x64x64]; per-pair semantics identical to ``forward``; "status": the library's
+                      trans [1xCxC, 1x64x64]; per-pair semantics identical to ``forward``; "status": the library's
                       status word (int32 device tensor; bit 0 = an activation left FP16's range, MMMOT_E_RANGE).
         check=True (default) reads the status word back (one host sync) and raises MmmotError when it is set;
         pipelined callers pass check=False and test ``out["status"]`` together with the results they copy back.
@@ -263,13 +279,14 @@ class TrackingNet(nn.Module):
             raise NotImplementedError("mmmot_b200.TrackingNet implements the eval-mode forward only (SURVEY §8f N4)")
         m = n if m is None else m
         L = n + m
+        self._check_points(points)
         lib = _lib.load()
         wts = self.prepared()
         dev = wts.flat.device
         if crops.device != dev or points.device != dev:
             raise _lib.MmmotError("inputs must live on the module's CUDA device")
         crops = crops.contiguous().float()
-        points = points.contiguous().float()
+        points = _aligned_rows(points.contiguous().float())
         split = points_split.detach().to("cpu", torch.int32).contiguous()
         if crops.shape[0] % L or split.numel() != crops.shape[0] + 1:
             raise _lib.MmmotError("crops / points_split do not match n, m")
@@ -386,7 +403,9 @@ class TrackingNet(nn.Module):
     def forward(self, dets, det_info, dets_split):
         """Reference signature (modules/tracking_net.py:165-193): one sample of K >= 2 frames.
 
-        dets L x 3 x H x W; det_info['points'] 1 x P x 3; det_info['points_split'] 1 x (L+1) float;
+        dets L x 3 x H x W; det_info['points'] 1 x P x C' (C' >= C, the net's point width: the first C columns are
+        used, as the reference's loader keeps x, y, z and, with without_reflectivity=False, r); det_info['points_split']
+        1 x (L+1) float;
         dets_split: K shape-(1,) int tensors, the detections of each frame.  The feature stages run once over all L
         detections of the sample (one GroupNorm domain, exactly like the reference), then the affinity stage on every
         pair of consecutive frames (mmmot_b200.ortools_solve solves the association programme of K > 2 frames as a
@@ -401,13 +420,18 @@ class TrackingNet(nn.Module):
         if self.training and len(splits) != 2:
             raise NotImplementedError("mmmot_b200.TrackingNet supports 2-frame samples (sample_max_len: 2)")
         L = sum(splits)
+        C = self.point_channels
+        raw = det_info['points']
+        if raw.dim() < 2 or raw.shape[-1] < C:
+            raise _lib.MmmotError(f"det_info['points'] must carry at least {C} columns per point for this net "
+                                  f"(without_reflectivity={C == 3}), got {list(raw.shape)}")
         lib = _lib.load()
         if self.training:
             self._prepared = None                  # parameters move under an optimizer: re-derive the operands every step
         wts = self.prepared()
         dev = wts.flat.device
         crops = dets.contiguous().float()
-        points = det_info['points'].reshape(-1, det_info['points'].shape[-1])[:, :3].contiguous().float()
+        points = _aligned_rows(raw.reshape(-1, raw.shape[-1])[:, :C].contiguous().float())
         split = det_info['points_split'].reshape(-1).detach().to("cpu", torch.int32).contiguous()
         if (crops.device != dev or points.device != dev or crops.shape[0] != L or split.numel() != L + 1
                 or len(splits) < 2 or min(splits) <= 0):

@@ -78,8 +78,8 @@ def pack_px(packed_u8, M, K):
 
 
 def prepare(state_dict, fusion):
-    """-> (list of fp32 CPU tensors indexed by weight id (None = unused), trans1 3x3, trans2 64x64,
-    per-id tensor-core output scales)."""
+    """-> (list of fp32 CPU tensors indexed by weight id (None = unused), trans1 CxC (C = 3 xyz or 4 xyz +
+    reflectance: the checkpoint's point width), trans2 64x64, per-id tensor-core output scales)."""
     sd = {k: v.detach().cpu() for k, v in state_dict.items()}
     out = [None] * W["COUNT"]
     f64 = lambda k: sd[k].double()
@@ -106,7 +106,7 @@ def prepare(state_dict, fusion):
     # PointNet trunk with the constant STN transforms folded in:
     #   x' = T1^T x  => conv1(x') = (W1 T1^T) x ;  x_local = T2^T x1 => conv2(x_local) = (W2 T2^T) x1
     pf = "point_net.feat"
-    t1 = stn_constant(sd, f"{pf}.stn1", 3)
+    t1 = stn_constant(sd, f"{pf}.stn1", sd[f"{pf}.stn1.idt"].shape[0])     # 3x3 on xyz, 4x4 with reflectance
     t2 = stn_constant(sd, f"{pf}.stn2", 64)
     ws = [f64(f"{pf}.conv{j}.weight").squeeze(-1) for j in range(1, 6)]
     ws[0] = ws[0] @ t1.t()
@@ -236,6 +236,7 @@ class DeviceWeights:
         for i, (t, o) in enumerate(zip(tensors, offs)):
             self.table.w[i] = None if t is None else base + 4 * o
             self.table.tc_scale[i] = scales[i]
+        self.table.point_channels = int(state_dict["point_net.feat.conv1.weight"].shape[1])
         self.ptr = ctypes.pointer(self.table)
         self.trans1 = self.trans1.to(device)
         self.trans2 = self.trans2.to(device)
