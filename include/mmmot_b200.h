@@ -151,6 +151,59 @@ int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops, int n_img
                          int L, float* feats, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Appearance on a ResNet-50/101/152 trunk + 4 SkipPool heads -> stack 0 of feats (reference appear_arch resnet50 |
+ * resnet101 | resnet152 with appear_skippool: modules/appear_net.py:60-83,114-128,213-256; torchvision Bottleneck v1.5,
+ * the stride on the 3x3 conv).  Eval mode: every BatchNorm folded into its conv (weights.py::prepare_resnet).
+ * Convolutions in execution order: 0 = stem (7x7 / 2, 3 -> 64); then, per block of layer1..layer4, conv1 (1x1),
+ * conv2 (3x3, stride 2 on block 0 of layer2..4), conv3 (1x1) and, on block 0 of every layer, downsample (1x1, same
+ * stride).  MMMOT_RESNET_MAX_CONVS bounds 1 + 3 * blocks + 4 (155 for ResNet-152).
+ *   wt[i]    fp32 Wt[K][Cout] for the FP32 engine; K order: 1x1 k = ci, 3x3 k = (ky*3+kx)*Cin + ci, stem
+ *            k = (ky*7+kx)*3 + ci (K = 147)
+ *   bias[i]  [Cout]: the folded BatchNorm shift (torchvision convs have no bias)
+ *   wp[i]    the same matrix as packed FP16 hi/lo tiles (weights.py::pack_tc), the stem's K zero-padded to 160;
+ *            wp_scale[i] its 2^-s output scale
+ *   head[s]  SkipPool head s on the C = 256 << s channels of layer s+1: the 10 tensors of MMMOT_W_SKIP0 (mid = C / 4)
+ */
+#define MMMOT_RESNET_MAX_CONVS 160
+typedef struct mmmot_resnet_weights {
+  int blocks[4];   /* bottleneck blocks of layer1..layer4: 3-4-6-3 (50), 3-4-23-3 (101), 3-8-36-3 (152) */
+  const float* wt[MMMOT_RESNET_MAX_CONVS];
+  const float* bias[MMMOT_RESNET_MAX_CONVS];
+  const void* wp[MMMOT_RESNET_MAX_CONVS];
+  float wp_scale[MMMOT_RESNET_MAX_CONVS];
+  const float* head[4][10];
+} mmmot_resnet_weights;
+/*   crops  [n_img][3][H][W] fp32 (H, W multiples of 32), n_img = pairs*L; feats as mmmot_appearance_fwd (stack 0).
+ * wts is not read (the heads live in rw); it may be NULL.  workspace: mmmot_appearance_resnet_workspace(n_img, H, W)
+ * bytes, the same for every block count and engine.  MMMOT_E_ARG (a null pointer, n_img or L <= 0, a block count < 1 or
+ * more convs than MMMOT_RESNET_MAX_CONVS) or MMMOT_E_SHAPE (H or W not a multiple of 32, n_img % L, more than 2^31
+ * stem pixels) before any CUDA call.  Engine: as mmmot_appearance_fwd (tensor cores when L*H*W >= 32768 in auto mode). */
+size_t mmmot_appearance_resnet_workspace(int n_img, int H, int W);
+int mmmot_appearance_resnet_fwd(const mmmot_weights* wts, const mmmot_resnet_weights* rw, const float* crops, int n_img,
+                                int H, int W, int L, float* feats, void* workspace, size_t workspace_bytes, void* stream);
+/* Test hook: one launch kind of mmmot_appearance_resnet_fwd, through the same code, on n_img images of H x W.  Engine:
+ * mmmot_set_engine 1 = FP32 engine (activations channel-major fp32 [C][n][H][W]), 0 or 2 = tensor cores (activations FP16
+ * hi/lo NHWC planes [2][n][H][W][C], the lo plane n*H*W*C elements after the hi one).  Outputs at Ho = H/stride etc.
+ *   op 0 gather: the taps of a ks x ks (1 or 3) / stride (1 or 2) / pad ks/2 conv of X (C channels, C % 32 == 0) -> Y:
+ *        tensor cores hi/lo rows [2][n*Ho*Wo][ks*ks*C] (planes n*Ho*Wo*ks*ks*C apart), FP32 [ks*ks*C][n*Ho*Wo] fp32;
+ *        k = (ky*ks+kx)*C + ci, out-of-image taps zero
+ *   op 1 stem gather: X = fp32 crops [n][3][H][W] -> Y: the stem's 7x7 / 2 / pad 3 taps, k = (ky*7+kx)*3 + ci, as
+ *        hi/lo rows [2][n*Ho*Wo][160] (k >= 147 zero; FP16 range flag in *status) or fp32 [147][n*Ho*Wo]
+ *   op 2 stem: X = crops -> Y = relu(stem conv + bias) with rw conv 0, 64 channels at H/2 (cols: gather scratch)
+ *   op 3 conv: rw conv `conv` (Wt / packed tiles with M outputs, K = ks*ks*C) on X (C channels) + bias (+ ReLU if relu)
+ *        -> Y (M channels at Ho x Wo); cols: gather scratch (stride 2, and every non-1x1 conv on the FP32 engine), kseg
+ *        (or NULL = one pass): K-segment scratch of the 3x3 stride-1 convs with K >= 2304 (fp32 [column tiles * 256][M])
+ *   op 4 max-pool: 3x3 / 2 / pad 1 of X (C = 64) -> Y
+ *   op 5 residual: Y = relu(Y + id), n*H*W*C elements in place (tensor cores: FP16 range flag in *status on a sum
+ *        >= 65504 or NaN)
+ *   op 6 mean: per-image channel means of X (C channels) -> Y [n][C] fp32
+ *   op 7 heads: X = the pooled maps [n][256 << s] of s = 0..3 back to back -> Y = feats [n/L][3][512][L], stack 0
+ * MMMOT_E_ARG, before any CUDA call, for an unknown op or arguments the op cannot take. */
+int mmmot_debug_resnet_op(int op, const mmmot_resnet_weights* rw, int conv, int n_img, int H, int W, int C, int ks, int stride,
+                          int M, int relu, int L, const void* X, const void* id, void* Y, void* cols, float* kseg, int* status,
+                          void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * PointNet encoder over ragged per-detection point sets -> stack 1 of feats.
  * Replaces PointNet_v1.forward, reference modules/point_net.py:25-44,115-153.
  *   points     [P_total][C]  C = wts->point_channels: xyz, or xyz + reflectance (16-byte aligned rows), detections

@@ -40,12 +40,23 @@ class Weights(ctypes.Structure):
     _fields_ = [("w", ctypes.c_void_p * W["COUNT"]), ("tc_scale", ctypes.c_float * W["COUNT"]), ("point_channels", ctypes.c_int)]
 
 
+RESNET_MAX_CONVS = 160
+
+
+class ResnetWeights(ctypes.Structure):
+    """struct mmmot_resnet_weights"""
+    _fields_ = [("blocks", ctypes.c_int * 4), ("wt", ctypes.c_void_p * RESNET_MAX_CONVS),
+                ("bias", ctypes.c_void_p * RESNET_MAX_CONVS), ("wp", ctypes.c_void_p * RESNET_MAX_CONVS),
+                ("wp_scale", ctypes.c_float * RESNET_MAX_CONVS), ("head", (ctypes.c_void_p * 10) * 4)]
+
+
 class MmmotError(RuntimeError):
     pass
 
 
 _vp, _i, _l, _f, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_long, ctypes.c_float, ctypes.c_size_t
 _wp = ctypes.POINTER(Weights)
+_rwp = ctypes.POINTER(ResnetWeights)
 
 # name -> (restype, argtypes); every symbol the header declares
 SIGNATURES = {
@@ -82,6 +93,9 @@ SIGNATURES = {
     "mmmot_timing_collect": (_i, [ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_long)]),
     "mmmot_appearance_workspace": (_sz, [_i, _i, _i]),
     "mmmot_appearance_fwd": (_i, [_wp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "mmmot_appearance_resnet_workspace": (_sz, [_i, _i, _i]),
+    "mmmot_appearance_resnet_fwd": (_i, [_wp, _rwp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "mmmot_debug_resnet_op": (_i, [_i, _rwp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mmmot_appearance_train_workspace": (_sz, [_i, _i, _i]),
     "mmmot_appearance_train_fwd": (_i, [_wp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "mmmot_pointnet_train_workspace": (_sz, [_i, _i, _l]),
@@ -132,7 +146,12 @@ def load():
             "(mmmot_b200 has no CPU fallback)")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
-        fn = getattr(lib, name)
+        try:
+            fn = getattr(lib, name)
+        except AttributeError:
+            # the ABI version only changes when an existing signature or struct does; an older library of the same
+            # version lacks the entry points added since, which must fail here rather than at the first call
+            raise MmmotError(f"{LIB_PATH} does not export {name}: it was built from older sources, rebuild it") from None
         fn.restype = res
         fn.argtypes = args
     if lib.mmmot_abi_version() != ABI_VERSION:

@@ -91,7 +91,8 @@ const char* const kTagNames[MM_T_COUNT] = {
     "pointnet.head_64to512_segsum",
     "affinity.l1_pair_512to1024", "affinity.newend_means", "affinity.l2_512to512", "affinity.l3_512to128",
     "affinity.logit", "lp.assign", "pointnet.moments_128", "pointnet.moments_64",
-    "pointnet.moments_finalize", "lp.flow"};
+    "pointnet.moments_finalize", "lp.flow", "resnet.stem", "resnet.maxpool", "resnet.conv1x1", "resnet.conv3x3",
+    "resnet.stride2", "resnet.residual", "resnet.mean_heads"};
 }  // namespace
 
 bool mm_timing_on() { return g_timing; }
@@ -225,6 +226,11 @@ extern "C" int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, cons
     default: return gemm_simt_launch<XM_CONV3>(p, st);
   }
 }
+
+// The FP32 engine on a plain operand X[k*x_ks + column] (XM_DIRECT, uniform tiling, one group): the ResNet trunk's
+// channel-major activations and gathered taps (resnet.cu).  Its (M, K) shapes are checked against fp64 through
+// mmmot_debug_simt_op, which runs the same launch (tests/test_resnet_appearance.py).
+int mm_simt_direct(const GemmP& p, cudaStream_t st) { return gemm_simt_launch<XM_DIRECT>(p, st); }
 
 // The producer variant gemm_gen_launch takes (1 = prefetching), computed on the host without any CUDA call.
 extern "C" int mmmot_debug_gen_prefetch(int gen, int m) {

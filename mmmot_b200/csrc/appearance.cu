@@ -424,6 +424,14 @@ extern "C" int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W
 
 int mm_launch_skip_heads(const mmmot_weights* wts, float* const* pooled, int n_img, int L, float* feats, cudaStream_t st);
 
+// per-image channel means of a planar NHWC map [2][n_img][hw][C] (planes `plane` apart) -> pooled[n_img][C]; the ResNet
+// trunk's SkipPool averages (resnet.cu)
+int mm_launch_plane_mean_planar(const __half* in, float* pooled, int n_img, int hw, int C, long plane, cudaStream_t st) {
+  plane_mean_planar_kernel<<<mm_cdiv((long)n_img * C, 128), 128, 0, st>>>(in, pooled, n_img, hw, C, plane);
+  MM_LAUNCH_CHECK();
+  return 0;
+}
+
 extern "C" size_t mmmot_appearance_workspace(int n_img, int H, int W) {
   MmArena a(nullptr, 0);
   carve_appearance(a, n_img, H, W, false);

@@ -44,7 +44,15 @@ enum {
   MM_T_PN_MOM128 = 29, MM_T_PN_MOM64 = 30,   // input moments of layer 5 and of the head (their GroupNorm statistics)
   MM_T_PN_MOMFIN = 31,                       // their slice tables, fixed-order reductions and fp64 statistics
   MM_T_FLOW = 32,         // association programme of K-frame samples (min-cost flow)
-  MM_T_COUNT = 33
+  // ResNet appearance trunk (resnet.cu), per launch kind
+  MM_T_RES_STEM = 33,     // stem: 7x7 tap gather + contraction
+  MM_T_RES_MAXPOOL = 34,  // 3x3 / 2 max-pool after the stem
+  MM_T_RES_1X1 = 35,      // stride-1 1x1 convs (conv1, conv3, layer1's downsample)
+  MM_T_RES_3X3 = 36,      // stride-1 3x3 convs
+  MM_T_RES_S2 = 37,       // stride-2 convs: their gather + contraction (conv2 and downsample of block 0, layer2..4)
+  MM_T_RES_ADD = 38,      // residual add + ReLU
+  MM_T_RES_HEADS = 39,    // SkipPool plane means + heads
+  MM_T_COUNT = 40
 };
 bool mm_timing_on();
 void mm_timing_begin(cudaStream_t st, int tag, double flop, double bytes);

@@ -25,6 +25,11 @@ VGG_POOL_AFTER = ((3, 10), (6,), (6,), (6,))
 SKIP_CHANNELS = (128, 256, 512, 512)          # channels of the four skip maps
 SKIP_OUT = 128                                # each SkipPool head emits 128 -> concat 512
 D = 512
+# ResNet trunks of appear_arch resnet50 / resnet101 / resnet152 (reference modules/appear_net.py:60-83): bottleneck
+# blocks of layer1..layer4 (torchvision resnet.py), widths 64 << s, outputs 4x that, one SkipPool head per layer
+RESNET_BLOCKS = {"resnet50": (3, 4, 6, 3), "resnet101": (3, 4, 23, 3), "resnet152": (3, 8, 36, 3)}
+RES_SKIP_CHANNELS = (256, 512, 1024, 2048)
+APPEAR_ARCHS = ("vgg",) + tuple(RESNET_BLOCKS)
 
 
 def skip_mid(c):
@@ -41,6 +46,43 @@ def _conv_bn(sd, prefix, idx, cin, cout, k):
     sd[f"{prefix}.{idx + 1}.running_mean"] = ((cout,), "run_mean")
     sd[f"{prefix}.{idx + 1}.running_var"] = ((cout,), "run_var")
     sd[f"{prefix}.{idx + 1}.num_batches_tracked"] = ((), "nbt")
+
+
+def _bn(sd, prefix, c, w_kind="norm_w"):
+    sd[f"{prefix}.weight"] = ((c,), w_kind)
+    sd[f"{prefix}.bias"] = ((c,), "norm_b")
+    sd[f"{prefix}.running_mean"] = ((c,), "run_mean")
+    sd[f"{prefix}.running_var"] = ((c,), "run_var")
+    sd[f"{prefix}.num_batches_tracked"] = ((), "nbt")
+
+
+def resnet_convs(arch):
+    """The convs of a ResNet trunk in execution order (mmmot_resnet_weights, include/mmmot_b200.h): (conv key, its
+    BatchNorm's key, cin, cout, kernel size, stride) -- the stem, then per bottleneck block conv1, conv2, conv3 and, on
+    block 0 of every layer, downsample."""
+    p = "appearance.layers"
+    out = [(f"{p}.conv1", f"{p}.bn1", 3, 64, 7, 2)]
+    cin = 64
+    for s, nb in enumerate(RESNET_BLOCKS[arch]):
+        w = 64 << s
+        for b in range(nb):
+            stride = 2 if (b == 0 and s > 0) else 1
+            q = f"{p}.layer{s + 1}.{b}"
+            out += [(f"{q}.conv1", f"{q}.bn1", cin, w, 1, 1), (f"{q}.conv2", f"{q}.bn2", w, w, 3, stride),
+                    (f"{q}.conv3", f"{q}.bn3", w, 4 * w, 1, 1)]
+            if b == 0:
+                out.append((f"{q}.downsample.0", f"{q}.downsample.1", cin, 4 * w, 1, stride))
+            cin = 4 * w
+    return out
+
+
+def _resnet(sd, arch):
+    """torchvision's resnetXX minus avgpool / fc (the reference's Resnet wrapper keeps conv1 .. layer4): bias-free convs,
+    each followed by a BatchNorm2d.  Registration order: conv1, bn1, then per block conv1, bn1, conv2, bn2, conv3, bn3,
+    downsample.  bn3 closes a residual branch (kind res_norm_w)."""
+    for conv, bn, cin, cout, k, _ in resnet_convs(arch):
+        sd[f"{conv}.weight"] = ((cout, cin, k, k), "conv")
+        _bn(sd, bn, cout, "res_norm_w" if conv.endswith("conv3") else "norm_w")
 
 
 def _lin_gn(sd, conv, norm, cin, cout, wshape):
@@ -62,9 +104,10 @@ def _stn(sd, p, cin, k):
     sd[f"{p}.output.bias"] = ((k * k,), "stn_out")
 
 
-def state_schema(fusion="C", point_in=3):
+def state_schema(fusion="C", point_in=3, appear_arch="vgg"):
     """OrderedDict key -> (shape, kind).  ``kind`` drives init / synthetic generation:
-    conv, bias, norm_w, norm_b, run_mean, run_var, nbt, eye, stn_out."""
+    conv, bias, norm_w, res_norm_w, norm_b, run_mean, run_var, nbt, eye, stn_out.
+    appear_arch: "vgg" (VGG16-BN) or a key of RESNET_BLOCKS."""
     sd = OrderedDict()
     # --- fusion_module (modules/fusion_net.py) ---
     f = "fusion_module"
@@ -80,11 +123,16 @@ def state_schema(fusion="C", point_in=3):
         _lin_gn(sd, f"{f}.input_w.0", f"{f}.input_w.1", 2 * D, D, (D, 2 * D, 1))
     else:
         raise ValueError(f"unknown fusion arch {fusion!r}")
-    # --- appearance (modules/appear_net.py, modules/vgg.py) ---
-    for s, stage in enumerate(VGG_STAGES):
-        for idx, cin, cout in stage:
-            _conv_bn(sd, f"appearance.layers.{s}", idx, cin, cout, 3)
-    for s, c in enumerate(SKIP_CHANNELS):
+    # --- appearance (modules/appear_net.py, modules/vgg.py or torchvision's ResNet) ---
+    if appear_arch == "vgg":
+        for s, stage in enumerate(VGG_STAGES):
+            for idx, cin, cout in stage:
+                _conv_bn(sd, f"appearance.layers.{s}", idx, cin, cout, 3)
+    elif appear_arch in RESNET_BLOCKS:
+        _resnet(sd, appear_arch)
+    else:
+        raise ValueError(f"unknown appearance arch {appear_arch!r}")
+    for s, c in enumerate(SKIP_CHANNELS if appear_arch == "vgg" else RES_SKIP_CHANNELS):
         p = f"appearance.global_pool.{s}.fc"
         m = skip_mid(c)
         sd[f"{p}.0.weight"] = ((c,), "norm_w")

@@ -11,16 +11,19 @@ import torch
 from .schema import state_schema
 
 
-def synthetic_state_dict(fusion="C", seed=0, point_in=3):
+def synthetic_state_dict(fusion="C", seed=0, point_in=3, appear_arch="vgg"):
     """A non-degenerate ``state_dict`` for ``TrackingNet`` with the reference's key names; point_in = 4 for a net on
-    xyz + reflectance points (``without_reflectivity=False``).
+    xyz + reflectance points (``without_reflectivity=False``); appear_arch "vgg" or "resnet50" / "resnet101" /
+    "resnet152" for the appearance trunk.
 
     Default inits make every GroupNorm the identity affine and both STN output layers zero
     (reference: modules/point_net.py:69-70), which hides bugs; so norm affines, BN running
-    statistics and the STN output layers are all randomised."""
+    statistics and the STN output layers are all randomised.  The BatchNorm closing each residual branch of a ResNet
+    (bn3) gets a small scale, as trained ResNets have: with unit-scale branches the activations would double block
+    after block (2^50 through ResNet-152)."""
     g = torch.Generator().manual_seed(1000 + seed)
     sd = {}
-    for key, (shape, kind) in state_schema(fusion, point_in).items():
+    for key, (shape, kind) in state_schema(fusion, point_in, appear_arch).items():
         if kind == "conv":
             fan_in = 1
             for s in shape[1:]:
@@ -30,6 +33,8 @@ def synthetic_state_dict(fusion="C", seed=0, point_in=3):
             t = torch.rand(shape, generator=g) * 0.2 - 0.1
         elif kind == "norm_w":
             t = torch.rand(shape, generator=g) + 0.5
+        elif kind == "res_norm_w":
+            t = torch.rand(shape, generator=g) * 0.2 + 0.1
         elif kind == "norm_b":
             t = torch.rand(shape, generator=g) * 0.4 - 0.2
         elif kind == "run_mean":

@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .schema import BUFFER_KINDS, VGG_POOL_AFTER, VGG_STAGES, state_schema
+from .schema import BUFFER_KINDS, RESNET_BLOCKS, VGG_POOL_AFTER, VGG_STAGES, state_schema
 
 # conv k of the 13 is followed by a 2x2 max-pool (so the map of conv k+1 is 4x smaller)
 VGG_POOLED_BEFORE = [idx in VGG_POOL_AFTER[s] for s, stage in enumerate(VGG_STAGES) for idx, _, _ in stage]
@@ -58,7 +58,7 @@ def _default_init(shape, kind, gen):
         for s in shape[1:]:
             fan_in *= s
         return torch.randn(shape, generator=gen) * (2.0 / fan_in) ** 0.5
-    if kind in ("norm_w", "run_var"):
+    if kind in ("norm_w", "res_norm_w", "run_var"):
         return torch.ones(shape)
     if kind == "eye":
         return torch.eye(shape[0])
@@ -79,7 +79,8 @@ class TrackingNet(nn.Module):
         # rejected loudly instead of silently computing something different
         unsupported = []
         if appear_len != 512 or point_len != 512: unsupported.append("appear_len/point_len != 512")
-        if appear_arch != 'vgg' or not appear_skippool or appear_fpn: unsupported.append("appearance must be vgg + skippool")
+        if appear_arch not in ('vgg',) + tuple(RESNET_BLOCKS) or not appear_skippool or appear_fpn:
+            unsupported.append("appearance must be vgg, resnet50, resnet101 or resnet152 + skippool")
         if point_arch != 'v1': unsupported.append("point_arch must be v1")
         if end_arch != 'v2' or end_mode not in _lib.END_MODE: unsupported.append("end_arch must be v2, end_mode avg or max")
         if score_arch not in ('branch_cls', 'branch_reg'): unsupported.append("score_arch must be branch_cls/branch_reg")
@@ -95,12 +96,13 @@ class TrackingNet(nn.Module):
         self.affinity_op = affinity_op
         self.end_mode = end_mode
         self.score_fusion_arch = score_fusion_arch
+        self.appear_arch = appear_arch
         # dropblock / use_dropout are identity in eval mode; accepted for config compatibility
         self.dropblock, self.use_dropout = dropblock, use_dropout
         # PointNet's input width (tracking_net.py:41): xyz, or xyz + LiDAR reflectance
         self.point_channels = 4 - int(bool(without_reflectivity))
         gen = torch.Generator().manual_seed(0)
-        for key, (shape, kind) in state_schema(score_fusion_arch, self.point_channels).items():
+        for key, (shape, kind) in state_schema(score_fusion_arch, self.point_channels, appear_arch).items():
             _register(self, key, _default_init(shape, kind, gen), kind in BUFFER_KINDS)
         for name, prm in self.named_parameters():
             if name.endswith(".idt"):           # reference point_net.py:62: requires_grad=False
@@ -127,7 +129,7 @@ class TrackingNet(nn.Module):
                                   "(there is no CPU fallback)")
         if self._prepared is None or self._prepared.flat.device != dev:
             _lib.load()
-            self._prepared = DeviceWeights(self.state_dict(), self.score_fusion_arch, dev)
+            self._prepared = DeviceWeights(self.state_dict(), self.score_fusion_arch, dev, self.appear_arch)
         return self._prepared
 
     def _split_to_device(self, s_host, dev):
@@ -175,7 +177,8 @@ class TrackingNet(nn.Module):
                 need += [lib.mmmot_appearance_train_workspace(pairs * L, H, W), lib.mmmot_pointnet_train_workspace(pairs, L, P),
                          lib.mmmot_w_det_train_workspace(L)]
             else:
-                need += [lib.mmmot_appearance_workspace(pairs * L, H, W), lib.mmmot_pointnet_workspace(pairs, L, P)]
+                app = (lib.mmmot_appearance_workspace if self.appear_arch == "vgg" else lib.mmmot_appearance_resnet_workspace)
+                need += [app(pairs * L, H, W), lib.mmmot_pointnet_workspace(pairs, L, P)]
             need.append(lib.mmmot_fusion_det_workspace(pairs, L))
         return max(need)
 
@@ -206,6 +209,9 @@ class TrackingNet(nn.Module):
             bn_det = torch.zeros(2, 2, 512, device=dev)
             _lib.check(lib.mmmot_appearance_train_fwd(wts.ptr, _vp(crops), pairs * L, H, W, L, _vp(feats), _vp(bn_vgg), _vp(dm2),
                                                       _vp(dm3), wsp, wsn, st), "mmmot_appearance_train_fwd")
+        elif wts.resnet is not None:
+            _lib.check(lib.mmmot_appearance_resnet_fwd(wts.ptr, wts.rptr, _vp(crops), pairs * L, H, W, L, _vp(feats), wsp, wsn,
+                                                       st), "mmmot_appearance_resnet_fwd")
         else:
             _lib.check(lib.mmmot_appearance_fwd(wts.ptr, _vp(crops), pairs * L, H, W, L, _vp(feats), wsp, wsn, st),
                        "mmmot_appearance_fwd")
@@ -417,6 +423,9 @@ class TrackingNet(nn.Module):
         and the BatchNorm layers' running averages are updated.  Forward only: no autograd graph is built through the
         CUDA library."""
         splits = [int(s) for s in dets_split]
+        if self.training and self.appear_arch != "vgg":
+            raise NotImplementedError("mmmot_b200.TrackingNet: the training-mode forward (batch-statistics BatchNorm) "
+                                      "runs the VGG appearance trunk only")
         if self.training and len(splits) != 2:
             raise NotImplementedError("mmmot_b200.TrackingNet supports 2-frame samples (sample_max_len: 2)")
         L = sum(splits)

@@ -20,7 +20,7 @@ import ctypes
 import torch
 
 from . import _lib
-from .schema import SKIP_CHANNELS, VGG_STAGES
+from .schema import RES_SKIP_CHANNELS, RESNET_BLOCKS, SKIP_CHANNELS, VGG_STAGES, resnet_convs
 
 EPS = 1e-5
 W = _lib.W
@@ -77,16 +77,56 @@ def pack_px(packed_u8, M, K):
     return t[:, 0, :, :, :8].permute(0, 2, 1, 3, 4, 5).contiguous().reshape(-1).view(torch.uint8)   # kc, kg, hl, mg, r, e
 
 
-def prepare(state_dict, fusion):
+def _skip_heads(sd, out, channels):
+    """The four SkipPool heads' 10 tensors each (the layout of MMMOT_W_SKIP0) -> out[10 s + j]."""
+    f64 = lambda k: sd[k].double()
+    for s, c in enumerate(channels):
+        p = f"appearance.global_pool.{s}.fc"
+        base = 10 * s
+        out[base + 0] = f64(f"{p}.0.weight"); out[base + 1] = f64(f"{p}.0.bias")
+        out[base + 2] = f64(f"{p}.1.weight").reshape(-1, c).t(); out[base + 3] = f64(f"{p}.1.bias")
+        out[base + 4] = f64(f"{p}.2.weight"); out[base + 5] = f64(f"{p}.2.bias")
+        w2 = f64(f"{p}.4.weight")
+        out[base + 6] = w2.reshape(w2.shape[0], -1).t(); out[base + 7] = f64(f"{p}.4.bias")
+        out[base + 8] = f64(f"{p}.5.weight"); out[base + 9] = f64(f"{p}.5.bias")
+
+
+def fold_bn_nobias(sd, conv, bn):
+    """Eval BatchNorm folded into a bias-free conv (torchvision's): w * s, bias = beta - mean * s, in fp64."""
+    w = sd[f"{conv}.weight"].double()
+    s = sd[f"{bn}.weight"].double() / torch.sqrt(sd[f"{bn}.running_var"].double() + EPS)
+    return w * s.reshape(-1, 1, 1, 1), sd[f"{bn}.bias"].double() - sd[f"{bn}.running_mean"].double() * s
+
+
+def prepare_resnet(state_dict, arch):
+    """ResNet appearance trunk -> (convs, heads): convs in execution order (schema.resnet_convs), each (Wt [K][Cout] fp32,
+    bias [Cout] fp32, packed tiles uint8, out_scale) with every BatchNorm folded and the K order of
+    mmmot_resnet_weights (1x1: ci; 3x3: (ky*3+kx)*Cin + ci; stem: (ky*7+kx)*3 + ci, packed K zero-padded 147 -> 160);
+    heads: the 40 fp32 tensors of the four SkipPool heads, head s at [10 s, 10 s + 10)."""
+    sd = {k: v.detach().cpu() for k, v in state_dict.items()}
+    convs = []
+    for conv, bn, cin, cout, k, _ in resnet_convs(arch):
+        w, b = fold_bn_nobias(sd, conv, bn)
+        wt = w.permute(2, 3, 1, 0).reshape(k * k * cin, cout)       # [co][ci][ky][kx] -> [(ky*k+kx)*cin + ci][co]
+        packed, scale = pack_tc(wt)
+        convs.append((wt.contiguous().float(), b.float(), packed, scale))
+    heads = [None] * 40
+    _skip_heads(sd, heads, RES_SKIP_CHANNELS)
+    return convs, [t.contiguous().float() for t in heads]
+
+
+def prepare(state_dict, fusion, appear_arch="vgg"):
     """-> (list of fp32 CPU tensors indexed by weight id (None = unused), trans1 CxC (C = 3 xyz or 4 xyz +
-    reflectance: the checkpoint's point width), trans2 64x64, per-id tensor-core output scales)."""
+    reflectance: the checkpoint's point width), trans2 64x64, per-id tensor-core output scales).  With a ResNet
+    appearance trunk the VGG and SkipPool ids stay None (prepare_resnet holds that stage's operands)."""
     sd = {k: v.detach().cpu() for k, v in state_dict.items()}
     out = [None] * W["COUNT"]
     f64 = lambda k: sd[k].double()
+    vgg = appear_arch == "vgg"
 
     # VGG trunk
     i = 0
-    for s, stage in enumerate(VGG_STAGES):
+    for s, stage in enumerate(VGG_STAGES if vgg else ()):
         for idx, cin, cout in stage:
             w, b = _fold_bn(sd, f"appearance.layers.{s}.{idx}", f"appearance.layers.{s}.{idx + 1}")
             # [co][ci][ky][kx] -> Wt[(ky*3+kx)*cin + ci][co]
@@ -94,15 +134,10 @@ def prepare(state_dict, fusion):
             out[W["VGG_B0"] + i] = b
             i += 1
     # SkipPool heads
-    for s, c in enumerate(SKIP_CHANNELS):
-        p = f"appearance.global_pool.{s}.fc"
-        base = W["SKIP0"] + 10 * s
-        out[base + 0] = f64(f"{p}.0.weight"); out[base + 1] = f64(f"{p}.0.bias")
-        out[base + 2] = f64(f"{p}.1.weight").reshape(-1, c).t(); out[base + 3] = f64(f"{p}.1.bias")
-        out[base + 4] = f64(f"{p}.2.weight"); out[base + 5] = f64(f"{p}.2.bias")
-        w2 = f64(f"{p}.4.weight")
-        out[base + 6] = w2.reshape(w2.shape[0], -1).t(); out[base + 7] = f64(f"{p}.4.bias")
-        out[base + 8] = f64(f"{p}.5.weight"); out[base + 9] = f64(f"{p}.5.bias")
+    if vgg:
+        heads = [None] * 40
+        _skip_heads(sd, heads, SKIP_CHANNELS)
+        out[W["SKIP0"]:W["SKIP0"] + 40] = heads
     # PointNet trunk with the constant STN transforms folded in:
     #   x' = T1^T x  => conv1(x') = (W1 T1^T) x ;  x_local = T2^T x1 => conv2(x_local) = (W2 T2^T) x1
     pf = "point_net.feat"
@@ -169,7 +204,7 @@ def prepare(state_dict, fusion):
     # training-mode operands (SURVEY 8f N4): unfolded conv weights + BatchNorm affines of the layers whose BatchNorm
     # uses batch statistics in .train() (VGG trunk, w_det)
     i = 0
-    for s_, stage in enumerate(VGG_STAGES):
+    for s_, stage in enumerate(VGG_STAGES if vgg else ()):
         for idx, cin, cout in stage:
             cp, bp = f"appearance.layers.{s_}.{idx}", f"appearance.layers.{s_}.{idx + 1}"
             out[W["VGG_RAWW0"] + i] = f64(f"{cp}.weight").permute(2, 3, 1, 0).reshape(9 * cin, cout)
@@ -190,7 +225,7 @@ def prepare(state_dict, fusion):
     def put(wid, wt):
         out[wid], scales[wid] = pack_tc(wt)
     i = 0
-    for s_, stage in enumerate(VGG_STAGES):
+    for s_, stage in enumerate(VGG_STAGES if vgg else ()):
         for idx, cin, cout in stage:
             w, _ = _fold_bn(sd, f"appearance.layers.{s_}.{idx}", f"appearance.layers.{s_}.{idx + 1}")
             if i == 0:
@@ -198,8 +233,9 @@ def prepare(state_dict, fusion):
             else:
                 put(W["VGG_WP0"] + i, out[W["VGG_WT0"] + i])          # packed NHWC input: K order tap*Cin + ci
             i += 1
-    out[W["VGG_WPX0"]] = pack_px(out[W["VGG_WP0"]], 64, 27)
-    out[W["VGG_WPX0"] + 1] = pack_px(out[W["VGG_WP0"] + 1], 64, 576)
+    if vgg:
+        out[W["VGG_WPX0"]] = pack_px(out[W["VGG_WP0"]], 64, 27)
+        out[W["VGG_WPX0"] + 1] = pack_px(out[W["VGG_WP0"] + 1], 64, 576)
     for j in range(5):
         put(W["PN_WP1"] + j, out[W["PN_L1"] + 4 * j])
     put(W["PN_WHAP"], out[W["PN_WHAT"]])
@@ -219,8 +255,14 @@ class DeviceWeights:
     """All prepared tensors in ONE flat device buffer (256-byte aligned slices) + the pointer table
     handed to the C ABI."""
 
-    def __init__(self, state_dict, fusion, device):
-        tensors, self.trans1, self.trans2, scales = prepare(state_dict, fusion)
+    def __init__(self, state_dict, fusion, device, appear_arch="vgg"):
+        tensors, self.trans1, self.trans2, scales = prepare(state_dict, fusion, appear_arch)
+        nmain = len(tensors)
+        self.resnet = None
+        if appear_arch != "vgg":
+            # the ResNet trunk's operands ride in the same flat buffer, behind the weight-id table's tensors
+            convs, heads = prepare_resnet(state_dict, appear_arch)
+            tensors = tensors + [t for c in convs for t in (c[0], c[1], c[2].view(torch.float32))] + heads
         offs, total = [], 0
         for t in tensors:
             offs.append(total)
@@ -233,9 +275,21 @@ class DeviceWeights:
         self.flat = flat.to(device)
         self.table = _lib.Weights()
         base = self.flat.data_ptr()
-        for i, (t, o) in enumerate(zip(tensors, offs)):
+        for i, (t, o) in enumerate(zip(tensors[:nmain], offs)):
             self.table.w[i] = None if t is None else base + 4 * o
             self.table.tc_scale[i] = scales[i]
+        if appear_arch != "vgg":
+            r = self.resnet = _lib.ResnetWeights()
+            r.blocks[:] = RESNET_BLOCKS[appear_arch]
+            for i, c in enumerate(convs):
+                o = offs[nmain + 3 * i: nmain + 3 * i + 3]
+                r.wt[i], r.bias[i], r.wp[i] = (base + 4 * x for x in o)
+                r.wp_scale[i] = c[3]
+            ho = offs[nmain + 3 * len(convs):]
+            for s in range(4):
+                for j in range(10):
+                    r.head[s][j] = base + 4 * ho[10 * s + j]
+            self.rptr = ctypes.pointer(r)
         self.table.point_channels = int(state_dict["point_net.feat.conv1.weight"].shape[1])
         self.ptr = ctypes.pointer(self.table)
         self.trans1 = self.trans1.to(device)
