@@ -405,7 +405,9 @@ int mmmot_set_kseg(int chunks);
  *   bit 8 (256)  pixel-major kernel without halo boxes (nine boxes per channel chunk)
  *   bit 9 (512)  no fused max-pool in the conv epilogues (separate max-pool kernel)
  *   bit 10 (1024) generated-operand engine (csrc/gemm_gen.cuh): producers without the software pipeline, every GEN
+ *                 (GEN_NORM: plain producers instead of TMA-staged source rows)
  *   bit 12 (4096) generated-operand engine: GEN_NORM producers with the software pipeline (prefetching variant)
+ *                 instead of TMA-staged source rows
  *   bit 13 (8192) PointNet layers 3, 4 through norm_split + the TMA-fed kernel instead of GEN_NORM producers
  *   bit 14 (16384) first VGG layer with a separate im2col pre-pass instead of in-kernel operand producers */
 int mmmot_set_debug(int flags);
@@ -433,6 +435,8 @@ int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, const float* bi
  *   mmmot_set_debug state; computed on the host without any CUDA call.  m: detections of a pairwise launch.
  * gen_staged: 1 if that variant stages the pairwise sources in shared memory by TMA (GEN_PAIR_* at m == 128 without
  *   bit 10), else 0; computed on the host like gen_prefetch.
+ * gen_norm_staged: 1 if a GEN_NORM launch under mmmot_set_debug flags dbg stages its source rows in shared memory by
+ *   TMA (the default; not with bit 10 or bit 12), else 0; computed on the host without any CUDA call.
  * gen: Y[row][y_ms] (fp32 channels-last, first M channels written, or NULL) = op(x) W^T + bias (+ ReLU if relu), Wp =
  *   packed FP16 hi/lo tiles of W [M][K] (weights.py::pack_tc).  Columns (operand rows):
  *     uniform tiling (tile_tab NULL): `groups` groups of S columns, 256-column tiles; column s of group g reads source
@@ -446,6 +450,7 @@ int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, const float* bi
  *   the variant taken, as gen_prefetch. */
 int mmmot_debug_gen_prefetch(int gen, int m);
 int mmmot_debug_gen_staged(int gen, int m);
+int mmmot_debug_gen_norm_staged(int dbg);
 int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_scale, const float* bias, int relu, const float* src,
                     int ld_src, const float* gsc, const float* gsh, int n, int m, int Lf, int S, int groups, long x_gs,
                     long y_gs, const void* tile_tab, int num_tiles, float* Y, long y_ms, void* part, int* prefetched,

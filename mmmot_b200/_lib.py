@@ -82,6 +82,7 @@ SIGNATURES = {
     "mmmot_fetch_pinned_i32": (_i, [_vp, _vp, _l, _vp]),
     "mmmot_debug_gen_prefetch": (_i, [_i, _i]),
     "mmmot_debug_gen_staged": (_i, [_i, _i]),
+    "mmmot_debug_gen_norm_staged": (_i, [_i]),
     "mmmot_debug_gen": (_i, [_i, _i, _i, _vp, _f, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _l, _l, _vp, _i, _vp, _l, _vp,
                              ctypes.POINTER(_i), _vp]),
     "mmmot_debug_pn_contraction": (_i, [_vp, _vp, _i, _i, _l, _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_l), _vp, _f, _vp, _i, _i,

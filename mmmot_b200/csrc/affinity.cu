@@ -294,9 +294,9 @@ AfWs carve(MmArena& a, int pairs, int n, int m) {
 bool affinity_use_tc(int n, int m) { return mm_engine() == 2 || (mm_engine() == 0 && n * m >= 64); }
 
 template <int GEN>
-int launch_gen(const GemmP& p, const mmmot_weights* wts, int wid, const float* src, int src_m, const float* gsc,
-               const float* gsh, int n, int m, int Lf, cudaStream_t st) {
-  return gemm_gen_launch<GEN>(p, (const uint4*)wts->w[wid], wts->tc_scale[wid], src, src_m, gsc, gsh, n, m, Lf, st);
+int launch_gen(const GemmP& p, const mmmot_weights* wts, int wid, const float* src, int src_m, long src_rows,
+               const float* gsc, const float* gsh, int n, int m, int Lf, cudaStream_t st) {
+  return gemm_gen_launch<GEN>(p, (const uint4*)wts->w[wid], wts->tc_scale[wid], src, src_m, src_rows, gsc, gsh, n, m, Lf, st);
 }
 
 }  // namespace
@@ -353,10 +353,10 @@ extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int
     p.part = w.part;
     if (timed) mm_timing_begin(st, MM_T_AFF_L1, 2.0 * 1024 * 512 * (double)G * NM, 4.0 * 1024 * (double)G * NM);
     int r = affinity_op == MMMOT_AFF_MULTIPLY
-                ? launch_gen<gen::GEN_PAIR_MUL>(p, wts, MMMOT_W_AF_W01P, w.fcl, 0, nullptr, nullptr, n, m, L, st)
+                ? launch_gen<gen::GEN_PAIR_MUL>(p, wts, MMMOT_W_AF_W01P, w.fcl, 0, 0, nullptr, nullptr, n, m, L, st)
             : affinity_op == MMMOT_AFF_MINUS_ABS
-                ? launch_gen<gen::GEN_PAIR_ABS>(p, wts, MMMOT_W_AF_W01P, w.fcl, 0, nullptr, nullptr, n, m, L, st)
-                : launch_gen<gen::GEN_PAIR_SUB>(p, wts, MMMOT_W_AF_W01P, w.fcl, 0, nullptr, nullptr, n, m, L, st);
+                ? launch_gen<gen::GEN_PAIR_ABS>(p, wts, MMMOT_W_AF_W01P, w.fcl, 0, 0, nullptr, nullptr, n, m, L, st)
+                : launch_gen<gen::GEN_PAIR_SUB>(p, wts, MMMOT_W_AF_W01P, w.fcl, 0, 0, nullptr, nullptr, n, m, L, st);
     if (r) return r;
     if (timed) mm_timing_end(st);
   } else {
@@ -401,12 +401,12 @@ extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int
     p.tile_tab = w.tiles; p.num_tiles = ne_tiles;
     p.Y = w.h1; p.y_ms = 512;
     p.part = w.npart;
-    MM_TRY(launch_gen<gen::GEN_COPY>(p, wts, MMMOT_W_NE_W1P, w.v, 512, nullptr, nullptr, 0, 0, 0, st));
+    MM_TRY(launch_gen<gen::GEN_COPY>(p, wts, MMMOT_W_NE_W1P, w.v, 512, 0, nullptr, nullptr, 0, 0, 0, st));
     MM_TRY(stats_reduce(w.npart, 512, 2 * G, 0, w.gstart, w.nstats, st, 2));
     MM_TRY(gn_finalize(w.nstats, W[MMMOT_W_NE_G1W], W[MMMOT_W_NE_G1B], w.cnt, 0, 2 * G, 512, 512, w.nsc1, w.nsh1, st, 0, 0, ar.status()));
     p.bias = W[MMMOT_W_NE_B2]; p.M = 128;
     p.Y = w.h2; p.y_ms = 128;
-    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_NE_W2P, w.h1, 512, w.nsc1, w.nsh1, 0, 0, 0, st));
+    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_NE_W2P, w.h1, 512, ldv, w.nsc1, w.nsh1, 0, 0, 0, st));
     MM_TRY(stats_reduce(w.npart, 128, 2 * G, 0, w.gstart, w.nstats, st, 2));
     MM_TRY(gn_finalize(w.nstats, W[MMMOT_W_NE_G2W], W[MMMOT_W_NE_G2B], w.cnt, 0, 2 * G, 128, 128, w.nsc2, w.nsh2, st));
     ne_final_cl_kernel<<<mm_cdiv((long)G * (n + m) * 32, 256), 256, 0, st>>>(w.h2, w.nsc2, w.nsh2, W[MMMOT_W_NE_W3], W[MMMOT_W_NE_B3],
@@ -443,14 +443,14 @@ extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int
     p.Y = w.y2; p.y_gs = NM; p.y_ms = 512;
     p.part = w.part;
     if (timed) mm_timing_begin(st, MM_T_AFF_L2, 2.0 * 512 * 512 * (double)G * NM, 4.0 * (512 + 512) * (double)G * NM);
-    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W2P, w.y01, 1024, w.sc1, w.sh1, 0, 0, 0, st));
+    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W2P, w.y01, 1024, (long)G * NM, w.sc1, w.sh1, 0, 0, 0, st));
     if (timed) mm_timing_end(st);
     MM_TRY(stats_reduce(w.part, 512, G, tpg, nullptr, w.stats, st, 2));
     MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G2W], W[MMMOT_W_AF_G2B], nullptr, NM, G, 512, 1, w.sc2, w.sh2, st, 0, 0, ar.status()));
     p.bias = W[MMMOT_W_AF_B3]; p.M = 128;
     p.Y = w.y3; p.y_ms = 128;
     if (timed) mm_timing_begin(st, MM_T_AFF_L3, 2.0 * 128 * 512 * (double)G * NM, 4.0 * (512 + 128) * (double)G * NM);
-    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W3P, w.y2, 512, w.sc2, w.sh2, 0, 0, 0, st));
+    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W3P, w.y2, 512, (long)G * NM, w.sc2, w.sh2, 0, 0, 0, st));
     if (timed) mm_timing_end(st);
     MM_TRY(stats_reduce(w.part, 128, G, tpg, nullptr, w.stats, st, 2));
     MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G3W], W[MMMOT_W_AF_G3B], nullptr, NM, G, 128, 1, w.sc3, w.sh3, st));

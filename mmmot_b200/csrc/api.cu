@@ -244,6 +244,9 @@ extern "C" int mmmot_debug_gen_staged(int gen, int m) {
   return gen_staged(gen, m, mm_debug_flags()) ? 1 : 0;
 }
 
+// Whether a GEN_NORM launch under debug flags dbg stages its source rows by TMA (1) or not, on the host, no CUDA call.
+extern "C" int mmmot_debug_gen_norm_staged(int dbg) { return gen_norm_staged(dbg) ? 1 : 0; }
+
 // One contraction of the generated-operand tensor-core engine (gemm_gen.cuh) through gemm_gen_launch, with the
 // arguments the affinity, PointNet and fusion stages pass it.
 extern "C" int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_scale, const float* bias, int relu,
@@ -265,12 +268,21 @@ extern "C" int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_s
   p.part = (double2*)part;
   const uint4* w = (const uint4*)Wp;
   cudaStream_t st = (cudaStream_t)stream;
+  // rows of the source the launch reads: the end of the last group, or of the table's last-ending tile (the stages pass
+  // their source's row count; here it is read back from the table)
+  long src_rows = tile_tab ? 0 : (long)(groups - 1) * x_gs + S;
+  if (tile_tab && gen == gen::GEN_NORM) {
+    std::vector<int4> tt(num_tiles);
+    MM_CUDA(cudaMemcpyAsync(tt.data(), tile_tab, sizeof(int4) * num_tiles, cudaMemcpyDeviceToHost, st));
+    MM_CUDA(cudaStreamSynchronize(st));
+    for (const int4& t : tt) src_rows = std::max(src_rows, (long)t.y + t.z);
+  }
   switch (gen) {
-    case gen::GEN_PAIR_MUL: return gemm_gen_launch<gen::GEN_PAIR_MUL>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
-    case gen::GEN_PAIR_ABS: return gemm_gen_launch<gen::GEN_PAIR_ABS>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
-    case gen::GEN_PAIR_SUB: return gemm_gen_launch<gen::GEN_PAIR_SUB>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
-    case gen::GEN_NORM: return gemm_gen_launch<gen::GEN_NORM>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
-    case gen::GEN_COPY: return gemm_gen_launch<gen::GEN_COPY>(p, w, wp_scale, src, ld_src, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_PAIR_MUL: return gemm_gen_launch<gen::GEN_PAIR_MUL>(p, w, wp_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_PAIR_ABS: return gemm_gen_launch<gen::GEN_PAIR_ABS>(p, w, wp_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_PAIR_SUB: return gemm_gen_launch<gen::GEN_PAIR_SUB>(p, w, wp_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_NORM: return gemm_gen_launch<gen::GEN_NORM>(p, w, wp_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st, prefetched);
+    case gen::GEN_COPY: return gemm_gen_launch<gen::GEN_COPY>(p, w, wp_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st, prefetched);
     default: return MMMOT_E_ARG;
   }
 }

@@ -188,7 +188,7 @@ extern "C" int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, i
       p.x_gs = L;                                            // rows per group (= per pair) of the source view below
       p.Y = Y; p.y_gs = L; p.y_ms = 512;
       p.part = stats ? w.part : nullptr;
-      MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[wp_id], wts->tc_scale[wp_id], w.f3 + (long)stack * 512, 1536,
+      MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[wp_id], wts->tc_scale[wp_id], w.f3 + (long)stack * 512, 1536, 0,
                                              nullptr, nullptr, 0, 0, 0, st)));
       if (stats) MM_TRY(stats_reduce(w.part, 512, pairs, tpg2, nullptr, w.stats, st, 2));
       if (stats) MM_TRY(gn_finalize(w.stats, wts->w[gw], wts->w[gb], nullptr, L, pairs, 512, 1, sc, sh, st));
@@ -214,11 +214,11 @@ extern "C" int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, i
     p.S = (int)rows; p.tiles_per_group = mm_cdiv(rows, tc::BN); p.num_tiles = p.tiles_per_group;
     p.x_gs = rows;
     p.Y = w.h1; p.y_gs = rows; p.y_ms = 512;
-    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W1P], wts->tc_scale[MMMOT_W_WD_W1P], w.f3, 512, nullptr,
+    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W1P], wts->tc_scale[MMMOT_W_WD_W1P], w.f3, 512, 0, nullptr,
                                            nullptr, 0, 0, 0, st)));
     p.bias = wts->w[MMMOT_W_WD_B2]; p.M = 256;
     p.Y = w.h2; p.y_ms = 256;
-    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W2P], wts->tc_scale[MMMOT_W_WD_W2P], w.h1, 512, nullptr,
+    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W2P], wts->tc_scale[MMMOT_W_WD_W2P], w.h1, 512, 0, nullptr,
                                            nullptr, 0, 0, 0, st)));
     det_score_rows_kernel<<<mm_cdiv(rows * 32, 256), 256, 0, st>>>(w.h2, wts->w[MMMOT_W_WD_W3], wts->w[MMMOT_W_WD_B3], score_flags,
                                                                   neg_threshold, rows, L, det_scores);

@@ -17,10 +17,10 @@
 // CTA (512 threads, persistent, one per SM): warps 0-7 are two consumer warpgroups (warpgroup h issues the wgmma chains
 // of the tile's 128 rows x column half h and runs that half's epilogue), warps 8-15 operand producers; the first
 // producer thread also fetches each chunk's pre-tiled FP16 hi/lo weight block (cp.async.bulk) and, for the pairwise
-// producers at m == 128, the chunk's fp32 sources (TMA, see gemm_gen_kernel).  One mbarrier per stage collects the
+// producers at m == 128 and GEN_NORM, the chunk's fp32 sources (TMA, see gemm_gen_kernel).  One mbarrier per stage collects the
 // weight expect_tx and the eight producer warps' arrivals.  The consumers hold 128 accumulator registers
 // each and take registers from the producers (setmaxnreg).  The accumulator image of a finished tile overlays
-// stages 0-1 of the ring, so the producers start the next tile once the epilogue has read it.
+// the first 128 KB of the ring, so the producers start the next tile once the epilogue has read it.
 #pragma once
 #include "gemm_tma.cuh"
 
@@ -43,6 +43,17 @@ constexpr int G_SRC_AHEAD = STAGES - 1;   // chunks whose sources are in flight 
 constexpr size_t G_SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 + 256 + STAGES * G_OBJ_BYTES;
 constexpr int G_MAX_K = 512;   // producer-side GroupNorm affine staged in shared memory
 __host__ __device__ constexpr bool staged(int GEN, bool PAIRED) { return PAIRED && GEN <= GEN_PAIR_SUB; }
+// Staged GroupNorm sources (GEN_NORM, ROW_TMA): three 48 KB operand stages (weight block | B hi | B lo, no free slot,
+// like tma::T_STAGE_BYTES) and a separate ring of G_NSRC slots, each one chunk's [256 rows x 32 channels] fp32 source
+// box (128-byte swizzle).  The accumulator image overlays the operand stages only, so the next tile's first boxes land
+// in the source slots while the epilogue still reads the image.
+constexpr int G_NSTAGE_BYTES = A_SUB + 2 * B_HALF;
+constexpr int G_SRC_BYTES = BN * BK * 4, G_NSRC = 2;
+constexpr size_t G_NSMEM_BYTES = (size_t)STAGES * G_NSTAGE_BYTES + G_NSRC * G_SRC_BYTES + 1024 + 256;
+static_assert(G_NSMEM_BYTES + 2 * G_MAX_K * 4 <= 227 * 1024, "staged GEN_NORM exceeds the 227 KB of shared memory per block");
+static_assert(STAGES * G_NSTAGE_BYTES >= 128 * BN * 4, "the accumulator image must fit in the operand stages it overlays");
+static_assert((STAGES * G_NSTAGE_BYTES) % 1024 == 0 && G_SRC_BYTES % 1024 == 0, "source slots 1024-aligned (128-byte swizzle)");
+static_assert(G_NSRC <= STAGES, "the source barriers reuse the pairwise staging's src_full / src_empty slots");
 
 struct GenP {
   TcP t;               // .g: M, K, bias, S (columns per group), tiles_per_group, num_tiles, Y / y_gs / y_ms (fp32
@@ -72,16 +83,22 @@ __device__ __forceinline__ void ld_global_256(const float* p, float (&v)[8]) {
 // G_SRC_AHEAD chunks ahead of the conversion; the producers hold no prefetch in registers.
 // GEN_NORM, GEN_COPY: the next chunk's source vectors are loaded into registers before the current chunk is converted
 // (any shape; GEN_NORM then re-reads the GroupNorm affine from shared memory per pair of items).
-template <int GEN, bool PAIRED>
+// ROW_TMA (GEN_NORM, !PAIRED): each chunk's [256 rows x 32 channels] source box is staged in shared memory by TMA
+// (map_det over the source rows), G_NSRC chunks ahead and across tile boundaries (G_NSTAGE_BYTES).
+template <int GEN, bool PAIRED, bool ROW_TMA = false>
 static __global__ void __launch_bounds__(G_THREADS, 1)
 gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const __grid_constant__ CUtensorMap map_obj) {
+  static_assert(!ROW_TMA || (GEN == GEN_NORM && !PAIRED), "source rows are staged for the plain GEN_NORM producers only");
+  constexpr int SB = ROW_TMA ? G_NSTAGE_BYTES : STAGE_BYTES;   // operand stage stride
+  constexpr int B_OFF = ROW_TMA ? A_SUB : 2 * A_SUB;           // generated operand (hi | lo) within a stage
   const GemmP& p = P.t.g;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(16) float s_gsc[GEN == GEN_NORM ? G_MAX_K : 4], s_gsh[GEN == GEN_NORM ? G_MAX_K : 4];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t bar0 = base + STAGES * STAGE_BYTES;
+  const uint32_t src0 = base + STAGES * SB;                    // ROW_TMA: the source slots
+  const uint32_t bar0 = src0 + (ROW_TMA ? G_NSRC * G_SRC_BYTES : 0);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
   const uint32_t free_bar = bar0 + 8u * (2 * STAGES);   // the epilogue has read the accumulator image
@@ -101,7 +118,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
     for (int s = 0; s < STAGES; s++) {
       mbar_init(full_bar(s), 1 + G_PROD_WARPS);   // weight expect_tx arrive + one arrive per producer warp
       mbar_init(empty_bar(s), G_EPI_WARPS);       // one arrive per consumer warp once its wgmmas have read the stage
-      if (staged(GEN, PAIRED)) {
+      if (staged(GEN, PAIRED) || (ROW_TMA && s < G_NSRC)) {
         mbar_init(src_full(s), 1);
         mbar_init(src_empty(s), G_PROD_WARPS);
       }
@@ -132,20 +149,21 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
 #pragma unroll
         for (int i = 0; i < 64; i++) acc[mb][i] = 0.f;
     };
-    if (!staged(GEN, PAIRED)) clear_acc();
+    constexpr bool TILE_CLEAR = staged(GEN, PAIRED) || ROW_TMA;
+    if (!TILE_CLEAR) clear_acc();
     for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       const int mg = (int)(t % mgroups);
       const int nt = (int)(t / mgroups);
       int g, c0, len;
       tile_cols(nt, g, c0, len);
-      // The first wgmma of each chain ignores the accumulators (scale_d = 0).  Staged pairwise variant: clearing them
-      // here rather than once per CTA leaves them dead from the image dump to the next tile, so the epilogue has their
+      // The first wgmma of each chain ignores the accumulators (scale_d = 0).  Staged variants: clearing them here
+      // rather than once per CTA leaves them dead from the image dump to the next tile, so the epilogue has their
       // registers (no spills).
-      if (staged(GEN, PAIRED)) clear_acc();
+      if (TILE_CLEAR) clear_acc();
       for (int kc = 0; kc < KC; kc++, it++) {
         const int s = it % STAGES;
         mbar_wait(full_bar(s), (it / STAGES) & 1);
-        const uint32_t sa = base + s * STAGE_BYTES, sb = sa + 2 * A_SUB + half * (128 / 8) * 128;
+        const uint32_t sa = base + s * SB, sb = sa + B_OFF + half * (128 / 8) * 128;
         if (!(P.t.dbg & 8)) {
           wgmma_fence();
 #pragma unroll
@@ -249,13 +267,35 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
     uint32_t it = 0, wcount = 0;
     int g_staged = -1;
     struct Raw { float a[NA][8]; float b[NB ? NB : 1][8]; };
+    // ROW_TMA: sit counts the source boxes this thread has taken; the first producer thread issues box is_pos = chunk
+    // is_kc of tile is_t, G_NSRC boxes ahead of sit, across tile boundaries
+    const bool gen_ops = !(P.t.dbg & 4);
+    uint32_t sit = 0, is_pos = 0;
+    long is_t = blockIdx.x;
+    int is_kc = 0;
+    auto issue_next = [&]() {
+      if (is_t >= total_tiles) return;
+      const int ss = is_pos % G_NSRC;
+      mbar_wait(src_empty(ss), ((is_pos / G_NSRC) & 1) ^ 1u);
+      int g, c0, len;
+      tile_cols((int)(is_t / mgroups), g, c0, len);
+      mbar_expect_tx(src_full(ss), G_SRC_BYTES);   // rows past the tensor are zero-filled and counted
+      tma::tma_load_2d(src0 + ss * G_SRC_BYTES, &map_det, is_kc * BK, (int)(g * p.x_gs + c0), src_full(ss));
+      is_pos++;
+      if (++is_kc == KC) { is_kc = 0; is_t += gridDim.x; }
+    };
+    if (ROW_TMA && pt == 0 && gen_ops)
+      for (int i = 0; i < G_NSRC; i++) issue_next();
+    // ROW_TMA: box row j of a chunk is tile row j, 16-byte unit u of it at u ^ (j & 7) (128-byte swizzle).  A thread's
+    // four rows cb + 64 r share j & 7 = cb & 7; a quarter warp's eight rows are consecutive: eight different j & 7, so
+    // its 16-byte reads of one k group hit eight different bank groups.  Rows past the group are masked by okmask.
+    const uint32_t u0 = (uint32_t)(((2 * kg) ^ (cb & 7)) * 16), u1 = (uint32_t)(((2 * kg + 1) ^ (cb & 7)) * 16);
+    uint32_t src_rb = 0;   // this thread's row cb in the current chunk's source slot
     for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       const int mg = (int)(t % mgroups);
       const int nt = (int)(t / mgroups);
       int g, c0, len;
       tile_cols(nt, g, c0, len);
-      if (wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);   // the previous tile's accumulator image has been read
-      wcount++;
       unsigned okmask = 0;
       // 32-bit element offsets of the items' rows (this thread's k group) relative to the tile's / group's base
       const float* tbase = ROWS ? P.src + ((long)g * p.x_gs + c0) * P.ld_src : P.src + (long)g * P.Lf * p.K;
@@ -288,6 +328,9 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
         asm volatile("bar.sync 1, %0;" ::"n"(G_PROD_WARPS * 32) : "memory");
         g_staged = g;
       }
+      // the affine (separate from the ring) is staged above while the consumers may still read the accumulator image
+      if (wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);   // the previous tile's accumulator image has been read
+      wcount++;
       auto load = [&](Raw& R, int kc) {
         if (P.t.dbg & 4) return;
 #pragma unroll
@@ -304,11 +347,11 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
             mbar_arrive(full_bar(s));
           } else {
             mbar_expect_tx(full_bar(s), A_SUB);
-            bulk_g2s(base + s * STAGE_BYTES, reinterpret_cast<const uint8_t*>(P.t.Wp) + ((size_t)kc * P.t.m_tiles + mg) * A_SUB,
+            bulk_g2s(base + s * SB, reinterpret_cast<const uint8_t*>(P.t.Wp) + ((size_t)kc * P.t.m_tiles + mg) * A_SUB,
                      A_SUB, full_bar(s));
           }
         }
-        uint8_t* bh = sm + s * STAGE_BYTES + 2 * A_SUB + off0;
+        uint8_t* bh = sm + s * SB + B_OFF + off0;
         if (!(P.t.dbg & 4)) {
           const uint32_t sca = smem_u32(s_gsc + kc * BK + kg * 8), sha = smem_u32(s_gsh + kc * BK + kg * 8);
           float4 sc0, sc1, sh0, sh1;
@@ -316,7 +359,14 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
           for (int r = 0; r < 4; r++) {
             float x[8];
             if (GEN == GEN_NORM) {
-              const float(&y)[8] = R.a[r];
+              float ys[8];
+              if constexpr (ROW_TMA) {   // row cb + 64 r of the staged box, channels kg*8 .. kg*8 + 7
+                float4 v0, v1;
+                lds128(src_rb + r * 64 * 128 + u0, v0);
+                lds128(src_rb + r * 64 * 128 + u1, v1);
+                ys[0] = v0.x; ys[1] = v0.y; ys[2] = v0.z; ys[3] = v0.w; ys[4] = v1.x; ys[5] = v1.y; ys[6] = v1.z; ys[7] = v1.w;
+              }
+              const float* y = ROW_TMA ? ys : R.a[r];
               // prefetching variant: the affine is re-read from shared memory per pair of items (volatile asm) instead
               // of holding the eight (scale, shift) pairs across the chunk: 16 registers for the prefetched vectors
               if (!PAIRED ? r == 0 : !(r & 1)) { lds128(sca, sc0); lds128(sca + 16, sc1); lds128(sha, sh0); lds128(sha + 16, sh1); }
@@ -357,7 +407,6 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
         // was last read by chunk c - 1, so the refill waits only for every producer warp to be done with that one.
         // A quarter warp's eight detections j = cb + 64 b share a k group and have eight different j & 7: its 16-byte
         // reads hit eight different bank groups.
-        const bool gen_ops = !(P.t.dbg & 4);
         const int row_det = g * P.Lf + P.n, row_obj = g * P.Lf + c0 / P.m;
         auto issue = [&](uint32_t pos, int kc) {
           const int s = pos % STAGES;
@@ -421,6 +470,22 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
           if (pt == 0 && gen_ops && kc + G_SRC_AHEAD < KC) issue(it + G_SRC_AHEAD, kc + G_SRC_AHEAD);
           it++;
         }
+      } else if (ROW_TMA) {
+        // emit converts straight from the chunk's source slot; once every producer warp is done with it, the first
+        // producer thread refills it with the box G_NSRC ahead (past the tile's last chunk: the next tile's).
+        Raw R;   // not read
+        for (int kc = 0; kc < KC; kc++) {
+          const int ss = sit % G_NSRC;
+          src_rb = src0 + ss * G_SRC_BYTES + (uint32_t)cb * 128u;
+          if (gen_ops) mbar_wait(src_full(ss), (sit / G_NSRC) & 1);
+          emit(R, kc);
+          if (gen_ops) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(src_empty(ss));
+            if (pt == 0) issue_next();
+          }
+          sit++;
+        }
       } else if (PREFETCH) {
         Raw R0, R1;
         load(R0, 0);
@@ -448,18 +513,22 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
 // Host launcher.  g: M, K (multiple of 32, <= 512 for GEN_NORM), bias, S / tiles_per_group / num_tiles (uniform column
 // tiling, 256 columns per tile) or tile_tab (GEN_NORM, GEN_COPY: ragged groups, absolute rows), x_gs (NORM: source rows per group), Y / y_gs / y_ms = fp32 channels-last output (or
 // null), part = two GroupNorm partials per tile (stats_reduce(..., mult = 2)).  Wp = weights packed by
-// weights.py::pack_tc.  PAIR: src = fcl [G][Lf][K]; NORM: src = [G*x_gs][ld_src] fp32, gsc/gsh [G][K].
-template <int GEN, bool PAIRED>
-static int gemm_gen_launch_t(const GemmP& g, const uint4* Wp, float out_scale, const float* src, int ld_src,
-                           const float* gsc, const float* gsh, int n, int m, int Lf, cudaStream_t st) {
+// weights.py::pack_tc.  PAIR: src = fcl [G][Lf][K]; NORM: src = [src_rows][ld_src] fp32, gsc/gsh [G][K].
+// src_rows: rows of a GEN_NORM source (the extent of its tensor map; rows past it read as zero), unused otherwise.
+template <int GEN, bool PAIRED, bool ROW_TMA = false>
+static int gemm_gen_launch_t(const GemmP& g, const uint4* Wp, float out_scale, const float* src, int ld_src, long src_rows,
+                             const float* gsc, const float* gsh, int n, int m, int Lf, cudaStream_t st) {
   if (!Wp || !src || g.num_tiles <= 0 || g.K % tc::BK) return MMMOT_E_ARG;
   if (g.tile_tab && ((GEN != gen::GEN_NORM && GEN != gen::GEN_COPY) || g.x_gs || g.y_gs)) return MMMOT_E_ARG;
   if (GEN == gen::GEN_NORM && (g.K > gen::G_MAX_K || !gsc || !gsh)) return MMMOT_E_ARG;
   if ((GEN == gen::GEN_NORM || GEN == gen::GEN_COPY) && (ld_src < g.K || (ld_src & 7))) return MMMOT_E_ARG;
+  // TMA: 16-byte aligned base (the row stride, ld_src * 4 bytes, is a multiple of 32)
+  if (ROW_TMA && (src_rows <= 0 || (reinterpret_cast<uintptr_t>(src) & 15))) return MMMOT_E_ARG;
+  constexpr size_t smem = ROW_TMA ? gen::G_NSMEM_BYTES : gen::G_SMEM_BYTES;
   int sms = 0;
   MM_TRY(mm_sm_count(&sms));
   static std::atomic<unsigned long long> attr{0};
-  MM_TRY(mm_ensure_smem(gen::gemm_gen_kernel<GEN, PAIRED>, gen::G_SMEM_BYTES, attr));
+  MM_TRY(mm_ensure_smem(gen::gemm_gen_kernel<GEN, PAIRED, ROW_TMA>, smem, attr));
   gen::GenP P;
   memset(&P, 0, sizeof(P));
   P.t.g = g;
@@ -478,12 +547,13 @@ static int gemm_gen_launch_t(const GemmP& g, const uint4* Wp, float out_scale, c
     // two whole object rows per tile against all m = 128 detections; maps over the feature stacks [G * Lf][K]
     if (m != 128 || Lf != n + m || g.tile_tab || g.tiles_per_group <= 0) return MMMOT_E_ARG;
     const long rows = (long)(g.num_tiles / g.tiles_per_group) * Lf;
-    MM_TRY(tma::make_map_2d_f32(&map_det, src, rows, g.K, 128, CU_TENSOR_MAP_SWIZZLE_128B));
-    MM_TRY(tma::make_map_2d_f32(&map_obj, src, rows, g.K, 2, CU_TENSOR_MAP_SWIZZLE_NONE));
+    MM_TRY(tma::make_map_2d_f32(&map_det, src, rows, g.K, g.K, 128, CU_TENSOR_MAP_SWIZZLE_128B));
+    MM_TRY(tma::make_map_2d_f32(&map_obj, src, rows, g.K, g.K, 2, CU_TENSOR_MAP_SWIZZLE_NONE));
   }
+  if (ROW_TMA) MM_TRY(tma::make_map_2d_f32(&map_det, src, src_rows, g.K, ld_src, tc::BN, CU_TENSOR_MAP_SWIZZLE_128B));
   const long total = (long)g.num_tiles * P.t.m_tiles;
   const int grid = (int)(total < sms ? total : sms);
-  gen::gemm_gen_kernel<GEN, PAIRED><<<grid, gen::G_THREADS, gen::G_SMEM_BYTES, st>>>(P, map_det, map_obj);
+  gen::gemm_gen_kernel<GEN, PAIRED, ROW_TMA><<<grid, gen::G_THREADS, smem, st>>>(P, map_det, map_obj);
   MM_LAUNCH_CHECK();
   return 0;
 }
@@ -505,13 +575,21 @@ static inline bool gen_staged(int GEN, int m, int dbg) {
   return GEN <= gen::GEN_PAIR_SUB && gen_prefetch(GEN, m, dbg);
 }
 
+// Whether a GEN_NORM launch stages its source rows by TMA (gemm_gen_kernel<GEN_NORM, false, true>): the default; bit 10
+// keeps the plain producers (the bit-for-bit reference), bit 12 the prefetching ones.  Pure host logic, like gen_prefetch
+// (mmmot_debug_gen_norm_staged).
+static inline bool gen_norm_staged(int dbg) { return !(dbg & (1024 | 4096)); }
+
 // prefetched (host, or NULL) receives the variant taken (gen_prefetch)
 template <int GEN>
-static int gemm_gen_launch(const GemmP& g, const uint4* Wp, float out_scale, const float* src, int ld_src,
+static int gemm_gen_launch(const GemmP& g, const uint4* Wp, float out_scale, const float* src, int ld_src, long src_rows,
                            const float* gsc, const float* gsh, int n, int m, int Lf, cudaStream_t st,
                            int* prefetched = nullptr) {
-  const bool pipe = gen_prefetch(GEN, m, mm_debug_flags());
+  const int dbg = mm_debug_flags();
+  const bool pipe = gen_prefetch(GEN, m, dbg);
   if (prefetched) *prefetched = pipe ? 1 : 0;
-  if (pipe) return gemm_gen_launch_t<GEN, true>(g, Wp, out_scale, src, ld_src, gsc, gsh, n, m, Lf, st);
-  return gemm_gen_launch_t<GEN, false>(g, Wp, out_scale, src, ld_src, gsc, gsh, n, m, Lf, st);
+  if (pipe) return gemm_gen_launch_t<GEN, true>(g, Wp, out_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st);
+  if constexpr (GEN == gen::GEN_NORM)
+    if (gen_norm_staged(dbg)) return gemm_gen_launch_t<GEN, false, true>(g, Wp, out_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st);
+  return gemm_gen_launch_t<GEN, false>(g, Wp, out_scale, src, ld_src, src_rows, gsc, gsh, n, m, Lf, st);
 }

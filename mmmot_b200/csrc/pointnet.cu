@@ -691,7 +691,7 @@ int pointnet_tc(const mmmot_weights* wts, const float* points, const int* det_sp
     if (gen_mid && i > 1) {
       // layers 3, 4: GroupNorm + ReLU of the previous layer applied by this contraction's operand producers
       // (gemm_gen.cuh) straight from its fp32 output: no normalised copy is written
-      MM_TRY((gemm_gen_launch<gen::GEN_NORM>(p, wp, wps, ys[i - 2], cin, w.sc, w.sh, 0, 0, 0, st)));
+      MM_TRY((gemm_gen_launch<gen::GEN_NORM>(p, wp, wps, ys[i - 2], cin, P, w.sc, w.sh, 0, 0, 0, st)));
     } else {                                                // FP16 hi/lo planes [2][P][cin] via TMA
       MM_TRY(gemm_tma_launch_mat(p, wp, wps, i == 1 ? w.x1p : w.xp, P * cin, P, cin, tc::OUT_CL, 0, st));
     }
@@ -716,7 +716,7 @@ int pointnet_tc(const mmmot_weights* wts, const float* points, const int* det_sp
     p.S = ndet; p.tiles_per_group = mm_cdiv(ndet, tc::BN); p.num_tiles = p.tiles_per_group;
     p.x_gs = ndet;
     p.Y = w.ut; p.y_gs = ndet; p.y_ms = 512;
-    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WHGP], wts->tc_scale[MMMOT_W_PN_WHGP], w.gmean, 1024,
+    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WHGP], wts->tc_scale[MMMOT_W_PN_WHGP], w.gmean, 1024, 0,
                                            nullptr, nullptr, 0, 0, 0, st)));
   }
   MM_TRY(pn_wide_layer(w, h_det_split, det_split, P, pairs, L, n_tiles, w.x1p, 64, wts->w[MMMOT_W_PN_WHAT],
@@ -730,7 +730,7 @@ int pointnet_tc(const mmmot_weights* wts, const float* points, const int* det_sp
   p.x_gs = L;
   p.Y = w.o; p.y_gs = L; p.y_ms = 512;
   p.part = w.part;
-  MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WOP], wts->tc_scale[MMMOT_W_PN_WOP], w.hmean, 512,
+  MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_PN_WOP], wts->tc_scale[MMMOT_W_PN_WOP], w.hmean, 512, 0,
                                          nullptr, nullptr, 0, 0, 0, st)));
   MM_TRY(stats_reduce(w.part, 512, pairs, tpg2, nullptr, w.stats, st, 2));
   MM_TRY(gn_finalize(w.stats, wts->w[MMMOT_W_PN_GOW], wts->w[MMMOT_W_PN_GOB], nullptr, L, pairs, 512, 32, w.sc, w.sh, st));
