@@ -204,6 +204,48 @@ int mmmot_debug_resnet_op(int op, const mmmot_resnet_weights* rw, int conv, int 
                           void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Appearance on a ResNet-50/101/152 trunk + the FPN head -> stack 0 of feats (reference appear_arch resnetXX with
+ * appear_skippool False, appear_fpn True: modules/appear_net.py:83-104,192-210).  Eval mode, BatchNorm folded
+ * (weights.py::prepare_fpn).  The trunk is mmmot_appearance_resnet_fwd's; the head, on the outputs f_k of layer k+1
+ * (C_k = 256 << k channels):
+ *   lat_k = relu(fpn_in[k](f_k)),  out = lat_3 upsampled (bilinear) and added level by level down to lat_0,
+ *   feats = relu(conv_last(avgpool(out))).
+ * With H and W multiples of 32 every upsample is an exact 2x, which preserves the mean, so avgpool(out) is computed as
+ * the sum of the four laterals' per-image means; no lateral or upsampled map is stored.
+ *   lat_wt[k]        fp32 Wt[C_k][512]: fpn_in[k].0 with fpn_in[k].1 folded (FP32 engine)
+ *   lat_bias[k]      [512] the folded BatchNorm shift
+ *   lat_wp[k]        the same matrix as packed FP16 hi/lo tiles (weights.py::pack_tc), lat_wp_scale[k] its output scale
+ *   last_wt, last_bias  fp32 Wt[512][512] and [512]: conv_last.1 with conv_last.2 folded
+ */
+typedef struct mmmot_fpn_weights {
+  const float* lat_wt[4];
+  const float* lat_bias[4];
+  const void* lat_wp[4];
+  float lat_wp_scale[4];
+  const float* last_wt;
+  const float* last_bias;
+} mmmot_fpn_weights;
+/* workspace: mmmot_appearance_resnet_fpn_workspace(n_img, H, W, L) bytes (no device needed; the same for both engines
+ * and every block count).  rw->head is not read.  Returns what mmmot_appearance_resnet_fwd returns for the same
+ * arguments (MMMOT_E_ARG also for a null pointer in fw), before any CUDA call.  Engine: as mmmot_appearance_resnet_fwd
+ * up to 23 layer3 blocks (ResNet-50/101); deeper trunks (ResNet-152) always run on the FP32 engine, because without a
+ * GroupNorm after the head the tensor-core trunk's accumulated error takes the scores past 1e-4 relative.
+ * A pair's result does not depend on the other pairs of the call (the laterals' column tiles never straddle two). */
+size_t mmmot_appearance_resnet_fpn_workspace(int n_img, int H, int W, int L);
+int mmmot_appearance_resnet_fpn_fwd(const mmmot_resnet_weights* rw, const mmmot_fpn_weights* fw, const float* crops, int n_img,
+                                    int H, int W, int L, float* feats, void* workspace, size_t workspace_bytes, void* stream);
+/* Test hook of the FPN head, through the code mmmot_appearance_resnet_fpn_fwd runs.  Engine as mmmot_debug_resnet_op.
+ *   op 0 lateral `level` (0..3): X = a stage output (C = 256 << level channels at h x w, the engine's layout of
+ *        mmmot_debug_resnet_op) -> Y = the per-image means of relu(lateral) [n][512]; L images per pair; workspace:
+ *        mmmot_appearance_resnet_fpn_workspace(n_img, h << (level + 2), w << (level + 2), L) bytes (tensor cores: FP16
+ *        range flag in its status word)
+ *   op 1 head: X = the four level means [4][n][512] -> Y = feats [n/L][3][512][L], stack 0 (level, h, w, workspace
+ *        unused)
+ * MMMOT_E_ARG, before any CUDA call, for an unknown op or arguments the op cannot take. */
+int mmmot_debug_fpn_op(int op, const mmmot_fpn_weights* fw, int level, int n_img, int h, int w, int L, const void* X, float* Y,
+                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * PointNet encoder over ragged per-detection point sets -> stack 1 of feats.
  * Replaces PointNet_v1.forward, reference modules/point_net.py:25-44,115-153.
  *   points     [P_total][C]  C = wts->point_channels: xyz, or xyz + reflectance (16-byte aligned rows), detections

@@ -50,6 +50,12 @@ class ResnetWeights(ctypes.Structure):
                 ("wp_scale", ctypes.c_float * RESNET_MAX_CONVS), ("head", (ctypes.c_void_p * 10) * 4)]
 
 
+class FpnWeights(ctypes.Structure):
+    """struct mmmot_fpn_weights"""
+    _fields_ = [("lat_wt", ctypes.c_void_p * 4), ("lat_bias", ctypes.c_void_p * 4), ("lat_wp", ctypes.c_void_p * 4),
+                ("lat_wp_scale", ctypes.c_float * 4), ("last_wt", ctypes.c_void_p), ("last_bias", ctypes.c_void_p)]
+
+
 class MmmotError(RuntimeError):
     pass
 
@@ -57,6 +63,7 @@ class MmmotError(RuntimeError):
 _vp, _i, _l, _f, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_long, ctypes.c_float, ctypes.c_size_t
 _wp = ctypes.POINTER(Weights)
 _rwp = ctypes.POINTER(ResnetWeights)
+_fwp = ctypes.POINTER(FpnWeights)
 
 # name -> (restype, argtypes); every symbol the header declares
 SIGNATURES = {
@@ -97,6 +104,9 @@ SIGNATURES = {
     "mmmot_appearance_resnet_workspace": (_sz, [_i, _i, _i]),
     "mmmot_appearance_resnet_fwd": (_i, [_wp, _rwp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "mmmot_debug_resnet_op": (_i, [_i, _rwp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mmmot_appearance_resnet_fpn_workspace": (_sz, [_i, _i, _i, _i]),
+    "mmmot_appearance_resnet_fpn_fwd": (_i, [_rwp, _fwp, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "mmmot_debug_fpn_op": (_i, [_i, _fwp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "mmmot_appearance_train_workspace": (_sz, [_i, _i, _i]),
     "mmmot_appearance_train_fwd": (_i, [_wp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "mmmot_pointnet_train_workspace": (_sz, [_i, _i, _l]),

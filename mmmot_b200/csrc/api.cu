@@ -92,7 +92,7 @@ const char* const kTagNames[MM_T_COUNT] = {
     "affinity.l1_pair_512to1024", "affinity.newend_means", "affinity.l2_512to512", "affinity.l3_512to128",
     "affinity.logit", "lp.assign", "pointnet.moments_128", "pointnet.moments_64",
     "pointnet.moments_finalize", "lp.flow", "resnet.stem", "resnet.maxpool", "resnet.conv1x1", "resnet.conv3x3",
-    "resnet.stride2", "resnet.residual", "resnet.mean_heads"};
+    "resnet.stride2", "resnet.residual", "resnet.mean_heads", "fpn.lateral", "fpn.head"};
 }  // namespace
 
 bool mm_timing_on() { return g_timing; }

@@ -52,7 +52,9 @@ enum {
   MM_T_RES_S2 = 37,       // stride-2 convs: their gather + contraction (conv2 and downsample of block 0, layer2..4)
   MM_T_RES_ADD = 38,      // residual add + ReLU
   MM_T_RES_HEADS = 39,    // SkipPool plane means + heads
-  MM_T_COUNT = 40
+  MM_T_FPN_LAT = 40,      // FPN laterals: contraction + per-image means (tables, segment sums or the FP32 map)
+  MM_T_FPN_HEAD = 41,     // FPN head: level sum + conv_last
+  MM_T_COUNT = 42
 };
 bool mm_timing_on();
 void mm_timing_begin(cudaStream_t st, int tag, double flop, double bytes);

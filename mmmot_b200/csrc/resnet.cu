@@ -277,6 +277,54 @@ int launch_heads(const mmmot_resnet_weights* rw, float* const* pooled, int n_img
   return 0;
 }
 
+// ---- FPN head (reference appear_net.py:83-104,192-210; DESIGN.md §5.1, "FPN head") ----
+// H and W are multiples of 32, so every top-down interpolate is an exact 2x bilinear upsample, which preserves the
+// spatial mean: avgpool(out) = sum over the four levels of the mean of their ReLU'd laterals.  The laterals are
+// therefore only ever reduced to per-image channel means; no 512-channel map exists.
+
+// Tables of one level's lateral on the tensor cores (h x w pixels per image, L images per pair): seg[pix] = image of
+// pixel pix; tiles: per pair, ceil(L*hw / 256) column tiles {pair, first pixel, length} that start at the pair's first
+// pixel, so how a pair's pixels fall into 32-column chunks does not depend on the pair's place in the batch; sc / sh
+// [pairs][512] = 1 / 0 (the epilogue's per-group affine).  One thread per item of the largest of the three.
+__global__ void fpn_tables_kernel(int n_img, int hw, int L, int tpp, int* __restrict__ seg, int4* __restrict__ tiles,
+                                  float* __restrict__ sc, float* __restrict__ sh) {
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int pairs = n_img / L;
+  const long per_pair = (long)L * hw;
+  if (idx < (long)n_img * hw) seg[idx] = (int)(idx / hw);
+  if (idx < (long)pairs * tpp) {
+    const int pair = (int)(idx / tpp), j = (int)(idx - (long)pair * tpp);
+    const long c0 = pair * per_pair + (long)j * tc::BN;
+    tiles[idx] = make_int4(pair, (int)c0, (int)min((long)tc::BN, per_pair - (long)j * tc::BN), 0);
+  }
+  if (idx < (long)pairs * 512) { sc[idx] = 1.f; sh[idx] = 0.f; }
+}
+
+// means[img][c] = segsum[img][c] * 2^-32 / hw
+__global__ void fpn_segsum_mean_kernel(const unsigned long long* __restrict__ segsum, long n, int hw,
+                                       float* __restrict__ means) {
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx < n) means[idx] = (float)((double)segsum[idx] * (1.0 / 4294967296.0) / (double)hw);
+}
+
+// One CTA (512 threads) per image: v = sum of the four level means [4][n_img][512], then ReLU(W_last v + b_last) with
+// conv_last.2 (BatchNorm) folded into conv_last.1 -> stack 0 of feats.  On the tensor cores the level means come from
+// 2^-32 fixed-point sums (fpn_segsum_mean_kernel): each per-(image, channel) sum of ReLU'd lateral values must stay
+// below 2^32 (at 224 x 224, an average lateral value below 1.3e6 on level 0).
+__global__ void __launch_bounds__(512) fpn_head_kernel(const float* __restrict__ means, int n_img,
+                                                       const float* __restrict__ wt, const float* __restrict__ bias,
+                                                       int L, float* __restrict__ feats) {
+  __shared__ float v[512];
+  const int img = blockIdx.x, t = threadIdx.x;
+  const long lv = (long)n_img * 512, o = (long)img * 512 + t;
+  v[t] = ((means[o] + means[lv + o]) + means[2 * lv + o]) + means[3 * lv + o];
+  __syncthreads();
+  float a = bias[t];
+  for (int c = 0; c < 512; c++) a = fmaf(wt[c * 512 + t], v[c], a);
+  const int pair = img / L, l = img - pair * L;
+  feats[(((long)pair * 3 + 0) * 512 + t) * L + l] = fmaxf(a, 0.f);
+}
+
 // ---- the trunk ----
 
 int total_convs(const int* blocks) { return 1 + 3 * (blocks[0] + blocks[1] + blocks[2] + blocks[3]) + 4; }
@@ -316,6 +364,31 @@ ResWs carve_resnet(MmArena& a, int n_img, int H, int W) {
   w.kseg = a.take<float>(kseg_floats(n_img, H, W));
   for (int s = 0; s < 4; s++) w.pooled[s] = a.take<float>((size_t)n_img * (256 << s));
   return w;
+}
+
+// The FPN head's scratch, behind the trunk's: the level means [4][n_img][512], one level's fixed-point sums and the
+// tables of the largest level (H/4 x W/4).  The FP32 engine's laterals ([512][n*hw], at most n*H*W*32 floats) go
+// through the trunk's gather scratch.
+struct FpnWs {
+  float* means;
+  unsigned long long* segsum;
+  float *sc, *sh;
+  int* seg;
+  int4 *tiles, *ctab;
+};
+int fpn_tiles_per_pair(int L, int hw) { return mm_cdiv((long)L * hw, tc::BN); }
+FpnWs carve_fpn(MmArena& a, int n_img, int H, int W, int L) {
+  FpnWs f = {};
+  const int hw0 = (H / 4) * (W / 4), pairs = mm_cdiv(n_img, L);
+  const size_t max_tiles = (size_t)pairs * fpn_tiles_per_pair(L, hw0);
+  f.means = a.take<float>((size_t)4 * n_img * 512);
+  f.segsum = a.take<unsigned long long>((size_t)n_img * 512);
+  f.sc = a.take<float>((size_t)pairs * 512);
+  f.sh = a.take<float>((size_t)pairs * 512);
+  f.seg = a.take<int>((size_t)n_img * hw0);
+  f.tiles = a.take<int4>(max_tiles);
+  f.ctab = a.take<int4>(2 * max_tiles);
+  return f;
 }
 
 // One conv of the graph on either engine.  x / y: the engine's activation layout at (h, w) / (h/stride, w/stride).
@@ -479,45 +552,64 @@ struct Trunk {
     if (timed) mm_timing_end(st);
     return 0;
   }
+
+  // FPN lateral k of a stage output x (C channels at h x w, L images per pair): the per-image channel means of
+  // relu(fpn_in[k] conv + folded BatchNorm) -> means [n_img][512].  Tensor cores: the contraction's segment-sum
+  // epilogue (Y = nullptr: nothing stored) over per-pair column tiles; FP32 engine: the lateral map into cols, then
+  // its means.
+  int lateral(const mmmot_fpn_weights* fw, int k, const float* x, int h, int w, int C, int L, const FpnWs& f,
+              float* means) const {
+    const int hw = h * w;
+    const long n_pix = (long)n_img * hw;
+    if (timed) mm_timing_begin(st, MM_T_FPN_LAT, 2.0 * 512 * C * n_pix, 4.0 * (double)n_pix * C);
+    GemmP p = gemm_defaults();
+    p.bias = fw->lat_bias[k]; p.M = 512; p.K = C;
+    if (tc) {
+      const int pairs = n_img / L, tpp = fpn_tiles_per_pair(L, hw);
+      const long items = std::max(n_pix, (long)pairs * 512);
+      fpn_tables_kernel<<<mm_cdiv(items, 256), 256, 0, st>>>(n_img, hw, L, tpp, f.seg, f.tiles, f.sc, f.sh);
+      MM_LAUNCH_CHECK();
+      tma::seg_chunk_tab_kernel<<<mm_cdiv(pairs * tpp * 2, 128), 128, 0, st>>>(f.tiles, pairs * tpp, f.seg, f.ctab);
+      MM_LAUNCH_CHECK();
+      MM_CUDA(cudaMemsetAsync(f.segsum, 0, (size_t)n_img * 512 * sizeof(unsigned long long), st));
+      p.tile_tab = f.tiles; p.num_tiles = pairs * tpp;
+      p.seg = f.seg; p.sc = f.sc; p.sh = f.sh;
+      MM_TRY(gemm_tma_launch_mat(p, (const uint4*)fw->lat_wp[k], fw->lat_wp_scale[k], reinterpret_cast<const __half*>(x),
+                                 n_pix * C, n_pix, C, tc::OUT_CL, 0, st, f.segsum, status, f.ctab));
+      fpn_segsum_mean_kernel<<<mm_cdiv((long)n_img * 512, 256), 256, 0, st>>>(f.segsum, (long)n_img * 512, hw, means);
+    } else {
+      p.relu = 1;
+      p.Wt = fw->lat_wt[k]; p.ldw = 512;
+      p.S = (int)n_pix; p.tiles_per_group = mm_cdiv(n_pix, 128); p.num_tiles = p.tiles_per_group;
+      p.X = x; p.x_ks = n_pix;
+      p.Y = cols; p.y_ms = n_pix;
+      MM_TRY(mm_simt_direct(p, st));
+      mean_cm_f32_kernel<<<mm_cdiv((long)n_img * 512 * 32, 256), 256, 0, st>>>(cols, n_img, hw, 512, means);
+    }
+    MM_LAUNCH_CHECK();
+    if (timed) mm_timing_end(st);
+    return 0;
+  }
 };
 
-}  // namespace
-
-extern "C" size_t mmmot_appearance_resnet_workspace(int n_img, int H, int W) {
-  if (n_img <= 0 || H <= 0 || W <= 0) return 0;
-  MmArena a(nullptr, 0);
-  carve_resnet(a, n_img, H, W);
-  return a.off;
-}
-
-extern "C" int mmmot_appearance_resnet_fwd(const mmmot_weights* wts, const mmmot_resnet_weights* rw, const float* crops,
-                                           int n_img, int H, int W, int L, float* feats, void* workspace,
-                                           size_t workspace_bytes, void* stream) {
-  (void)wts;
-  if (!rw || !crops || !feats || !workspace || n_img <= 0 || L <= 0) return MMMOT_E_ARG;
-  for (int s = 0; s < 4; s++)
-    if (rw->blocks[s] < 1 || rw->blocks[s] > MMMOT_RESNET_MAX_CONVS) return MMMOT_E_ARG;
-  if (total_convs(rw->blocks) > MMMOT_RESNET_MAX_CONVS) return MMMOT_E_ARG;
-  if (H <= 0 || W <= 0 || H % 32 || W % 32 || n_img % L) return MMMOT_E_SHAPE;
-  if ((long)n_img * (H / 2) * (W / 2) >= (1L << 31)) return MMMOT_E_SHAPE;
-  const int nconv = total_convs(rw->blocks);
-  for (int i = 0; i < nconv; i++)
-    if (!rw->wt[i] || !rw->bias[i] || !rw->wp[i]) return MMMOT_E_ARG;
-  for (int s = 0; s < 4; s++)
-    for (int j = 0; j < 10; j++)
-      if (!rw->head[s][j]) return MMMOT_E_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  MmArena ar(workspace, workspace_bytes);
-  ResWs ws = carve_resnet(ar, n_img, H, W);
-  if (!ar.ok()) return MMMOT_E_WORKSPACE;
-
+// Trunk setup shared by the entry points: the engine (per-pair shapes only, never the batch size, as in
+// mmmot_appearance_fwd) and the scratch of a carved workspace.
+Trunk make_trunk(const mmmot_resnet_weights* rw, int n_img, int H, int W, int L, const ResWs& ws, int* status,
+                 cudaStream_t st) {
   Trunk t;
   t.rw = rw; t.n_img = n_img;
-  // engine choice depends on per-pair shapes only (never on the batch size), as in mmmot_appearance_fwd
   t.tc = mm_engine() == 2 || (mm_engine() == 0 && (long)L * H * W >= 32768);
   t.timed = mm_timing_on();
-  t.cols = ws.cols; t.kseg = ws.kseg; t.status = ar.status(); t.st = st;
+  t.cols = ws.cols; t.kseg = ws.kseg; t.status = status; t.st = st;
+  return t;
+}
 
+// The trunk on the fp32 NCHW crops: stem, max-pool, layer1..layer4.  on_stage(s, x, h, w, C) runs on the output of
+// layer s+1 (C = 256 << s channels at h x w, in the engine's layout) while it is live.
+template <class OnStage>
+int run_trunk(const Trunk& t, const float* crops, int H, int W, const ResWs& ws, OnStage on_stage) {
+  const mmmot_resnet_weights* rw = t.rw;
+  const int n_img = t.n_img;
   // buffers: x (block input), t1 (conv1), t2 (conv2), y (conv3, then the block output), d (downsample)
   float *x = ws.act[0], *t1 = ws.act[1], *t2 = ws.act[2], *y = ws.act[3], *d = ws.act[4];
   MM_TRY(t.stem(crops, H, W, y));
@@ -543,12 +635,123 @@ extern "C" int mmmot_appearance_resnet_fwd(const mmmot_weights* wts, const mmmot
       std::swap(x, y);
       h = ho; w = wo; cin = cout;
     }
-    MM_TRY(t.mean(x, h, w, cout, ws.pooled[s]));
+    MM_TRY(on_stage(s, x, h, w, cout));
   }
+  return 0;
+}
+
+// The trunk's arguments, checked before any CUDA call: the block counts, the shapes, every conv's pointers.
+int check_trunk(const mmmot_resnet_weights* rw, int n_img, int H, int W, int L) {
+  for (int s = 0; s < 4; s++)
+    if (rw->blocks[s] < 1 || rw->blocks[s] > MMMOT_RESNET_MAX_CONVS) return MMMOT_E_ARG;
+  if (total_convs(rw->blocks) > MMMOT_RESNET_MAX_CONVS) return MMMOT_E_ARG;
+  if (H <= 0 || W <= 0 || H % 32 || W % 32 || n_img % L) return MMMOT_E_SHAPE;
+  if ((long)n_img * (H / 2) * (W / 2) >= (1L << 31)) return MMMOT_E_SHAPE;
+  const int nconv = total_convs(rw->blocks);
+  for (int i = 0; i < nconv; i++)
+    if (!rw->wt[i] || !rw->bias[i] || !rw->wp[i]) return MMMOT_E_ARG;
+  return 0;
+}
+
+constexpr int kFpnMaxTcBlocks3 = 23;   // layer3 blocks of ResNet-101: the deepest FPN trunk run on the tensor cores
+
+bool fpn_weights_ok(const mmmot_fpn_weights* fw) {
+  if (!fw || !fw->last_wt || !fw->last_bias) return false;
+  for (int k = 0; k < 4; k++)
+    if (!fw->lat_wt[k] || !fw->lat_bias[k] || !fw->lat_wp[k]) return false;
+  return true;
+}
+
+int launch_fpn_head(const mmmot_fpn_weights* fw, const float* means, int n_img, int L, float* feats, bool timed,
+                    cudaStream_t st) {
+  if (timed) mm_timing_begin(st, MM_T_FPN_HEAD, 2.0 * 512 * 512 * n_img, 4.0 * (512.0 * 512 + 4.0 * 512 * n_img));
+  fpn_head_kernel<<<n_img, 512, 0, st>>>(means, n_img, fw->last_wt, fw->last_bias, L, feats);
+  MM_LAUNCH_CHECK();
+  if (timed) mm_timing_end(st);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" size_t mmmot_appearance_resnet_workspace(int n_img, int H, int W) {
+  if (n_img <= 0 || H <= 0 || W <= 0) return 0;
+  MmArena a(nullptr, 0);
+  carve_resnet(a, n_img, H, W);
+  return a.off;
+}
+
+extern "C" int mmmot_appearance_resnet_fwd(const mmmot_weights* wts, const mmmot_resnet_weights* rw, const float* crops,
+                                           int n_img, int H, int W, int L, float* feats, void* workspace,
+                                           size_t workspace_bytes, void* stream) {
+  (void)wts;
+  if (!rw || !crops || !feats || !workspace || n_img <= 0 || L <= 0) return MMMOT_E_ARG;
+  MM_TRY(check_trunk(rw, n_img, H, W, L));
+  for (int s = 0; s < 4; s++)
+    for (int j = 0; j < 10; j++)
+      if (!rw->head[s][j]) return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  MmArena ar(workspace, workspace_bytes);
+  ResWs ws = carve_resnet(ar, n_img, H, W);
+  if (!ar.ok()) return MMMOT_E_WORKSPACE;
+
+  const Trunk t = make_trunk(rw, n_img, H, W, L, ws, ar.status(), st);
+  MM_TRY(run_trunk(t, crops, H, W, ws, [&](int s, const float* x, int h, int w, int C) {
+    return t.mean(x, h, w, C, ws.pooled[s]);
+  }));
   if (t.timed) mm_timing_begin(st, MM_T_RES_HEADS, 0.0, 0.0);
   MM_TRY(launch_heads(rw, ws.pooled, n_img, L, feats, st));
   if (t.timed) mm_timing_end(st);
   return 0;
+}
+
+extern "C" size_t mmmot_appearance_resnet_fpn_workspace(int n_img, int H, int W, int L) {
+  if (n_img <= 0 || H <= 0 || W <= 0 || L <= 0) return 0;
+  MmArena a(nullptr, 0);
+  carve_resnet(a, n_img, H, W);
+  carve_fpn(a, n_img, H, W, L);
+  return a.off;
+}
+
+extern "C" int mmmot_appearance_resnet_fpn_fwd(const mmmot_resnet_weights* rw, const mmmot_fpn_weights* fw,
+                                               const float* crops, int n_img, int H, int W, int L, float* feats,
+                                               void* workspace, size_t workspace_bytes, void* stream) {
+  if (!rw || !crops || !feats || !workspace || n_img <= 0 || L <= 0) return MMMOT_E_ARG;
+  MM_TRY(check_trunk(rw, n_img, H, W, L));
+  if (!fpn_weights_ok(fw)) return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  MmArena ar(workspace, workspace_bytes);
+  ResWs ws = carve_resnet(ar, n_img, H, W);
+  FpnWs f = carve_fpn(ar, n_img, H, W, L);
+  if (!ar.ok()) return MMMOT_E_WORKSPACE;
+
+  Trunk t = make_trunk(rw, n_img, H, W, L, ws, ar.status(), st);
+  // No GroupNorm follows this head, so the trunk's tensor-core error reaches the features undamped: the contractions'
+  // accumulation bias adds up block by block, and at ResNet-152's 36 layer3 blocks it takes the link scores past 1e-4
+  // (DESIGN.md §5.1, "FPN head").  Trunks deeper than ResNet-101 run on the FP32 engine in every engine mode.
+  if (rw->blocks[2] > kFpnMaxTcBlocks3) t.tc = false;
+  MM_TRY(run_trunk(t, crops, H, W, ws, [&](int s, const float* x, int h, int w, int C) {
+    return t.lateral(fw, s, x, h, w, C, L, f, f.means + (long)s * n_img * 512);
+  }));
+  return launch_fpn_head(fw, f.means, n_img, L, feats, t.timed, st);
+}
+
+// Test hook of the FPN head, through the code mmmot_appearance_resnet_fpn_fwd runs.  See include/mmmot_b200.h.
+extern "C" int mmmot_debug_fpn_op(int op, const mmmot_fpn_weights* fw, int level, int n_img, int h, int w, int L,
+                                  const void* X, float* Y, void* workspace, size_t workspace_bytes, void* stream) {
+  if (op < 0 || op > 1 || !fpn_weights_ok(fw) || !X || !Y || n_img <= 0 || L <= 0 || n_img % L) return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (op == 1) return launch_fpn_head(fw, (const float*)X, n_img, L, Y, false, st);
+  if (level < 0 || level > 3 || h <= 0 || w <= 0 || !workspace) return MMMOT_E_ARG;
+  const int H = h << (level + 2), W = w << (level + 2);
+  if ((long)n_img * (H / 2) * (W / 2) >= (1L << 31)) return MMMOT_E_SHAPE;
+  MmArena ar(workspace, workspace_bytes);
+  ResWs ws = carve_resnet(ar, n_img, H, W);
+  FpnWs f = carve_fpn(ar, n_img, H, W, L);
+  if (!ar.ok()) return MMMOT_E_WORKSPACE;
+  Trunk t = make_trunk(nullptr, n_img, H, W, L, ws, ar.status(), st);
+  t.tc = mm_engine() != 1;
+  t.timed = false;
+  return t.lateral(fw, level, (const float*)X, h, w, 256 << level, L, f, Y);
 }
 
 // Test hook: one launch kind of the ResNet trunk through the Trunk members mmmot_appearance_resnet_fwd calls, on the

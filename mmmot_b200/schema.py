@@ -104,10 +104,27 @@ def _stn(sd, p, cin, k):
     sd[f"{p}.output.bias"] = ((k * k,), "stn_out")
 
 
-def state_schema(fusion="C", point_in=3, appear_arch="vgg"):
+def _fpn(sd):
+    """The FPN head (reference modules/appear_net.py:83-104): per ResNet stage a bias-free 1x1 lateral C -> 512 and its
+    BatchNorm2d (fpn_in.k.0 / .1), then conv_last.1 (1x1, 512 -> 512, with bias) and its BatchNorm2d conv_last.2."""
+    for k, c in enumerate(RES_SKIP_CHANNELS):
+        sd[f"appearance.fpn_in.{k}.0.weight"] = ((D, c, 1, 1), "conv")
+        _bn(sd, f"appearance.fpn_in.{k}.1", D)
+    sd["appearance.conv_last.1.weight"] = ((D, D, 1, 1), "conv")
+    sd["appearance.conv_last.1.bias"] = ((D,), "bias")
+    _bn(sd, "appearance.conv_last.2", D)
+
+
+APPEAR_HEADS = ("skippool", "fpn")
+
+
+def state_schema(fusion="C", point_in=3, appear_arch="vgg", appear_head="skippool"):
     """OrderedDict key -> (shape, kind).  ``kind`` drives init / synthetic generation:
     conv, bias, norm_w, res_norm_w, norm_b, run_mean, run_var, nbt, eye, stn_out.
-    appear_arch: "vgg" (VGG16-BN) or a key of RESNET_BLOCKS."""
+    appear_arch: "vgg" (VGG16-BN) or a key of RESNET_BLOCKS; appear_head: "skippool" (four SkipPool heads,
+    appear_skippool) or "fpn" (the FPN head, appear_fpn; ResNet trunks only)."""
+    if appear_head not in APPEAR_HEADS or (appear_head == "fpn" and appear_arch == "vgg"):
+        raise ValueError(f"unsupported appearance head {appear_head!r} on {appear_arch!r}")
     sd = OrderedDict()
     # --- fusion_module (modules/fusion_net.py) ---
     f = "fusion_module"
@@ -132,7 +149,9 @@ def state_schema(fusion="C", point_in=3, appear_arch="vgg"):
         _resnet(sd, appear_arch)
     else:
         raise ValueError(f"unknown appearance arch {appear_arch!r}")
-    for s, c in enumerate(SKIP_CHANNELS if appear_arch == "vgg" else RES_SKIP_CHANNELS):
+    if appear_head == "fpn":
+        _fpn(sd)
+    for s, c in enumerate(() if appear_head == "fpn" else SKIP_CHANNELS if appear_arch == "vgg" else RES_SKIP_CHANNELS):
         p = f"appearance.global_pool.{s}.fc"
         m = skip_mid(c)
         sd[f"{p}.0.weight"] = ((c,), "norm_w")

@@ -79,8 +79,9 @@ class TrackingNet(nn.Module):
         # rejected loudly instead of silently computing something different
         unsupported = []
         if appear_len != 512 or point_len != 512: unsupported.append("appear_len/point_len != 512")
-        if appear_arch not in ('vgg',) + tuple(RESNET_BLOCKS) or not appear_skippool or appear_fpn:
-            unsupported.append("appearance must be vgg, resnet50, resnet101 or resnet152 + skippool")
+        if appear_arch not in ('vgg',) + tuple(RESNET_BLOCKS) or bool(appear_skippool) == bool(appear_fpn) or \
+                (appear_fpn and appear_arch == 'vgg'):
+            unsupported.append("appearance must be vgg + skippool, or resnet50, resnet101 or resnet152 + skippool or fpn")
         if point_arch != 'v1': unsupported.append("point_arch must be v1")
         if end_arch != 'v2' or end_mode not in _lib.END_MODE: unsupported.append("end_arch must be v2, end_mode avg or max")
         if score_arch not in ('branch_cls', 'branch_reg'): unsupported.append("score_arch must be branch_cls/branch_reg")
@@ -97,12 +98,14 @@ class TrackingNet(nn.Module):
         self.end_mode = end_mode
         self.score_fusion_arch = score_fusion_arch
         self.appear_arch = appear_arch
+        self.appear_head = "fpn" if appear_fpn else "skippool"
         # dropblock / use_dropout are identity in eval mode; accepted for config compatibility
         self.dropblock, self.use_dropout = dropblock, use_dropout
         # PointNet's input width (tracking_net.py:41): xyz, or xyz + LiDAR reflectance
         self.point_channels = 4 - int(bool(without_reflectivity))
         gen = torch.Generator().manual_seed(0)
-        for key, (shape, kind) in state_schema(score_fusion_arch, self.point_channels, appear_arch).items():
+        for key, (shape, kind) in state_schema(score_fusion_arch, self.point_channels, appear_arch,
+                                                self.appear_head).items():
             _register(self, key, _default_init(shape, kind, gen), kind in BUFFER_KINDS)
         for name, prm in self.named_parameters():
             if name.endswith(".idt"):           # reference point_net.py:62: requires_grad=False
@@ -129,7 +132,8 @@ class TrackingNet(nn.Module):
                                   "(there is no CPU fallback)")
         if self._prepared is None or self._prepared.flat.device != dev:
             _lib.load()
-            self._prepared = DeviceWeights(self.state_dict(), self.score_fusion_arch, dev, self.appear_arch)
+            self._prepared = DeviceWeights(self.state_dict(), self.score_fusion_arch, dev, self.appear_arch,
+                                           self.appear_head)
         return self._prepared
 
     def _split_to_device(self, s_host, dev):
@@ -177,8 +181,13 @@ class TrackingNet(nn.Module):
                 need += [lib.mmmot_appearance_train_workspace(pairs * L, H, W), lib.mmmot_pointnet_train_workspace(pairs, L, P),
                          lib.mmmot_w_det_train_workspace(L)]
             else:
-                app = (lib.mmmot_appearance_workspace if self.appear_arch == "vgg" else lib.mmmot_appearance_resnet_workspace)
-                need += [app(pairs * L, H, W), lib.mmmot_pointnet_workspace(pairs, L, P)]
+                if self.appear_arch == "vgg":
+                    app = lib.mmmot_appearance_workspace(pairs * L, H, W)
+                elif self.appear_head == "fpn":
+                    app = lib.mmmot_appearance_resnet_fpn_workspace(pairs * L, H, W, L)
+                else:
+                    app = lib.mmmot_appearance_resnet_workspace(pairs * L, H, W)
+                need += [app, lib.mmmot_pointnet_workspace(pairs, L, P)]
             need.append(lib.mmmot_fusion_det_workspace(pairs, L))
         return max(need)
 
@@ -209,6 +218,9 @@ class TrackingNet(nn.Module):
             bn_det = torch.zeros(2, 2, 512, device=dev)
             _lib.check(lib.mmmot_appearance_train_fwd(wts.ptr, _vp(crops), pairs * L, H, W, L, _vp(feats), _vp(bn_vgg), _vp(dm2),
                                                       _vp(dm3), wsp, wsn, st), "mmmot_appearance_train_fwd")
+        elif wts.fpn is not None:
+            _lib.check(lib.mmmot_appearance_resnet_fpn_fwd(wts.rptr, wts.fptr, _vp(crops), pairs * L, H, W, L, _vp(feats), wsp,
+                                                           wsn, st), "mmmot_appearance_resnet_fpn_fwd")
         elif wts.resnet is not None:
             _lib.check(lib.mmmot_appearance_resnet_fwd(wts.ptr, wts.rptr, _vp(crops), pairs * L, H, W, L, _vp(feats), wsp, wsn,
                                                        st), "mmmot_appearance_resnet_fwd")

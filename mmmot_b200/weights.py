@@ -98,21 +98,41 @@ def fold_bn_nobias(sd, conv, bn):
     return w * s.reshape(-1, 1, 1, 1), sd[f"{bn}.bias"].double() - sd[f"{bn}.running_mean"].double() * s
 
 
-def prepare_resnet(state_dict, arch):
-    """ResNet appearance trunk -> (convs, heads): convs in execution order (schema.resnet_convs), each (Wt [K][Cout] fp32,
-    bias [Cout] fp32, packed tiles uint8, out_scale) with every BatchNorm folded and the K order of
-    mmmot_resnet_weights (1x1: ci; 3x3: (ky*3+kx)*Cin + ci; stem: (ky*7+kx)*3 + ci, packed K zero-padded 147 -> 160);
-    heads: the 40 fp32 tensors of the four SkipPool heads, head s at [10 s, 10 s + 10)."""
-    sd = {k: v.detach().cpu() for k, v in state_dict.items()}
+def _resnet_trunk(sd, arch):
     convs = []
     for conv, bn, cin, cout, k, _ in resnet_convs(arch):
         w, b = fold_bn_nobias(sd, conv, bn)
         wt = w.permute(2, 3, 1, 0).reshape(k * k * cin, cout)       # [co][ci][ky][kx] -> [(ky*k+kx)*cin + ci][co]
         packed, scale = pack_tc(wt)
         convs.append((wt.contiguous().float(), b.float(), packed, scale))
+    return convs
+
+
+def prepare_resnet(state_dict, arch):
+    """ResNet appearance trunk -> (convs, heads): convs in execution order (schema.resnet_convs), each (Wt [K][Cout] fp32,
+    bias [Cout] fp32, packed tiles uint8, out_scale) with every BatchNorm folded and the K order of
+    mmmot_resnet_weights (1x1: ci; 3x3: (ky*3+kx)*Cin + ci; stem: (ky*7+kx)*3 + ci, packed K zero-padded 147 -> 160);
+    heads: the 40 fp32 tensors of the four SkipPool heads, head s at [10 s, 10 s + 10)."""
+    sd = {k: v.detach().cpu() for k, v in state_dict.items()}
+    convs = _resnet_trunk(sd, arch)
     heads = [None] * 40
     _skip_heads(sd, heads, RES_SKIP_CHANNELS)
     return convs, [t.contiguous().float() for t in heads]
+
+
+def prepare_fpn(state_dict):
+    """The FPN head (mmmot_fpn_weights) -> (laterals, last): laterals[k] = (Wt [C_k][512] fp32, bias [512] fp32, packed
+    tiles uint8, out_scale) of fpn_in[k] with its BatchNorm folded (C_k = 256 << k); last = (Wt [512][512] fp32,
+    bias [512] fp32) of conv_last.1 with conv_last.2 folded."""
+    sd = {k: v.detach().cpu() for k, v in state_dict.items()}
+    lats = []
+    for k, c in enumerate(RES_SKIP_CHANNELS):
+        w, b = fold_bn_nobias(sd, f"appearance.fpn_in.{k}.0", f"appearance.fpn_in.{k}.1")
+        wt = w.reshape(-1, c).t()
+        packed, scale = pack_tc(wt)
+        lats.append((wt.contiguous().float(), b.float(), packed, scale))
+    w, b = _fold_bn(sd, "appearance.conv_last.1", "appearance.conv_last.2")
+    return lats, (w.reshape(w.shape[0], -1).t().contiguous().float(), b.float())
 
 
 def prepare(state_dict, fusion, appear_arch="vgg"):
@@ -255,13 +275,18 @@ class DeviceWeights:
     """All prepared tensors in ONE flat device buffer (256-byte aligned slices) + the pointer table
     handed to the C ABI."""
 
-    def __init__(self, state_dict, fusion, device, appear_arch="vgg"):
+    def __init__(self, state_dict, fusion, device, appear_arch="vgg", appear_head="skippool"):
         tensors, self.trans1, self.trans2, scales = prepare(state_dict, fusion, appear_arch)
         nmain = len(tensors)
-        self.resnet = None
+        self.resnet = self.fpn = None
         if appear_arch != "vgg":
-            # the ResNet trunk's operands ride in the same flat buffer, behind the weight-id table's tensors
-            convs, heads = prepare_resnet(state_dict, appear_arch)
+            # the ResNet trunk's operands (and its head's) ride in the same flat buffer, behind the weight-id table's
+            if appear_head == "fpn":
+                convs = _resnet_trunk({k: v.detach().cpu() for k, v in state_dict.items()}, appear_arch)
+                lats, last = prepare_fpn(state_dict)
+                heads = [t for c in lats for t in (c[0], c[1], c[2].view(torch.float32))] + list(last)
+            else:
+                convs, heads = prepare_resnet(state_dict, appear_arch)
             tensors = tensors + [t for c in convs for t in (c[0], c[1], c[2].view(torch.float32))] + heads
         offs, total = [], 0
         for t in tensors:
@@ -286,9 +311,17 @@ class DeviceWeights:
                 r.wt[i], r.bias[i], r.wp[i] = (base + 4 * x for x in o)
                 r.wp_scale[i] = c[3]
             ho = offs[nmain + 3 * len(convs):]
-            for s in range(4):
-                for j in range(10):
-                    r.head[s][j] = base + 4 * ho[10 * s + j]
+            if appear_head == "fpn":
+                f = self.fpn = _lib.FpnWeights()
+                for k in range(4):
+                    f.lat_wt[k], f.lat_bias[k], f.lat_wp[k] = (base + 4 * x for x in ho[3 * k:3 * k + 3])
+                    f.lat_wp_scale[k] = lats[k][3]
+                f.last_wt, f.last_bias = base + 4 * ho[12], base + 4 * ho[13]
+                self.fptr = ctypes.pointer(f)
+            else:
+                for s in range(4):
+                    for j in range(10):
+                        r.head[s][j] = base + 4 * ho[10 * s + j]
             self.rptr = ctypes.pointer(r)
         self.table.point_channels = int(state_dict["point_net.feat.conv1.weight"].shape[1])
         self.ptr = ctypes.pointer(self.table)
