@@ -451,7 +451,8 @@ int mmmot_set_kseg(int chunks);
  *   bit 12 (4096) generated-operand engine: GEN_NORM producers with the software pipeline (prefetching variant)
  *                 instead of TMA-staged source rows
  *   bit 13 (8192) PointNet layers 3, 4 through norm_split + the TMA-fed kernel instead of GEN_NORM producers
- *   bit 14 (16384) first VGG layer with a separate im2col pre-pass instead of in-kernel operand producers */
+ *   bit 14 (16384) first VGG layer with a separate im2col pre-pass instead of in-kernel operand producers
+ *   bit 15 (32768) first VGG block as two launches (layer 0, then layer 1 + pool) instead of the fused kernel */
 int mmmot_set_debug(int flags);
 
 /* Test hook: one launch of the FP32 FFMA engine in any operand mode, with its GroupNorm partials (device pointers).
@@ -546,7 +547,15 @@ int mmmot_debug_linear_planar(const void* Wp, float wp_scale, const float* bias,
  * vgg_conv0: the first VGG layer, fp32 NCHW crops [n][3][H][W] -> Y[2][n][H][W][64] (y_plane apart), bias + ReLU.
  *   wt [27][64] fp32 (k = (ky*3+kx)*3 + ci, debug bit 5), Wp / Wpx packed tiles with k = ci*9 + ky*3 + kx, cols
  *   [2][n*H*W][32] FP16 scratch of the im2col variant.  variant (host, or NULL) receives 0 = taps generated in the
- *   contraction kernel, 1 = im2col + matrix contraction, 2 = FP32 FFMA. */
+ *   contraction kernel, 1 = im2col + matrix contraction, 2 = FP32 FFMA.
+ * vgg_conv01: the first VGG block (layers 0 and 1, bias + ReLU, then the 2x2 max-pool) as mmmot_appearance_fwd runs it,
+ *   crops [n][3][H][W] (H, W even) -> the pooled map, two FP16 planes [n][H/2][W/2][64] n*H/2*W/2*64 elements apart, in
+ *   buf0 or buf1 (*out, host, receives 0 or 1).  buf0, buf1: FP16 buffers of 2*n*H*W*64 elements each (the two-launch
+ *   path's full-resolution maps; the fused launch writes buf1 only).  Layer 0's weights as vgg_conv0, layer 1's as
+ *   conv_layer (Wp1, its compact tiles Wpx1); kseg_scratch as conv_layer.  fused (host, or NULL) receives 1 if the single
+ *   fused launch ran (it needs both compact tiles; debug bit 15 forces the two launches), 0 for the two launches.
+ * vgg_conv01_plan: *fused (host) = whether vgg_conv01 of that shape takes the fused launch (given both compact tiles),
+ *   computed on the host without any CUDA call under the current mmmot_set_debug / mmmot_set_kseg state. */
 int mmmot_debug_conv_plan(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg, int* plan);
 int mmmot_debug_conv_layer(const void* Wp, const void* Wpx, float wp_scale, const float* bias, const void* Xhi, long x_plane,
                            int n_img, int H, int W, int C, int M, void* Yhi, long y_plane, long y_plane_pooled,
@@ -555,6 +564,11 @@ int mmmot_debug_conv_layer(const void* Wp, const void* Wpx, float wp_scale, cons
 int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W, const float* wt, const float* bias, const void* Wp,
                           float wp_scale, const void* Wpx, void* Yhi, long y_plane, void* cols, int* status, int* variant,
                           void* stream);
+int mmmot_debug_vgg_conv01(const float* crops, int n_img, int H, int W, const float* wt0, const float* bias0, const void* Wp0,
+                           float wp_scale0, const void* Wpx0, const float* bias1, const void* Wp1, float wp_scale1,
+                           const void* Wpx1, void* buf0, void* buf1, float* kseg_scratch, int* status, int* out, int* fused,
+                           void* stream);
+int mmmot_debug_vgg_conv01_plan(int n_img, int H, int W, int* fused);
 
 /* Test hooks of the kernels between the contractions.
  * stage_layout: where one run of a stage leaves its intermediates in the caller's workspace, computed on the host without

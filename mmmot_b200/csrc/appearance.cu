@@ -7,6 +7,7 @@
 
 #include "gemm_tma.cuh"
 #include "norm_ops.cuh"
+#include "vgg_conv01.cuh"
 
 namespace {
 
@@ -317,6 +318,49 @@ static int vgg_conv0_launch(const float* crops, int n_img, int H, int W, const f
   return 0;
 }
 
+// The first VGG block (layers 0 and 1, then the 2x2 max-pool) of the tensor-core trunk on the two activation buffers
+// hb[0], hb[1] (each two planes of n_img*H*W*64 FP16 elements).  Where vgg_conv01_fused allows it, one launch
+// (vgg_conv01.cuh) writes the pooled planes into hb[1].  Otherwise two launches: layer 0 into hb[0] (im2col scratch in
+// hb[1]), layer 1 into hb[1] with the pool fused into its epilogue, or full-resolution into hb[1] and max-pooled into
+// hb[0].  *out receives the buffer holding the pooled planes (n_img*H/2*W/2*64 elements apart), *fused (or NULL) 1 for
+// the single launch.  timed: every launch tagged as the trunk's other layers are (the fused one as conv 1).
+static int vgg_block01_launch(const float* crops, int n_img, int H, int W, const float* wt0, const float* bias0,
+                              const uint4* Wp0, float scale0, const uint4* Wpx0, const float* bias1, const uint4* Wp1,
+                              float scale1, const uint4* Wpx1, __half* const* hb, float* kseg_scratch, int* status,
+                              bool timed, int* out, int* fused, cudaStream_t st) {
+  const double npix = (double)n_img * H * W;
+  const long plane = (long)n_img * H * W * 64, plane_p = plane / 4;
+  const bool f = vgg_conv01_fused(n_img, H, W, Wpx0 && Wpx1, mm_debug_flags(), mm_kseg_chunks());
+  if (fused) *fused = f ? 1 : 0;
+  if (f) {
+    // algorithmic FLOPs of both layers; compulsory bytes: crops in + pooled map out at 4 B per element
+    if (timed) mm_timing_begin(st, MM_T_VGG0 + 1, 2.0 * 64 * 9.0 * (3 + 64) * npix, 4.0 * npix * (3 + 64 / 4.0));
+    MM_TRY(vgg_conv01_launch(crops, n_img, H, W, Wpx0, scale0, bias0, Wpx1, scale1, bias1, hb[1], plane_p, status, st));
+    if (timed) mm_timing_end(st);
+    *out = 1;
+    return 0;
+  }
+  if (timed) mm_timing_begin(st, MM_T_VGG0, 2.0 * 64 * 9.0 * 3 * npix, 4.0 * npix * (3 + 64));
+  MM_TRY(vgg_conv0_launch(crops, n_img, H, W, wt0, bias0, Wp0, scale0, Wpx0, hb[0], plane, hb[1], status, nullptr, st));
+  if (timed) mm_timing_end(st);
+  if (timed) mm_timing_begin(st, MM_T_VGG0 + 1, 2.0 * 64 * 9.0 * 64 * npix, 4.0 * npix * (64 + 64 / 4.0));
+  GemmP p = gemm_defaults();
+  p.bias = bias1; p.M = 64; p.relu = 1;
+  int pooled = 0;
+  MM_TRY(gemm_tma_launch_conv(p, Wp1, scale1, hb[0], plane, n_img, H, W, 64, hb[1], plane, st, kseg_scratch, plane_p,
+                              &pooled, status, nullptr, Wpx1));
+  if (timed) mm_timing_end(st);
+  if (timed) mm_timing_begin(st, MM_T_VGG_POOL, 0.0, pooled ? 12.0 * n_img * 64 : 4.0 * 6.0 * plane_p);
+  if (!pooled) {
+    const long n8 = plane_p / 8;
+    maxpool2_planar_kernel<<<mm_cdiv(n8, 256), 256, 0, st>>>(hb[1], hb[0], n8, H / 2, W / 2, 64, plane, plane_p);
+    MM_LAUNCH_CHECK();
+  }
+  if (timed) mm_timing_end(st);
+  *out = pooled ? 1 : 0;
+  return 0;
+}
+
 // What the FP32 trunk needs in training mode: the BatchNorm scratch, where the batch statistics go, and the DropBlock
 // weights of the two deepest skip maps
 struct VggTrain {
@@ -422,6 +466,26 @@ extern "C" int mmmot_debug_vgg_conv0(const float* crops, int n_img, int H, int W
                           (__half*)cols, status, variant, (cudaStream_t)stream);
 }
 
+// Test hooks: the first VGG block exactly as mmmot_appearance_fwd runs it (vgg_block01_launch), and whether it takes the
+// fused launch (host only, assuming the compact tiles are there).
+extern "C" int mmmot_debug_vgg_conv01(const float* crops, int n_img, int H, int W, const float* wt0, const float* bias0,
+                                      const void* Wp0, float wp_scale0, const void* Wpx0, const float* bias1, const void* Wp1,
+                                      float wp_scale1, const void* Wpx1, void* buf0, void* buf1, float* kseg_scratch,
+                                      int* status, int* out, int* fused, void* stream) {
+  if (!crops || !bias0 || !bias1 || !Wp1 || !buf0 || !buf1 || !out || n_img <= 0 || H <= 0 || W <= 0 || (H | W) & 1)
+    return MMMOT_E_ARG;
+  __half* const hb[2] = {(__half*)buf0, (__half*)buf1};
+  return vgg_block01_launch(crops, n_img, H, W, wt0, bias0, (const uint4*)Wp0, wp_scale0, (const uint4*)Wpx0, bias1,
+                            (const uint4*)Wp1, wp_scale1, (const uint4*)Wpx1, hb, kseg_scratch, status, false, out, fused,
+                            (cudaStream_t)stream);
+}
+
+extern "C" int mmmot_debug_vgg_conv01_plan(int n_img, int H, int W, int* fused) {
+  if (!fused || n_img <= 0 || H <= 0 || W <= 0) return MMMOT_E_ARG;
+  *fused = vgg_conv01_fused(n_img, H, W, true, mm_debug_flags(), mm_kseg_chunks()) ? 1 : 0;
+  return 0;
+}
+
 int mm_launch_skip_heads(const mmmot_weights* wts, float* const* pooled, int n_img, int L, float* feats, cudaStream_t st);
 
 // per-image channel means of a planar NHWC map [2][n_img][hw][C] (planes `plane` apart) -> pooled[n_img][C]; the ResNet
@@ -461,39 +525,39 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
   const bool tc_trunk = mm_engine() == 2 || (mm_engine() == 0 && (long)L * H * W >= 32768);
   if (tc_trunk) {
     __half* hb[2] = {reinterpret_cast<__half*>(ws.buf[0]), reinterpret_cast<__half*>(ws.buf[1])};
-    const __half* cur = nullptr;
-    long cur_plane = 0;
-    int which = 0, h = H, w = W;
     const bool timed = mm_timing_on();   // roofline hook: every launch tagged (stage, layer)
     int* status = ar.status();
-    for (int i = 0; i < 13; i++) {
+    // layers 0 and 1 and the first pool (no skip map after it)
+    int which = 0;
+    MM_TRY(vgg_block01_launch(crops, n_img, H, W, wts->w[MMMOT_W_VGG_WT0], wts->w[MMMOT_W_VGG_B0],
+                              (const uint4*)wts->w[MMMOT_W_VGG_WP0], wts->tc_scale[MMMOT_W_VGG_WP0],
+                              (const uint4*)wts->w[MMMOT_W_VGG_WPX0], wts->w[MMMOT_W_VGG_B0 + 1],
+                              (const uint4*)wts->w[MMMOT_W_VGG_WP0 + 1], wts->tc_scale[MMMOT_W_VGG_WP0 + 1],
+                              (const uint4*)wts->w[MMMOT_W_VGG_WPX0 + 1], hb, ws.kseg_scratch, status, timed, &which, nullptr,
+                              st));
+    int h = H / 2, w = W / 2;
+    const __half* cur = hb[which];
+    long cur_plane = (long)n_img * h * w * 64;
+    which ^= 1;
+    for (int i = 2; i < 13; i++) {
       const int cout = kVggCout[i], cin = kVggCin[i];
       const long plane_out = (long)n_img * h * w * cout;
       int pooled_in_epilogue = 0;
       // algorithmic FLOPs 2*Cout*9Cin*pixels; compulsory bytes: activation in + activation out at 4 B per element
-      // (the pooled map when the 2x2 max-pool is fused into the epilogue)
       if (timed) mm_timing_begin(st, MM_T_VGG0 + i, 2.0 * cout * 9.0 * cin * (double)n_img * h * w,
-                                 4.0 * (double)n_img * h * w * (cin + (i == 1 ? cout / 4.0 : cout)));
-      if (i == 0) {
-        // im2col taps (if that variant runs) in the other activation buffer, dead once the contraction has run
-        MM_TRY(vgg_conv0_launch(crops, n_img, h, w, wts->w[MMMOT_W_VGG_WT0], wts->w[MMMOT_W_VGG_B0],
-                                (const uint4*)wts->w[MMMOT_W_VGG_WP0], wts->tc_scale[MMMOT_W_VGG_WP0],
-                                (const uint4*)wts->w[MMMOT_W_VGG_WPX0], hb[which], plane_out, hb[which ^ 1], status,
-                                nullptr, st));
-      } else {
-        GemmP p = gemm_defaults();
-        p.bias = wts->w[MMMOT_W_VGG_B0 + i];
-        p.M = cout;
-        p.relu = 1;
-        // a pooled layer asks for the 2x2 max-pool to be fused into the epilogue; a skip map's global average (SkipPool)
-        // rides along as per-image fixed-point sums
-        const bool skip_layer = kPoolAfter[i] && kSkipAfter[i] >= 0;
-        if (skip_layer) MM_CUDA(cudaMemsetAsync(ws.pool_sum, 0, (size_t)n_img * cout * sizeof(unsigned long long), st));
-        MM_TRY(gemm_tma_launch_conv(p, (const uint4*)wts->w[MMMOT_W_VGG_WP0 + i], wts->tc_scale[MMMOT_W_VGG_WP0 + i], cur,
-                                    cur_plane, n_img, h, w, cin, hb[which], plane_out, st, ws.kseg_scratch,
-                                    kPoolAfter[i] ? plane_out / 4 : 0, &pooled_in_epilogue, status,
-                                    skip_layer ? ws.pool_sum : nullptr, i == 1 ? (const uint4*)wts->w[MMMOT_W_VGG_WPX0 + 1] : nullptr));
-      }
+                                 4.0 * (double)n_img * h * w * (cin + cout));
+      GemmP p = gemm_defaults();
+      p.bias = wts->w[MMMOT_W_VGG_B0 + i];
+      p.M = cout;
+      p.relu = 1;
+      // a pooled layer asks for the 2x2 max-pool to be fused into the epilogue; a skip map's global average (SkipPool)
+      // rides along as per-image fixed-point sums
+      const bool skip_layer = kPoolAfter[i] && kSkipAfter[i] >= 0;
+      if (skip_layer) MM_CUDA(cudaMemsetAsync(ws.pool_sum, 0, (size_t)n_img * cout * sizeof(unsigned long long), st));
+      MM_TRY(gemm_tma_launch_conv(p, (const uint4*)wts->w[MMMOT_W_VGG_WP0 + i], wts->tc_scale[MMMOT_W_VGG_WP0 + i], cur,
+                                  cur_plane, n_img, h, w, cin, hb[which], plane_out, st, ws.kseg_scratch,
+                                  kPoolAfter[i] ? plane_out / 4 : 0, &pooled_in_epilogue, status,
+                                  skip_layer ? ws.pool_sum : nullptr, nullptr));
       if (timed) mm_timing_end(st);
       cur = hb[which]; cur_plane = plane_out; which ^= 1;
       if (kPoolAfter[i]) {
@@ -511,7 +575,7 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
           cur = hb[which]; cur_plane = plane_p; which ^= 1;
         }
         int s = kSkipAfter[i];
-        if (s >= 0 && pooled_in_epilogue && i > 1) {
+        if (s >= 0 && pooled_in_epilogue) {
           const long nn = (long)n_img * kSkipC[s];
           pool_sum_mean_kernel<<<mm_cdiv(nn, 256), 256, 0, st>>>(ws.pool_sum, ws.pooled[s], nn, 1.0f / (float)(h * w));
           MM_LAUNCH_CHECK();
