@@ -607,9 +607,22 @@ int mmmot_debug_vgg_conv01_plan(int n_img, int H, int W, int* fused);
  *                 128 (FP32), then the end columns
  *       [29] cnt  int [2G] columns per new/end group (m new, n end)   [30] gstart  int [2G + 1] first tile per group
  *       The statistics of the first affinity layer, the second and the first new/end layer do not survive the stage.
- *     stage 1, 2 offsets:
- *       [0] f3    TC only: detection-major rows [(pair*L + l)*3 + stack][512]
+ *     stage 1, 13 offsets (f3 and h2 first, then carve order; the fusion buffers are per pair and channel-last on TC,
+ *     [pair*L + l][512], channel-major on FP32, [pair][512][L]):
+ *       [0] f3    TC only: detection-major rows [(pair*L + l)*3 + stack][512]; stacks 0 and 1 the transpose of feats,
+ *                 stack 2 the fused features
  *       [1] h2    second w_det layer (after its ReLU): TC [(pair*L + l)*3 + stack][256], FP32 [g][256][L]
+ *       [2] yp    input_w (A) or input_p (B, C) before its GroupNorm   [3] yi  input_i before its GroupNorm (B, C)
+ *       [4] gp    gate_p logits (C)   [5] gi  gate_i logits (C)
+ *       [6] scp [7] shp   GroupNorm(512, 512) affine of yp [pair][512]
+ *       [8] sci [9] shi   GroupNorm(512, 512) affine of yi [pair][512] (B, C)
+ *       [10] h1   first w_det layer (after its ReLU): TC [(pair*L + l)*3 + stack][512], FP32 [g][512][L]
+ *       [11] stats  fp64 (sum, sum of squares) [pairs][512][2], written by each GroupNorm branch in turn: at the end
+ *                 the last branch's (yp for A, yi for B and C)
+ *       [12] part  fp64 (sum, sum of squares) per column-tile partial [tile*k + half][512], k = 2 on TC (256-column
+ *                 tiles, two halves) and 1 on FP32 (128-column tiles), tiles pair*tpg .. (pair+1)*tpg - 1 of each
+ *                 pair; at the end the last GroupNorm branch's
+ *       A buffer the fusion architecture does not use is left untouched.
  *     stage 2, 27 offsets (carve order; ndet = pairs*L detections, d = pair*L + l; a buffer a path does not use has
  *     size 0 there; sc / sh / stats / part are reused layer after layer and end as conv2's):
  *       [0] xt    FP32: 3-channel points channel-major [3][P] (4-channel points are transposed into t1 instead, which

@@ -153,12 +153,13 @@ extern "C" size_t mmmot_fusion_det_workspace(int pairs, int L) {
   return a.off;
 }
 
-// mmmot_debug_stage_layout, stage 1: where mmmot_fusion_det_fwd leaves F3 and h2 (a dry carve; no CUDA call)
+// mmmot_debug_stage_layout, stage 1: where mmmot_fusion_det_fwd leaves its intermediates (a dry carve; no CUDA call):
+// f3 and h2 first, then the rest in carve order
 int mm_fusion_det_layout(int pairs, int L, size_t* off, int* tensor_cores) {
   MmArena a(nullptr, 0);
   const FdWs w = carve(a, pairs, L);
-  off[0] = (size_t)reinterpret_cast<uintptr_t>(w.f3);
-  off[1] = (size_t)reinterpret_cast<uintptr_t>(w.h2);
+  const void* bufs[13] = {w.f3, w.h2, w.yp, w.yi, w.gp, w.gi, w.scp, w.shp, w.sci, w.shi, w.h1, w.stats, w.part};
+  for (int i = 0; i < 13; i++) off[i] = (size_t)reinterpret_cast<uintptr_t>(bufs[i]);
   if (tensor_cores) *tensor_cores = fusion_det_use_tc(L) ? 1 : 0;
   return 0;
 }

@@ -129,7 +129,7 @@ def nan_workspace(lib, nbytes):
 AF_BUFS = ("y01", "y3", "z", "fcl", "sc0", "sh0", "sc3", "sh3", "v", "h2", "nsc2", "nsh2", "rmax", "rsum", "cmax", "csum",
            "y2", "sc1", "sh1", "sc2", "sh2", "h1", "nsc1", "nsh1", "stats", "nstats", "part", "npart", "tiles", "cnt",
            "gstart")
-FD_BUFS = ("f3", "h2")
+FD_BUFS = ("f3", "h2", "yp", "yi", "gp", "gi", "scp", "shp", "sci", "shi", "h1", "stats", "part")
 PN_BUFS = ("xt", "y1", "t0", "t1", "big", "segsum", "x1p", "xp", "gmean", "u", "ut", "hmean", "o", "sc1", "sh1", "sc",
            "sh", "stats", "mom", "part", "gstart", "sstart", "seg", "cnt", "tiles", "ctab", "end")
 STAGE_BUFS = (AF_BUFS, FD_BUFS, PN_BUFS)
@@ -279,6 +279,20 @@ def stats_ratios(S1, S2, y, grp, G):
     rm = ((m - mean).abs() / tm.clamp_min(1e-300))[keep]
     cond = (mean.abs() / var.clamp_min(1e-300).sqrt())[keep]
     return float(rv.max()), float(rm.max()), float(cond.max())
+
+
+def reduce_ref(part, ranges):
+    """stats_reduce's fixed-order fp64 sum of part [slots][M][2] over each group's slot range [t0, t1) -> [G][M][2]."""
+    out = []
+    for t0, t1 in ranges:
+        tot = torch.zeros_like(part[0])
+        for y in range(8):
+            s = torch.zeros_like(part[0])
+            for t in range(t0 + y, t1, 8):
+                s = s + part[t]
+            tot = tot + s
+        out.append(tot)
+    return torch.stack(out)
 
 
 def group_sum(v, idx, G):

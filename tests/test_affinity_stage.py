@@ -61,7 +61,8 @@ import torch
 
 from kernel_kit import (BN, TAU, XM, Workspace, affine_bound, case_seed, contraction_bound, eval_net, gn_affine,
                         gn_stats, group_moments, impl_launches, lib_state, nan_output, nan_workspace, ne_tiles_host,
-                        norm_operand, pair_operand, ref_linear, report, stage_layout, stats_ratios, vp, worst_ratio)
+                        norm_operand, pair_operand, reduce_ref, ref_linear, report, stage_layout, stats_ratios, vp,
+                        worst_ratio)
 from mmmot_b200 import _lib
 from mmmot_b200.synthetic import synthetic_state_dict
 
@@ -138,20 +139,6 @@ def gn_check(y, grp, G, gamma, beta, sc, sh, cpg=1):
     """sc / sh [G][C] of a GroupNorm over the stored y [cols][C] (fp64) -> worst err / bound of both."""
     a, b, Ta, Tb = affine_bound(gn_stats(y, grp, G, cpg=cpg), gamma, beta)
     return max(worst_ratio(sc, a, Ta), worst_ratio(sh, b, Tb))
-
-
-def reduce_ref(part, ranges):
-    """stats_reduce's fixed-order fp64 sum of part [slots][M][2] over each group's slot range [t0, t1) -> [G][M][2]."""
-    out = []
-    for t0, t1 in ranges:
-        tot = torch.zeros_like(part[0])
-        for y in range(8):
-            s = torch.zeros_like(part[0])
-            for t in range(t0 + y, t1, 8):
-                s = s + part[t]
-            tot = tot + s
-        out.append(tot)
-    return torch.stack(out)
 
 
 def ne_groups(G, n, m, device):

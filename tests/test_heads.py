@@ -99,7 +99,11 @@ def af_sizes(pairs, n, m):
 
 
 def fd_sizes(pairs, L):
-    return dict(f3=4 * 3 * pairs * 512 * L, h2=4 * 3 * pairs * 256 * L)
+    """Bytes of each fusion / detection-score intermediate (the header's shapes; part holds two partials per 128
+    columns, room for either path's tiling)."""
+    n, pc = pairs * 512 * L, pairs * 512
+    return dict(f3=12 * n, h2=6 * n, yp=4 * n, yi=4 * n, gp=4 * n, gi=4 * n, scp=4 * pc, shp=4 * pc, sci=4 * pc, shi=4 * pc,
+                h1=12 * n, stats=16 * pc, part=16 * pc * 2 * -(-L // 128))
 
 
 # ------------------------------------------------------------------------------------------------ fp64 bounds
