@@ -30,6 +30,15 @@ D = 512
 RESNET_BLOCKS = {"resnet50": (3, 4, 6, 3), "resnet101": (3, 4, 23, 3), "resnet152": (3, 8, 36, 3)}
 RES_SKIP_CHANNELS = (256, 512, 1024, 2048)
 APPEAR_ARCHS = ("vgg",) + tuple(RESNET_BLOCKS)
+# appear_len = point_len of the nets the reference builds: vgg16_bn_512 / _256 / _128 (modules/vgg.py:83-98, configs D,
+# D_256, D_128) and every PointNet, fusion, affinity and w_det width divided by 512 // width (modules/point_net.py:10-19)
+WIDTHS = (512, 256, 128)
+
+
+def vgg_stages(width=D):
+    """VGG_STAGES of the width-``width`` trunk: every conv's channels divided by 512 // width, the image's 3 kept."""
+    r = D // width
+    return tuple(tuple((idx, cin if cin == 3 else cin // r, cout // r) for idx, cin, cout in st) for st in VGG_STAGES)
 
 
 def skip_mid(c):
@@ -93,20 +102,20 @@ def _lin_gn(sd, conv, norm, cin, cout, wshape):
         sd[f"{norm}.bias"] = ((cout,), "norm_b")
 
 
-def _stn(sd, p, cin, k):
+def _stn(sd, p, cin, k, r=1):
     sd[f"{p}.idt"] = ((k, k), "eye")
-    _lin_gn(sd, f"{p}.conv1", f"{p}.bn1", cin, 64, (64, cin, 1))
-    _lin_gn(sd, f"{p}.conv2", f"{p}.bn2", 64, 128, (128, 64, 1))
-    _lin_gn(sd, f"{p}.conv3", f"{p}.bn3", 128, 1024, (1024, 128, 1))
-    _lin_gn(sd, f"{p}.fc1", f"{p}.fc_bn1", 1024, 512, (512, 1024))
-    _lin_gn(sd, f"{p}.fc2", f"{p}.fc_bn2", 512, 256, (256, 512))
-    sd[f"{p}.output.weight"] = ((k * k, 256), "stn_out")
+    _lin_gn(sd, f"{p}.conv1", f"{p}.bn1", cin, 64 // r, (64 // r, cin, 1))
+    _lin_gn(sd, f"{p}.conv2", f"{p}.bn2", 64 // r, 128 // r, (128 // r, 64 // r, 1))
+    _lin_gn(sd, f"{p}.conv3", f"{p}.bn3", 128 // r, 1024 // r, (1024 // r, 128 // r, 1))
+    _lin_gn(sd, f"{p}.fc1", f"{p}.fc_bn1", 1024 // r, 512 // r, (512 // r, 1024 // r))
+    _lin_gn(sd, f"{p}.fc2", f"{p}.fc_bn2", 512 // r, 256 // r, (256 // r, 512 // r))
+    sd[f"{p}.output.weight"] = ((k * k, 256 // r), "stn_out")
     sd[f"{p}.output.bias"] = ((k * k,), "stn_out")
 
 
-def _fpn(sd):
-    """The FPN head (reference modules/appear_net.py:83-104): per ResNet stage a bias-free 1x1 lateral C -> 512 and its
-    BatchNorm2d (fpn_in.k.0 / .1), then conv_last.1 (1x1, 512 -> 512, with bias) and its BatchNorm2d conv_last.2."""
+def _fpn(sd, D=D):
+    """The FPN head (reference modules/appear_net.py:83-104): per ResNet stage a bias-free 1x1 lateral C -> D and its
+    BatchNorm2d (fpn_in.k.0 / .1), then conv_last.1 (1x1, D -> D, with bias) and its BatchNorm2d conv_last.2."""
     for k, c in enumerate(RES_SKIP_CHANNELS):
         sd[f"appearance.fpn_in.{k}.0.weight"] = ((D, c, 1, 1), "conv")
         _bn(sd, f"appearance.fpn_in.{k}.1", D)
@@ -118,31 +127,35 @@ def _fpn(sd):
 APPEAR_HEADS = ("skippool", "fpn")
 
 
-def state_schema(fusion="C", point_in=3, appear_arch="vgg", appear_head="skippool"):
+def state_schema(fusion="C", point_in=3, appear_arch="vgg", appear_head="skippool", width=D):
     """OrderedDict key -> (shape, kind).  ``kind`` drives init / synthetic generation:
     conv, bias, norm_w, res_norm_w, norm_b, run_mean, run_var, nbt, eye, stn_out.
     appear_arch: "vgg" (VGG16-BN) or a key of RESNET_BLOCKS; appear_head: "skippool" (four SkipPool heads,
-    appear_skippool) or "fpn" (the FPN head, appear_fpn; ResNet trunks only)."""
+    appear_skippool) or "fpn" (the FPN head, appear_fpn; ResNet trunks only); width: appear_len = point_len, one of
+    WIDTHS (the reference divides every width of the net below 512 by r = 512 // width)."""
     if appear_head not in APPEAR_HEADS or (appear_head == "fpn" and appear_arch == "vgg"):
         raise ValueError(f"unsupported appearance head {appear_head!r} on {appear_arch!r}")
+    if width not in WIDTHS:
+        raise ValueError(f"unsupported width {width!r} (appear_len = point_len must be one of {WIDTHS})")
+    d, r = width, D // width
     sd = OrderedDict()
     # --- fusion_module (modules/fusion_net.py) ---
     f = "fusion_module"
     if fusion == "C":
         for g in ("gate_p", "gate_i"):
-            _lin_gn(sd, f"{f}.{g}.0", None, D, D, (D, D, 1))
+            _lin_gn(sd, f"{f}.{g}.0", None, d, d, (d, d, 1))
         for g in ("input_p", "input_i"):
-            _lin_gn(sd, f"{f}.{g}.0", f"{f}.{g}.1", D, D, (D, D, 1))
+            _lin_gn(sd, f"{f}.{g}.0", f"{f}.{g}.1", d, d, (d, d, 1))
     elif fusion == "B":
         for g in ("input_p", "input_i"):
-            _lin_gn(sd, f"{f}.{g}.0", f"{f}.{g}.1", D, D, (D, D, 1))
+            _lin_gn(sd, f"{f}.{g}.0", f"{f}.{g}.1", d, d, (d, d, 1))
     elif fusion == "A":
-        _lin_gn(sd, f"{f}.input_w.0", f"{f}.input_w.1", 2 * D, D, (D, 2 * D, 1))
+        _lin_gn(sd, f"{f}.input_w.0", f"{f}.input_w.1", 2 * d, d, (d, 2 * d, 1))
     else:
         raise ValueError(f"unknown fusion arch {fusion!r}")
     # --- appearance (modules/appear_net.py, modules/vgg.py or torchvision's ResNet) ---
     if appear_arch == "vgg":
-        for s, stage in enumerate(VGG_STAGES):
+        for s, stage in enumerate(vgg_stages(width)):
             for idx, cin, cout in stage:
                 _conv_bn(sd, f"appearance.layers.{s}", idx, cin, cout, 3)
     elif appear_arch in RESNET_BLOCKS:
@@ -150,44 +163,46 @@ def state_schema(fusion="C", point_in=3, appear_arch="vgg", appear_head="skippoo
     else:
         raise ValueError(f"unknown appearance arch {appear_arch!r}")
     if appear_head == "fpn":
-        _fpn(sd)
-    for s, c in enumerate(() if appear_head == "fpn" else SKIP_CHANNELS if appear_arch == "vgg" else RES_SKIP_CHANNELS):
+        _fpn(sd, d)
+    skip = () if appear_head == "fpn" else tuple(c // r for c in SKIP_CHANNELS) if appear_arch == "vgg" else RES_SKIP_CHANNELS
+    for s, c in enumerate(skip):
         p = f"appearance.global_pool.{s}.fc"
         m = skip_mid(c)
         sd[f"{p}.0.weight"] = ((c,), "norm_w")
         sd[f"{p}.0.bias"] = ((c,), "norm_b")
         _lin_gn(sd, f"{p}.1", f"{p}.2", c, m, (m, c, 1, 1))
-        _lin_gn(sd, f"{p}.4", f"{p}.5", m, SKIP_OUT, (SKIP_OUT, m, 1, 1))
+        _lin_gn(sd, f"{p}.4", f"{p}.5", m, d // 4, (d // 4, m, 1, 1))
     # --- point_net (modules/point_net.py) ---
     p = "point_net.feat"
-    _stn(sd, f"{p}.stn1", point_in, point_in)
-    _lin_gn(sd, f"{p}.conv1", f"{p}.bn1", point_in, 64, (64, point_in, 1))
-    _lin_gn(sd, f"{p}.conv2", f"{p}.bn2", 64, 64, (64, 64, 1))
-    _stn(sd, f"{p}.stn2", 64, 64)
-    _lin_gn(sd, f"{p}.conv3", f"{p}.bn3", 64, 64, (64, 64, 1))
-    _lin_gn(sd, f"{p}.conv4", f"{p}.bn4", 64, 128, (128, 64, 1))
-    _lin_gn(sd, f"{p}.conv5", f"{p}.bn5", 128, 1024, (1024, 128, 1))
-    sd["point_net.conv1.weight"] = ((512, 1088, 1), "conv")
-    sd["point_net.conv1.bias"] = ((512,), "bias")
-    sd["point_net.conv2.weight"] = ((512, 512, 1), "conv")
-    sd["point_net.conv2.bias"] = ((512,), "bias")
-    for n in ("bn1", "bn2", "avg_bn"):
-        sd[f"point_net.{n}.weight"] = ((512,), "norm_w")
-        sd[f"point_net.{n}.bias"] = ((512,), "norm_b")
+    c64, c128, c1024, c512 = 64 // r, 128 // r, 1024 // r, 512 // r
+    _stn(sd, f"{p}.stn1", point_in, point_in, r)
+    _lin_gn(sd, f"{p}.conv1", f"{p}.bn1", point_in, c64, (c64, point_in, 1))
+    _lin_gn(sd, f"{p}.conv2", f"{p}.bn2", c64, c64, (c64, c64, 1))
+    _stn(sd, f"{p}.stn2", c64, c64, r)
+    _lin_gn(sd, f"{p}.conv3", f"{p}.bn3", c64, c64, (c64, c64, 1))
+    _lin_gn(sd, f"{p}.conv4", f"{p}.bn4", c64, c128, (c128, c64, 1))
+    _lin_gn(sd, f"{p}.conv5", f"{p}.bn5", c128, c1024, (c1024, c128, 1))
+    sd["point_net.conv1.weight"] = ((c512, c64 + c1024, 1), "conv")
+    sd["point_net.conv1.bias"] = ((c512,), "bias")
+    sd["point_net.conv2.weight"] = ((d, c512, 1), "conv")
+    sd["point_net.conv2.bias"] = ((d,), "bias")
+    for n, c in (("bn1", c512), ("bn2", d), ("avg_bn", c512)):
+        sd[f"point_net.{n}.weight"] = ((c,), "norm_w")
+        sd[f"point_net.{n}.bias"] = ((c,), "norm_b")
     # --- w_link (modules/gcn.py, modules/new_end.py) ---
     ne = "w_link.w_new_end"
-    _lin_gn(sd, f"{ne}.conv0.0", f"{ne}.conv0.1", D, D, (D, D, 1, 1))
-    _lin_gn(sd, f"{ne}.conv1.0", f"{ne}.conv1.1", D, D, (D, D, 1))
-    _lin_gn(sd, f"{ne}.conv1.3", f"{ne}.conv1.4", D, 128, (128, D, 1))
-    _lin_gn(sd, f"{ne}.conv1.6", None, 128, 1, (1, 128, 1))
-    _lin_gn(sd, "w_link.conv1.0", "w_link.conv1.1", D, D, (D, D, 1, 1))
-    _lin_gn(sd, "w_link.conv1.3", "w_link.conv1.4", D, D, (D, D, 1, 1))
-    _lin_gn(sd, "w_link.conv1.6", "w_link.conv1.7", D, 128, (128, D, 1, 1))
-    _lin_gn(sd, "w_link.conv1.9", None, 128, 1, (1, 128, 1, 1))
+    _lin_gn(sd, f"{ne}.conv0.0", f"{ne}.conv0.1", d, d, (d, d, 1, 1))
+    _lin_gn(sd, f"{ne}.conv1.0", f"{ne}.conv1.1", d, d, (d, d, 1))
+    _lin_gn(sd, f"{ne}.conv1.3", f"{ne}.conv1.4", d, d // 4, (d // 4, d, 1))
+    _lin_gn(sd, f"{ne}.conv1.6", None, d // 4, 1, (1, d // 4, 1))
+    _lin_gn(sd, "w_link.conv1.0", "w_link.conv1.1", d, d, (d, d, 1, 1))
+    _lin_gn(sd, "w_link.conv1.3", "w_link.conv1.4", d, d, (d, d, 1, 1))
+    _lin_gn(sd, "w_link.conv1.6", "w_link.conv1.7", d, d // 4, (d // 4, d, 1, 1))
+    _lin_gn(sd, "w_link.conv1.9", None, d // 4, 1, (1, d // 4, 1, 1))
     # --- w_det (modules/tracking_net.py:91-100) ---
-    _conv_bn(sd, "w_det", 0, D, D, 0)
-    _conv_bn(sd, "w_det", 3, D, D // 2, 0)
-    sd["w_det.6.weight"] = ((1, D // 2, 1), "conv")
+    _conv_bn(sd, "w_det", 0, d, d, 0)
+    _conv_bn(sd, "w_det", 3, d, d // 2, 0)
+    sd["w_det.6.weight"] = ((1, d // 2, 1), "conv")
     sd["w_det.6.bias"] = ((1,), "bias")
     return sd
 

@@ -11,10 +11,11 @@ import torch
 from .schema import state_schema
 
 
-def synthetic_state_dict(fusion="C", seed=0, point_in=3, appear_arch="vgg", appear_head="skippool"):
+def synthetic_state_dict(fusion="C", seed=0, point_in=3, appear_arch="vgg", appear_head="skippool", width=512):
     """A non-degenerate ``state_dict`` for ``TrackingNet`` with the reference's key names; point_in = 4 for a net on
     xyz + reflectance points (``without_reflectivity=False``); appear_arch "vgg" or "resnet50" / "resnet101" /
-    "resnet152" for the appearance trunk; appear_head "skippool" or "fpn" (``appear_fpn=True``, ResNet trunks).
+    "resnet152" for the appearance trunk; appear_head "skippool" or "fpn" (``appear_fpn=True``, ResNet trunks); width
+    the net's appear_len = point_len (512, 256 or 128).
 
     Default inits make every GroupNorm the identity affine and both STN output layers zero
     (reference: modules/point_net.py:69-70), which hides bugs; so norm affines, BN running
@@ -23,7 +24,7 @@ def synthetic_state_dict(fusion="C", seed=0, point_in=3, appear_arch="vgg", appe
     after block (2^50 through ResNet-152)."""
     g = torch.Generator().manual_seed(1000 + seed)
     sd = {}
-    for key, (shape, kind) in state_schema(fusion, point_in, appear_arch, appear_head).items():
+    for key, (shape, kind) in state_schema(fusion, point_in, appear_arch, appear_head, width).items():
         if kind == "conv":
             fan_in = 1
             for s in shape[1:]:

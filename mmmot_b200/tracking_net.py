@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .schema import BUFFER_KINDS, RESNET_BLOCKS, VGG_POOL_AFTER, VGG_STAGES, state_schema
+from .schema import BUFFER_KINDS, RESNET_BLOCKS, VGG_POOL_AFTER, VGG_STAGES, WIDTHS, state_schema
 
 # conv k of the 13 is followed by a 2x2 max-pool (so the map of conv k+1 is 4x smaller)
 VGG_POOLED_BEFORE = [idx in VGG_POOL_AFTER[s] for s, stage in enumerate(VGG_STAGES) for idx, _, _ in stage]
@@ -78,7 +78,8 @@ class TrackingNet(nn.Module):
         # the value space of the shipped experiments/*/config.yaml (SURVEY §8b); anything else is
         # rejected loudly instead of silently computing something different
         unsupported = []
-        if appear_len != 512 or point_len != 512: unsupported.append("appear_len/point_len != 512")
+        if appear_len != point_len or appear_len not in WIDTHS:
+            unsupported.append(f"appear_len/point_len must be equal and one of {WIDTHS}")
         if appear_arch not in ('vgg',) + tuple(RESNET_BLOCKS) or bool(appear_skippool) == bool(appear_fpn) or \
                 (appear_fpn and appear_arch == 'vgg'):
             unsupported.append("appearance must be vgg + skippool, or resnet50, resnet101 or resnet152 + skippool or fpn")
@@ -99,13 +100,16 @@ class TrackingNet(nn.Module):
         self.score_fusion_arch = score_fusion_arch
         self.appear_arch = appear_arch
         self.appear_head = "fpn" if appear_fpn else "skippool"
+        # appear_len = point_len: the width of the feature stacks (a narrower net runs as its 512-wide embedding,
+        # weights.embed_width)
+        self.width = appear_len
         # dropblock / use_dropout are identity in eval mode; accepted for config compatibility
         self.dropblock, self.use_dropout = dropblock, use_dropout
         # PointNet's input width (tracking_net.py:41): xyz, or xyz + LiDAR reflectance
         self.point_channels = 4 - int(bool(without_reflectivity))
         gen = torch.Generator().manual_seed(0)
         for key, (shape, kind) in state_schema(score_fusion_arch, self.point_channels, appear_arch,
-                                                self.appear_head).items():
+                                                self.appear_head, self.width).items():
             _register(self, key, _default_init(shape, kind, gen), kind in BUFFER_KINDS)
         for name, prm in self.named_parameters():
             if name.endswith(".idt"):           # reference point_net.py:62: requires_grad=False
@@ -133,7 +137,7 @@ class TrackingNet(nn.Module):
         if self._prepared is None or self._prepared.flat.device != dev:
             _lib.load()
             self._prepared = DeviceWeights(self.state_dict(), self.score_fusion_arch, dev, self.appear_arch,
-                                           self.appear_head)
+                                           self.appear_head, self.width)
         return self._prepared
 
     def _split_to_device(self, s_host, dev):
@@ -288,7 +292,8 @@ class TrackingNet(nn.Module):
         points_split  (B*(n+m) + 1,) int     CSR offsets, CPU tensor (the reference reads it with
                                              .item() per detection: modules/point_net.py:33-35)
         returns dict: det B x 3 x L, link B x 3 x n x m, new B x 3 x m, end B x 3 x n (un-padded),
-                      trans [1xCxC, 1x64x64]; per-pair semantics identical to ``forward``; "status": the library's
+                      trans [1xCxC, 1xKxK] (K = 64 * width / 512); feats B x 3 x width x L with keep_feats, in the
+                      reference's channel order; per-pair semantics identical to ``forward``; "status": the library's
                       status word (int32 device tensor; bit 0 = an activation left FP16's range, MMMOT_E_RANGE).
         check=True (default) reads the status word back (one host sync) and raises MmmotError when it is set;
         pipelined callers pass check=False and test ``out["status"]`` together with the results they copy back.
@@ -337,7 +342,9 @@ class TrackingNet(nn.Module):
                 # the status word (FP16 range flag) of this chunk, accumulated into out["status"] in stream order
                 out["status"] |= ws[:4].view(torch.int32)
         out["trans"] = [wts.trans1.unsqueeze(0).clone(), wts.trans2.unsqueeze(0).clone()]
-        if not keep_feats:
+        if keep_feats:
+            out["feats"] = wts.narrow(out["feats"])
+        else:
             del out["feats"]
         if check:
             self._raise_on_status(out["status"])
@@ -346,14 +353,15 @@ class TrackingNet(nn.Module):
     @torch.no_grad()
     def associate_batch(self, feats, n, m=None):
         """Affinity / start-end / softmax stage alone (reference TrackingNet.associate on every
-        stack): feats B x 3 x 512 x (n+m) CUDA -> (link B x 3 x n x m, new B x 3 x m, end B x 3 x n)."""
+        stack): feats B x 3 x width x (n+m) CUDA -> (link B x 3 x n x m, new B x 3 x m, end B x 3 x n)."""
         m = n if m is None else m
         lib = _lib.load()
         wts = self.prepared()
         dev = wts.flat.device
         feats = feats.contiguous().float()
         B = feats.shape[0]
-        assert feats.shape[1:] == (3, 512, n + m) and feats.device == dev
+        assert feats.shape[1:] == (3, self.width, n + m) and feats.device == dev
+        feats = wts.widen(feats)
         link = torch.empty(B, 3, n, m, device=dev)
         new = torch.empty(B, 3, m, device=dev)
         end = torch.empty(B, 3, n, device=dev)
@@ -438,6 +446,9 @@ class TrackingNet(nn.Module):
         if self.training and self.appear_arch != "vgg":
             raise NotImplementedError("mmmot_b200.TrackingNet: the training-mode forward (batch-statistics BatchNorm) "
                                       "runs the VGG appearance trunk only")
+        if self.training and self.width != 512:
+            raise NotImplementedError("mmmot_b200.TrackingNet: the training-mode forward runs 512-wide nets only "
+                                      f"(appear_len = point_len = {self.width} runs in eval mode)")
         if self.training and len(splits) != 2:
             raise NotImplementedError("mmmot_b200.TrackingNet supports 2-frame samples (sample_max_len: 2)")
         L = sum(splits)

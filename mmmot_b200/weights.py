@@ -10,7 +10,9 @@ C ABI expects (``enum mmmot_weight_id`` in include/mmmot_b200.h):
 * the 1088-wide head conv (modules/point_net.py:13,27-28) split into its 64 local and 1024
   per-detection-global columns (SURVEY B-9);
 * affinity conv1.0 and new/end conv0 stacked into one 512 -> 1024 matrix (same input tensor);
-* every matrix transposed to Wt[K][Cout].
+* every matrix transposed to Wt[K][Cout];
+* a net narrower than 512 (appear_len = point_len = 256 or 128) embedded in an equivalent 512-wide one first
+  (embed_width), so the same operands and kernels run it.
 
 The folding is done once in fp64 on the host and rounded to fp32; it is checkpoint conversion,
 not part of the per-frame path.
@@ -20,7 +22,7 @@ import ctypes
 import torch
 
 from . import _lib
-from .schema import RES_SKIP_CHANNELS, RESNET_BLOCKS, SKIP_CHANNELS, VGG_STAGES, resnet_convs
+from .schema import D, RES_SKIP_CHANNELS, RESNET_BLOCKS, SKIP_CHANNELS, SKIP_OUT, VGG_STAGES, resnet_convs, state_schema
 
 EPS = 1e-5
 W = _lib.W
@@ -271,12 +273,88 @@ def prepare(state_dict, fusion, appear_arch="vgg"):
     return out, t1.float(), t2.float(), scales
 
 
+def stack_index(width):
+    """pi: channel i of a 512-wide feature stack of the embedded net carries channel pi(i) of the width-``width`` net's
+    stack.  The SkipPool heads write head s to channels [128 s, 128 s + 128), so pi maps that block onto copies of head
+    s's width / 4 channels: pi(i) = (i // 128) * width / 4 + i % (width / 4).  Each aligned 32-channel block then holds
+    one whole group of PointNet's GroupNorm(16 // r, width) (groups of 32), which GroupNorm(16, 512) sees unchanged."""
+    q = width // 4
+    i = torch.arange(D)
+    return (i // SKIP_OUT) * q + i % q
+
+
+def _channel_index(red, pad, width):
+    """The channels of a width-``red`` activation of the narrow net in its ``pad``-wide copy (pad / red copies of each):
+    the feature stacks (and every other width-``width`` activation) by stack_index, any other one tiled."""
+    if red == pad:
+        return None
+    if red == width and pad == D:
+        return stack_index(width)
+    return torch.arange(pad) % red
+
+
+def embed_width(state_dict, fusion, width, appear_arch="vgg", appear_head="skippool"):
+    """The state_dict of a width-``width`` net (appear_len = point_len in {256, 128}, the reference's key names and
+    shapes) -> an fp64 state_dict of the 512-wide net that computes it exactly, each activation as k identical copies
+    (k = its 512-wide width over its own: 1, 2 or 4, so every division below is exact).  A layer whose input grows
+    k_in-fold gets W_pad[i][j] = W[pi_out(i)][pi_in(j)] / k_in and bias b[pi_out(i)]; per-channel parameters (BatchNorm,
+    GroupNorm affines and running statistics) are gathered by pi.  Per-channel operations keep the copies equal, and
+    GroupNorm(1, C) or GroupNorm(G, C) over whole copies of its groups sees the narrow net's statistics.
+
+    Two inputs are concatenations (fusion A's input_w: image | LiDAR stack; PointNet's head conv: local 64 | global 1024
+    features) and are indexed piecewise.  STN2's output row (a, b) is T2[pi(a)][pi(b)]: its output layer and idt are
+    embedded as T2_pad = T2[pi][pi] / k, which turns x T2 on the narrow features into x_pad T2_pad on their copies."""
+    sd = {k: v.detach().cpu() for k, v in state_dict.items()}
+    point_in = sd["point_net.feat.conv1.weight"].shape[1]
+    wide = state_schema(fusion, point_in, appear_arch, appear_head)
+    ix = lambda red, pad: _channel_index(red, pad, width)
+    out = {}
+    for key, (shape, _) in wide.items():
+        t = sd[key].double() if sd[key].is_floating_point() else sd[key].clone()
+        if t.dim() >= 1 and t.shape[0] != shape[0]:
+            t = t[ix(t.shape[0], shape[0])]
+        if t.dim() >= 2 and t.shape[1] != shape[1]:
+            c = t.shape[1]
+            if key == "fusion_module.input_w.0.weight":
+                j = torch.cat([ix(c // 2, D), c // 2 + ix(c // 2, D)])
+            elif key == "point_net.conv1.weight":
+                c64 = sd["point_net.feat.conv1.weight"].shape[0]
+                j = torch.cat([ix(c64, 64), c64 + ix(c - c64, 1024)])
+            else:
+                j = ix(c, shape[1])
+            t = t[:, j] / (shape[1] // c)
+        out[key] = t
+    # STN2 emits the 64/r x 64/r matrix T2 flattened: row a * 64/r + b of its output layer; idt was gathered and divided
+    # above like a matrix [a][b] (rows by pi, columns by pi over k)
+    k2 = sd["point_net.feat.stn2.idt"].shape[0]
+    if k2 != 64:
+        p = ix(k2, 64)
+        rows = (p[:, None] * k2 + p[None, :]).reshape(-1)
+        s = "point_net.feat.stn2"
+        kk = 64 // k2
+        out[f"{s}.output.weight"] = sd[f"{s}.output.weight"].double()[rows][:, ix(256 * k2 // 64, 256)] / (kk * kk)
+        out[f"{s}.output.bias"] = sd[f"{s}.output.bias"].double()[rows] / kk
+    return out
+
+
 class DeviceWeights:
     """All prepared tensors in ONE flat device buffer (256-byte aligned slices) + the pointer table
     handed to the C ABI."""
 
-    def __init__(self, state_dict, fusion, device, appear_arch="vgg", appear_head="skippool"):
+    def __init__(self, state_dict, fusion, device, appear_arch="vgg", appear_head="skippool", width=D):
+        self.width = width
+        narrow = None
+        if width != D:
+            # a narrow net runs as its 512-wide embedding; trans keeps the narrow net's T2, features its channels
+            narrow = state_dict
+            state_dict = embed_width(state_dict, fusion, width, appear_arch, appear_head)
+            pi = stack_index(width)
+            self.widen_index = pi.to(device)
+            self.narrow_index = (pi[:, None] == torch.arange(width)).int().argmax(0).to(device)     # first copy
         tensors, self.trans1, self.trans2, scales = prepare(state_dict, fusion, appear_arch)
+        if narrow is not None:
+            k2 = narrow["point_net.feat.stn2.idt"].shape[0]
+            self.trans2 = stn_constant({k: v.detach().cpu() for k, v in narrow.items()}, "point_net.feat.stn2", k2).float()
         nmain = len(tensors)
         self.resnet = self.fpn = None
         if appear_arch != "vgg":
@@ -327,3 +405,11 @@ class DeviceWeights:
         self.ptr = ctypes.pointer(self.table)
         self.trans1 = self.trans1.to(device)
         self.trans2 = self.trans2.to(device)
+
+    def narrow(self, feats):
+        """B x 3 x 512 x L features of the embedded net -> B x 3 x width x L, the narrow net's channels in its order."""
+        return feats if self.width == D else feats.index_select(2, self.narrow_index)
+
+    def widen(self, feats):
+        """B x 3 x width x L features of the narrow net -> their 512-wide embedding (narrow's inverse)."""
+        return feats if self.width == D else feats.index_select(2, self.widen_index).contiguous()
