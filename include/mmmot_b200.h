@@ -452,7 +452,9 @@ int mmmot_set_kseg(int chunks);
  *                 instead of TMA-staged source rows
  *   bit 13 (8192) PointNet layers 3, 4 through norm_split + the TMA-fed kernel instead of GEN_NORM producers
  *   bit 14 (16384) first VGG layer with a separate im2col pre-pass instead of in-kernel operand producers
- *   bit 15 (32768) first VGG block as two launches (layer 0, then layer 1 + pool) instead of the fused kernel */
+ *   bit 15 (32768) first VGG block as two launches (layer 0, then layer 1 + pool) instead of the fused kernel
+ *   bit 16 (65536) PointNet's per-detection-sum passes (layer 5, head) on the general TMA-fed kernel instead of the
+ *                  dedicated one (csrc/gemm_segsum.cuh; mmmot_debug_segsum_kernel) */
 int mmmot_set_debug(int flags);
 
 /* Test hook: one launch of the FP32 FFMA engine in any operand mode, with its GroupNorm partials (device pointers).
@@ -512,6 +514,12 @@ int mmmot_debug_pn_contraction(const int* det_split, const int* h_det_split, int
                                int* cnt, int* gstart, int* seg, void* ctab, long* n_tiles, const void* Wp, float wp_scale,
                                const float* bias, int M, int K, const void* Xhi, float* Y, void* part, const float* addend,
                                int ld_add, unsigned long long* segsum, const float* sc, const float* sh, void* stream);
+
+/* Which kernel a matrix-mode contraction with per-detection sums (segsum, as mmmot_debug_pn_contraction) takes under
+ * the current mmmot_set_debug state: 1 = the dedicated per-detection-sum kernel (csrc/gemm_segsum.cuh: K = 64 or 128,
+ * no Y, no partials, no ReLU, debug bit 16 clear), 0 = the general TMA-fed kernel; MMMOT_E_ARG unless K is a positive
+ * multiple of 32.  Computed on the host without any CUDA call. */
+int mmmot_debug_segsum_kernel(int K, int has_y, int has_part, int relu);
 
 /* Test hook of the GroupNorm statistics of PointNet's two widest tensor-core layers (csrc/pointnet.cu), computed as
  * mmmot_pointnet_fwd computes them under the current mmmot_set_debug bits: y = x Wt + bias (+ addend[det]) over the

@@ -97,6 +97,7 @@ SIGNATURES = {
                              ctypes.POINTER(_i), _vp]),
     "mmmot_debug_pn_contraction": (_i, [_vp, _vp, _i, _i, _l, _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_l), _vp, _f, _vp, _i, _i,
                                         _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "mmmot_debug_segsum_kernel": (_i, [_i, _i, _i, _i]),
     "mmmot_debug_pn_stats": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                   _sz, _vp]),
     "mmmot_debug_stage_layout": (_i, [_i, _i, _i, _i, ctypes.POINTER(_sz), ctypes.POINTER(_i)]),

@@ -247,6 +247,13 @@ extern "C" int mmmot_debug_gen_staged(int gen, int m) {
 // Whether a GEN_NORM launch under debug flags dbg stages its source rows by TMA (1) or not, on the host, no CUDA call.
 extern "C" int mmmot_debug_gen_norm_staged(int dbg) { return gen_norm_staged(dbg) ? 1 : 0; }
 
+// Which kernel a per-detection-sum launch of the TMA-fed contraction takes (1 = gemm_segsum_kernel, 0 = gemm_tma_kernel)
+// under the current debug flags, on the host, no CUDA call.
+extern "C" int mmmot_debug_segsum_kernel(int K, int has_y, int has_part, int relu) {
+  if (K <= 0 || K % tc::BK) return MMMOT_E_ARG;
+  return segsum_dedicated(K, true, has_y != 0, has_part != 0, relu != 0, mm_debug_flags()) ? 1 : 0;
+}
+
 // One contraction of the generated-operand tensor-core engine (gemm_gen.cuh) through gemm_gen_launch, with the
 // arguments the affinity, PointNet and fusion stages pass it.
 extern "C" int mmmot_debug_gen(int gen, int M, int K, const void* Wp, float wp_scale, const float* bias, int relu,

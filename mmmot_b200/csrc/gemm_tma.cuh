@@ -682,6 +682,27 @@ static int gemm_tma_px_launch_gen27(const float* crops, int n_img, int H, int W,
   return 0;
 }
 
+#include "gemm_segsum.cuh"
+
+// Whether a matrix-mode launch takes gemm_segsum_kernel (gemm_segsum.cuh): the per-detection-sum pass at K = 64 or 128
+// with nothing stored, no statistics and no ReLU before the affine; debug bit 16 (65536) keeps gemm_tma_kernel (A/B
+// runs).  Pure host logic, no CUDA call (mmmot_debug_segsum_kernel).
+static inline bool segsum_dedicated(int K, bool segsum, bool y, bool part, bool relu, int dbg) {
+  return segsum && !y && !part && !relu && (K == 64 || K == 128) && !(dbg & 65536);
+}
+
+template <int K>
+static int gemm_segsum_launch(const tma::TmaP& P, const CUtensorMap& mh, const CUtensorMap& ml, int sms, cudaStream_t st) {
+  static std::atomic<unsigned long long> attr{0};
+  MM_TRY(mm_ensure_smem(tma::gemm_segsum_kernel<K>, tma::SegsumCfg<K>::SMEM, attr));
+  const int mg_per = tma::segsum_mg_per(P.t.g.num_tiles, P.t.m_tiles, sms);
+  const long units = (long)P.t.g.num_tiles * ((P.t.m_tiles + mg_per - 1) / mg_per);
+  const int grid = (int)(units < sms ? units : sms);
+  tma::gemm_segsum_kernel<K><<<grid, tma::SS_THREADS, tma::SegsumCfg<K>::SMEM, st>>>(P, mh, ml, mg_per);
+  MM_LAUNCH_CHECK();
+  return 0;
+}
+
 // 1x1 contraction on planar FP16 (hi, lo) channels-last activations X_hi[rows][ldx], X_lo = X_hi + x_plane.
 // g: M, K (multiple of 32), bias, tiles, x_gs (rows per group), Y / y_ms / y_gs, part, addend...
 static int gemm_tma_launch_mat(const GemmP& g, const uint4* Wp, float out_scale, const __half* Xhi, long x_plane,
@@ -715,6 +736,10 @@ static int gemm_tma_launch_mat(const GemmP& g, const uint4* Wp, float out_scale,
       !(P.t.dbg & 64)) {
     if (Wpx) { P.t.Wp = Wpx; P.wcompact = 1; }
     return gemm_tma_px_launch(P, mh, ml, sms, st);
+  }
+  if (segsum_dedicated(g.K, segsum != nullptr, g.Y != nullptr, g.part != nullptr, g.relu != 0, P.t.dbg)) {
+    if (!g.seg || !g.sc || !g.sh) return MMMOT_E_ARG;
+    return g.K == 128 ? gemm_segsum_launch<128>(P, mh, ml, sms, st) : gemm_segsum_launch<64>(P, mh, ml, sms, st);
   }
   const long total = (long)g.num_tiles * P.t.m_tiles;
   const int grid = (int)(total < sms ? total : sms);

@@ -4,7 +4,10 @@ Run on a GPU box:  python tools/pn_times.py [n] [pts] [pairs] [channels]     TC_
 channels: the point width, 3 (xyz) or 4 (xyz + reflectance, a without_reflectivity=False net), or a comma list such as
 3,4: one net per width on the same xyz, measured in ROUNDS alternating rounds (default 5) in this one process.  Each
 round times the stage over REPS untimed-hook calls (default 20) with CUDA events (median per call), then one call with
-the tagged timing hook on for the per-kernel lines.  The card's name, power limit and max SM clock come first."""
+the tagged timing hook on for the per-kernel lines (every round for layer 1 and the per-detection-sum passes, round 0
+for the rest).  TC_DBG takes a comma list too, alternated within each round in this one process: TC_DBG=0,65536 sets
+the dedicated per-detection-sum kernel against the general TMA-fed one.  The card's name, power limit and max SM clock
+come first."""
 import ctypes
 import os
 import statistics
@@ -83,7 +86,7 @@ def main():
             print(f"round {r} n={n} pts={pts} pairs={pairs} channels={c} dbg={dbg}: PointNet stage {ms:.3f} ms "
                   f"(median of {reps})")
             for name, (tms, fl, by, cnt) in tags.items():
-                if r == 0 or name.startswith("pointnet.l1"):
+                if r == 0 or name.startswith("pointnet.l1") or name.endswith("_segsum"):
                     print(f"   {name:32s} {tms:8.3f} ms  {fl / tms / 1e9 if tms else 0:8.1f} TFLOP/s  "
                           f"{by / tms / 1e6 if tms else 0:8.1f} GB/s")
     lib.mmmot_set_debug(0)
