@@ -274,6 +274,15 @@ size_t mmmot_fusion_det_workspace(int pairs, int L);
 int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold,
                          int pairs, int L, float* feats, float* det_scores,
                          void* workspace, size_t workspace_bytes, void* stream);
+/* One stack `stack` (0 image, 1 LiDAR, 2 fused) of mmmot_fusion_det_fwd, for a tracker that reads that stack only:
+ *   det_scores [pairs][L], bit-identical to stack `stack` of mmmot_fusion_det_fwd's det_scores.
+ *   stack 0 or 1: w_det on that stack of feats alone; no other stack is read, feats is not written, no fusion runs.
+ *   stack 2: fusion A/B/C writes stack 2 of feats as mmmot_fusion_det_fwd does, then w_det on stack 2 alone.
+ * The workspace (any stack) is smaller than mmmot_fusion_det_workspace's.  MMMOT_E_ARG for a stack outside 0..2. */
+size_t mmmot_fusion_det_stack_workspace(int pairs, int L);
+int mmmot_fusion_det_stack_fwd(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold,
+                               int pairs, int L, int stack, float* feats, float* det_scores,
+                               void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Training-mode variants (SURVEY.md 8f row N4) of the two stages that contain BatchNorm: in .train() the reference's
@@ -320,6 +329,16 @@ int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mo
                        int pairs, int n, int m, const float* feats,
                        float* link, float* new_s, float* end_s,
                        void* workspace, size_t workspace_bytes, void* stream);
+/* The same stage on one stack `stack` (0 image, 1 LiDAR, 2 fused) of each pair, a third of the work:
+ *   feats [pairs][3][512][N+M] as above, of which only stack `stack` is read
+ *   link  [pairs][N][M]   new_s [pairs][M]   end_s [pairs][N]
+ * bit-identical to stack `stack` of mmmot_affinity_fwd's outputs (every plan choice depends on (N, M) only).  The
+ * workspace is a third of mmmot_affinity_workspace's.  MMMOT_E_ARG for a stack outside 0..2. */
+size_t mmmot_affinity_stack_workspace(int pairs, int n, int m);
+int mmmot_affinity_stack_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode,
+                             int pairs, int stack, int n, int m, const float* feats,
+                             float* link, float* new_s, float* end_s,
+                             void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Association integer programme for 2-frame pairs, solved exactly as a rectangular

@@ -121,8 +121,12 @@ SIGNATURES = {
     "mmmot_pointnet_fwd": (_i, [_wp, _vp, _vp, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "mmmot_fusion_det_workspace": (_sz, [_i, _i]),
     "mmmot_fusion_det_fwd": (_i, [_wp, _i, _i, _f, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "mmmot_fusion_det_stack_workspace": (_sz, [_i, _i]),
+    "mmmot_fusion_det_stack_fwd": (_i, [_wp, _i, _i, _f, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "mmmot_affinity_workspace": (_sz, [_i, _i, _i]),
     "mmmot_affinity_fwd": (_i, [_wp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "mmmot_affinity_stack_workspace": (_sz, [_i, _i, _i]),
+    "mmmot_affinity_stack_fwd": (_i, [_wp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "mmmot_crop_workspace": (_sz, [_i, _i]),
     "mmmot_crop_count": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
     "mmmot_crop_scatter": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _i, _vp, _vp, _sz, _vp]),

@@ -2,7 +2,8 @@
 // Replaces reference modules/gcn.py:68-82 (affinity_module.forward), modules/new_end.py:62-82
 // (NewEndIndicator_v2.forward, mode 'avg') and modules/tracking_net.py:106-126 (associate).
 //
-// Groups g = pair*3 + stack.  The pairwise tensor x[g][c][i][j] (reference gcn.py:13,24-27;
+// Groups g = pair*3 + stack (every stack), or g = pair when one stack runs alone: group g then reads feature block
+// g*3 + stack, and the stage does a third of the work.  The pairwise tensor x[g][c][i][j] (reference gcn.py:13,24-27;
 // 100.7 MB per pair at N=M=128) is generated inside the first contraction's operand producers and
 // never exists in HBM; affinity conv1.0 and new/end conv0 (both 512->512 on the same x) run as
 // ONE 512->1024 contraction.  On the tensor-core path (gemm_gen.cuh) the GroupNorm + ReLU between
@@ -262,9 +263,10 @@ struct AfWs {
   int *cnt, *gstart;
   double2 *part, *npart;
 };
-AfWs carve(MmArena& a, int pairs, int n, int m) {
+// G: groups (3 per pair for every stack, 1 for one stack)
+AfWs carve(MmArena& a, size_t G, int n, int m) {
   AfWs w;
-  size_t G = (size_t)pairs * 3, NM = (size_t)n * m, ldv = G * (n + m);
+  size_t NM = (size_t)n * m, ldv = G * (n + m);
   w.y01 = a.take<float>(G * 1024 * NM);
   w.y2 = a.take<float>(G * 512 * NM);
   w.y3 = a.take<float>(G * 128 * NM);
@@ -303,14 +305,20 @@ int launch_gen(const GemmP& p, const mmmot_weights* wts, int wid, const float* s
 
 extern "C" size_t mmmot_affinity_workspace(int pairs, int n, int m) {
   MmArena a(nullptr, 0);
-  carve(a, pairs, n, m);
+  carve(a, (size_t)pairs * 3, n, m);
+  return a.off;
+}
+
+extern "C" size_t mmmot_affinity_stack_workspace(int pairs, int n, int m) {
+  MmArena a(nullptr, 0);
+  carve(a, (size_t)pairs, n, m);
   return a.off;
 }
 
 // mmmot_debug_stage_layout, stage 0: where mmmot_affinity_fwd leaves its intermediates (a dry carve; no CUDA call)
 int mm_affinity_layout(int pairs, int n, int m, size_t* off, int* tensor_cores) {
   MmArena a(nullptr, 0);
-  const AfWs w = carve(a, pairs, n, m);
+  const AfWs w = carve(a, (size_t)pairs * 3, n, m);
   const void* const bufs[31] = {w.y01, w.y3, w.z, w.fcl, w.sc0, w.sh0, w.sc3, w.sh3,
                                 w.v, w.h2, w.nsc2, w.nsh2, w.rmax, w.rsum, w.cmax, w.csum,
                                 w.y2, w.sc1, w.sh1, w.sc2, w.sh2, w.h1, w.nsc1, w.nsh1,
@@ -320,19 +328,27 @@ int mm_affinity_layout(int pairs, int n, int m, size_t* off, int* tensor_cores) 
   return 0;
 }
 
-extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs,
-                                  int n, int m, const float* feats, float* link, float* new_s,
-                                  float* end_s, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!wts || !feats || !link || !new_s || !end_s || !workspace || pairs <= 0 || n <= 0 || m <= 0)
+namespace {
+
+// The stage on every stack (stack < 0: G = 3*pairs groups, group g reads feature block g) or on one (G = pairs, group g
+// reads block g*3 + stack).  Every plan choice depends on the per-pair shape only, so a group's results do not depend on
+// which of the two it runs in.
+int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs, int stack,
+                       int n, int m, const float* feats, float* link, float* new_s, float* end_s, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  if (!wts || !feats || !link || !new_s || !end_s || !workspace || pairs <= 0 || n <= 0 || m <= 0 || stack > 2)
     return MMMOT_E_ARG;
   if (affinity_op < 0 || affinity_op > MMMOT_AFF_MINUS || softmax_mode < 0 || softmax_mode > MMMOT_SM_DUAL_MAX ||
       end_mode < MMMOT_END_AVG || end_mode > MMMOT_END_MAX)
     return MMMOT_E_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   MmArena ar(workspace, workspace_bytes);
-  AfWs w = carve(ar, pairs, n, m);
+  const int G = stack < 0 ? pairs * 3 : pairs, NM = n * m, L = n + m;
+  AfWs w = carve(ar, (size_t)G, n, m);
   if (!ar.ok()) return MMMOT_E_WORKSPACE;
-  const int G = pairs * 3, NM = n * m, L = n + m;
+  // group g's feature block [512][L]: fbase + g*fgs
+  const float* fbase = stack < 0 ? feats : feats + (long)stack * 512 * L;
+  const long fgs = (stack < 0 ? 1L : 3L) * 512 * L;
   const bool use_tc = affinity_use_tc(n, m);
   const int tpg = mm_cdiv(NM, use_tc ? tc::BN : 128);
   const float* const* W = wts->w;
@@ -342,9 +358,10 @@ extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int
   // FP32 engine: y01[g][1024][NM].  Tensor-core engine: channels-last y01[g*NM + s][1024].
   const int pm = use_tc ? 2 : 1;   // GroupNorm partials per column tile
   if (use_tc) {
-    MM_TRY(transpose_f32(feats, w.fcl, 512, L, G, st));
-    feats_range_kernel<<<148, 256, 0, st>>>(feats, (long)G * 512 * L, affinity_op == MMMOT_AFF_MULTIPLY ? 255.9f : 65504.f,
-                                           ar.status());
+    MM_TRY(transpose_f32(fbase, w.fcl, 512, L, G, fgs, st));
+    // every stack: one contiguous range; one stack: a block per pair
+    feats_range_kernel<<<148, 256, 0, st>>>(fbase, stack < 0 ? (long)G * 512 * L : 512L * L, stack < 0 ? 1 : G, fgs,
+                                           affinity_op == MMMOT_AFF_MULTIPLY ? 255.9f : 65504.f, ar.status());
     MM_LAUNCH_CHECK();
     GemmP p = gemm_defaults();
     p.bias = W[MMMOT_W_AF_B01]; p.M = 1024; p.K = 512;
@@ -363,7 +380,7 @@ extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int
     GemmP p = gemm_defaults();
     p.Wt = W[MMMOT_W_AF_W01T]; p.bias = W[MMMOT_W_AF_B01]; p.ldw = 1024; p.M = 1024; p.K = 512;
     p.S = NM; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
-    p.X = feats; p.n = n; p.m = m; p.Lf = L;
+    p.X = fbase; p.x_gs = fgs; p.n = n; p.m = m; p.Lf = L;
     p.Y = w.y01; p.y_gs = 1024L * NM; p.y_ms = NM;
     p.part = w.part;
     int r = affinity_op == MMMOT_AFF_MULTIPLY    ? gemm_simt_launch<XM_PAIR_MUL>(p, st)
@@ -492,4 +509,22 @@ extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int
     MM_LAUNCH_CHECK();
   }
   return 0;
+}
+
+}  // namespace
+
+extern "C" int
+mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs,
+                                  int n, int m, const float* feats, float* link, float* new_s,
+                                  float* end_s, void* workspace, size_t workspace_bytes, void* stream) {
+  return mmmot_affinity_fwd(wts, affinity_op, softmax_mode, end_mode, pairs, -1, n, m, feats, link, new_s, end_s, workspace,
+                      workspace_bytes, stream);
+}
+
+extern "C" int mmmot_affinity_stack_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs,
+                                        int stack, int n, int m, const float* feats, float* link, float* new_s, float* end_s,
+                                        void* workspace, size_t workspace_bytes, void* stream) {
+  if (stack < 0 || stack > 2) return MMMOT_E_ARG;
+  return mmmot_affinity_fwd(wts, affinity_op, softmax_mode, end_mode, pairs, stack, n, m, feats, link, new_s, end_s, workspace,
+                      workspace_bytes, stream);
 }

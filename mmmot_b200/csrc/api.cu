@@ -211,6 +211,7 @@ extern "C" int mmmot_debug_simt_op(int mode, int M, int K, const float* Wt, cons
     p.S = S; p.tiles_per_group = mm_cdiv(S, 128); p.num_tiles = p.tiles_per_group * groups;
   }
   p.X = X; p.x_gs = x_gs; p.x_ks = x_ks; p.sc = sc; p.sh = sh;
+  if (pair) p.x_gs = (long)K * Lf;   // the pairwise groups of F = X [groups][K][Lf] are packed
   p.n = n; p.m = m; p.Lf = Lf;
   p.H = H; p.W = W; p.Cin = Cin;
   p.addend = addend; p.seg = seg; p.ld_add = ld_add;

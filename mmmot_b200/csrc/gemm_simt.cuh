@@ -5,7 +5,8 @@
 //   XM_NORM_RELU  Xin = relu(X[g][k][s]*sc[g][k] + sh[g][k])     (GroupNorm+ReLU of the producer layer,
 //                                                                folded into the consumer's load)
 //   XM_PAIR_*     Xin = f[g][k][i] (*|-) f[g][k][n+j], s = i*m + j  (reference modules/gcn.py:6-41;
-//                                                                the 3xDxNxM tensor is never stored)
+//                                                                the 3xDxNxM tensor is never stored);
+//                 f[g] = X + g*x_gs, [K][Lf]
 //   XM_CONV3      Xin = im2col of a 3x3 / pad 1 convolution, k = (ky*3+kx)*Cin + ci, s = (img,y,x)
 // and a fused epilogue: bias, optional per-(detection) addend, optional ReLU, optional
 // per-(tile, channel) sum / sum-of-squares partials for the following GroupNorm (fp64, reduced in a
@@ -36,7 +37,7 @@ struct GemmP {
   long x_gs, x_ks;
   const float* sc;  // [G][K]
   const float* sh;
-  // pair generator: F[g][K][Lf], objs = columns [0,n), dets = columns [n, n+m)
+  // pair generator: F[g] = X + g*x_gs, [K][Lf]; objs = columns [0,n), dets = columns [n, n+m)
   int n, m, Lf;
   // conv3x3: X = in[img][Cin][H][W], Y = out[img][M][H][W]; S = n_img*H*W in one group
   int H, W, Cin;
@@ -162,7 +163,7 @@ __global__ void __launch_bounds__(256, 2) gemm_simt_kernel(const GemmP p) {
           rb[h * 4 + r] = v;
         }
       } else {
-        const float* fr = p.X + ((long)g * p.K + (kok ? k : 0)) * p.Lf;
+        const float* fr = p.X + (long)g * p.x_gs + (long)(kok ? k : 0) * p.Lf;
 #pragma unroll
         for (int r = 0; r < 4; r++) {
           float v = 0.f;

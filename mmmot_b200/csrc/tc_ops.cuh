@@ -42,12 +42,13 @@ static inline int norm_split(const float* in, long ldi, const float* sc, const f
   return 0;
 }
 
-// dst[g][col][row] = src[g][row][col]   (small matrices: feature stacks 512 x L, U 512 x ndet)
+// dst[g][col][row] = src[g*src_gs + row*cols + col]   (small matrices: feature stacks 512 x L, U 512 x ndet); src_gs =
+// rows*cols for packed groups, larger to pick one block out of every few (one feature stack of each pair)
 static __global__ void transpose_kernel(const float* __restrict__ src, float* __restrict__ dst, int rows, int cols,
-                                        int groups) {
+                                        long src_gs) {
   __shared__ float tile[32][33];
   const int g = blockIdx.z;
-  const float* s = src + (long)g * rows * cols;
+  const float* s = src + (long)g * src_gs;
   float* d = dst + (long)g * rows * cols;
   const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
@@ -60,19 +61,20 @@ static __global__ void transpose_kernel(const float* __restrict__ src, float* __
     if (r < rows && c < cols) d[(long)c * rows + r] = tile[threadIdx.x][i];
   }
 }
-static inline int transpose_f32(const float* src, float* dst, int rows, int cols, int groups, cudaStream_t st) {
+static inline int transpose_f32(const float* src, float* dst, int rows, int cols, int groups, long src_gs, cudaStream_t st) {
   dim3 grid(mm_cdiv(cols, 32), mm_cdiv(rows, 32), groups), block(32, 8);
-  transpose_kernel<<<grid, block, 0, st>>>(src, dst, rows, cols, groups);
+  transpose_kernel<<<grid, block, 0, st>>>(src, dst, rows, cols, src_gs);
   MM_LAUNCH_CHECK();
   return 0;
 }
 
 // Range guard of the pairwise producers (gemm_gen.cuh GEN_PAIR_*), which convert f_i (*|-) f_j to FP16 hi/lo unseen:
 // flag the status word when a feature is large enough for the op to reach 65504 (|f| >= 255.9 for the product,
-// |f| >= 65504 for the differences).  feats [n] fp32.
-static __global__ void feats_range_kernel(const float* __restrict__ f, long n, float limit, int* status) {
+// |f| >= 65504 for the differences).  Scans f[g*gs + i], g < groups, i < n (fp32).
+static __global__ void feats_range_kernel(const float* __restrict__ f, long n, int groups, long gs, float limit, int* status) {
   float amax = 0.f;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
-    amax = fmaxf(amax, fabsf(f[i]));
+  for (int g = 0; g < groups; g++)
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
+      amax = fmaxf(amax, fabsf(f[g * gs + i]));
   if (status && !(amax < limit)) atomicOr(status, 1);
 }

@@ -14,6 +14,7 @@ import os
 import numpy as np
 import torch
 
+from ._lib import MmmotError
 from .solvers import ortools_solve
 
 _FIELDS = ("name", "truncated", "occluded", "alpha", "bbox", "dimensions", "location", "rotation_y")
@@ -102,9 +103,21 @@ class TrackingModule(object):
         """tracking_model.py:68-81: forward -> assignment programme on the ``test_mode`` stack -> ids.
 
         Samples of K > 2 frames pass every transition's link matrix to the programme.  (The reference passes only
-        ``link_score[0]`` and fails there with a KeyError, solvers.py:91.)"""
-        det_score, link_score, new_score, end_score, _ = self.model(det_imgs, det_info, det_split)
+        ``link_score[0]`` and fails there with a KeyError, solvers.py:91.)
+
+        With one sensor missing (det_imgs None, or det_info without points, as the reference's 2-D loader gives it:
+        det_info = []) the ``test_mode`` stack is computed alone (``forward_stack``) when it does not need that sensor;
+        otherwise MmmotError names the missing sensor."""
+        has_points = bool(det_info) and "points" in det_info
         t = self.test_mode
+        if det_imgs is None or not has_points:
+            missing = self.model._missing_sensor(t, det_imgs is not None, has_points)
+            if missing is not None:
+                raise MmmotError(f"test_mode {t} needs the {missing} input, which was not given")
+            det_score, link_score, new_score, end_score, _ = self.model.forward_stack(det_imgs, det_info, det_split, t)
+            t = 0
+        else:
+            det_score, link_score, new_score, end_score, _ = self.model(det_imgs, det_info, det_split)
         if len(det_split) == 2:
             assign_det, assign_link, assign_new, assign_end = ortools_solve(
                 det_score[t], [link_score[0][t:t + 1]], new_score[t], end_score[t], det_split)

@@ -11,6 +11,8 @@ module lives on a CUDA device and the shared library loads.
 New relative to the reference (which handles one frame-pair per call, SURVEY F12):
 ``forward_batch`` runs B independent frame-pairs in one pass with per-pair semantics identical
 to ``forward``, and ``predict_batch`` also solves the association programme on the device.
+``forward_stack`` and the ``stack`` argument of ``forward_batch`` / ``predict_batch`` compute one
+feature stack alone (image, LiDAR or fused), so a tracker runs without the sensor it does not read.
 """
 import ctypes
 
@@ -23,6 +25,10 @@ from .schema import BUFFER_KINDS, RESNET_BLOCKS, VGG_POOL_AFTER, VGG_STAGES, WID
 # conv k of the 13 is followed by a 2x2 max-pool (so the map of conv k+1 is 4x smaller)
 VGG_POOLED_BEFORE = [idx in VGG_POOL_AFTER[s] for s, stage in enumerate(VGG_STAGES) for idx, _, _ in stage]
 from .weights import DeviceWeights
+
+
+STACKS = (0, 1, 2)                     # 0: image, 1: LiDAR, 2: fused (tracking_net.py:40)
+SENSORS = ("image", "LiDAR")
 
 
 def _vp(t):
@@ -175,29 +181,37 @@ class TrackingNet(nn.Module):
         return self._ws
 
     # ------------------------------------------------------------------ core
-    def _workspace_bytes(self, pairs, transitions, L=0, P=0, H=0, W=0):
+    def _workspace_bytes(self, pairs, transitions, L=0, P=0, H=0, W=0, stack=None):
         """Workspace of one call on `pairs` samples: the affinity stage on every (n, m) of `transitions` and, when L > 0,
-        the feature stages on L detections, P points and H x W crops (their training variants in training mode)."""
+        the feature stages on L detections, P points and H x W crops (their training variants in training mode).
+        stack: None for every stack, else the one stack computed (the stages it does not need are left out)."""
         lib = _lib.load()
-        need = [lib.mmmot_affinity_workspace(pairs, n, m) for n, m in transitions]
+        aff = lib.mmmot_affinity_workspace if stack is None else lib.mmmot_affinity_stack_workspace
+        need = [aff(pairs, n, m) for n, m in transitions]
         if L:
             if self.training:
                 need += [lib.mmmot_appearance_train_workspace(pairs * L, H, W), lib.mmmot_pointnet_train_workspace(pairs, L, P),
                          lib.mmmot_w_det_train_workspace(L)]
             else:
-                if self.appear_arch == "vgg":
-                    app = lib.mmmot_appearance_workspace(pairs * L, H, W)
+                if stack == 1:
+                    pass                    # the LiDAR stack alone: no appearance trunk
+                elif self.appear_arch == "vgg":
+                    need.append(lib.mmmot_appearance_workspace(pairs * L, H, W))
                 elif self.appear_head == "fpn":
-                    app = lib.mmmot_appearance_resnet_fpn_workspace(pairs * L, H, W, L)
+                    need.append(lib.mmmot_appearance_resnet_fpn_workspace(pairs * L, H, W, L))
                 else:
-                    app = lib.mmmot_appearance_resnet_workspace(pairs * L, H, W)
-                need += [app, lib.mmmot_pointnet_workspace(pairs, L, P)]
-            need.append(lib.mmmot_fusion_det_workspace(pairs, L))
+                    need.append(lib.mmmot_appearance_resnet_workspace(pairs * L, H, W))
+                if stack != 0:
+                    need.append(lib.mmmot_pointnet_workspace(pairs, L, P))
+            need.append(lib.mmmot_fusion_det_workspace(pairs, L) if stack is None else
+                        lib.mmmot_fusion_det_stack_workspace(pairs, L))
         return max(need)
 
-    def _features(self, wts, ws, st, crops, points, split, pairs, L, feats, det):
+    def _features(self, wts, ws, st, crops, points, split, pairs, L, feats, det, stack=None):
         """Appearance, PointNet and fusion / detection score of `pairs` samples of L detections on stream `st`:
         feats pairs x 3 x 512 x L, det pairs x 3 x L.  split: the CSR point offsets, CPU int32.
+        With `stack` (eval mode) only that stack is computed, det is pairs x 1 x L, and the input it does not need may
+        be None: the appearance trunk is skipped for the LiDAR stack (1), PointNet for the image stack (0).
 
         In training mode (reference TrackingNet.forward with self.training, modules/tracking_net.py:152-162) the
         BatchNorm layers (VGG trunk, w_det) normalise with the statistics of this call and det scores are raw logits
@@ -207,7 +221,7 @@ class TrackingNet(nn.Module):
         (bn_vgg 13 x 2 x 512, bn_det 2 x 2 x 512) in training mode, else None."""
         lib = _lib.load()
         dev = feats.device
-        H, W = crops.shape[-2:]
+        H, W = crops.shape[-2:] if crops is not None else (0, 0)
         wsp, wsn = _vp(ws), ctypes.c_size_t(ws.numel())
         train = self.training
         if train:
@@ -222,6 +236,8 @@ class TrackingNet(nn.Module):
             bn_det = torch.zeros(2, 2, 512, device=dev)
             _lib.check(lib.mmmot_appearance_train_fwd(wts.ptr, _vp(crops), pairs * L, H, W, L, _vp(feats), _vp(bn_vgg), _vp(dm2),
                                                       _vp(dm3), wsp, wsn, st), "mmmot_appearance_train_fwd")
+        elif stack == 1:
+            pass                            # the LiDAR stack alone: no appearance trunk
         elif wts.fpn is not None:
             _lib.check(lib.mmmot_appearance_resnet_fpn_fwd(wts.rptr, wts.fptr, _vp(crops), pairs * L, H, W, L, _vp(feats), wsp,
                                                            wsn, st), "mmmot_appearance_resnet_fpn_fwd")
@@ -231,28 +247,37 @@ class TrackingNet(nn.Module):
         else:
             _lib.check(lib.mmmot_appearance_fwd(wts.ptr, _vp(crops), pairs * L, H, W, L, _vp(feats), wsp, wsn, st),
                        "mmmot_appearance_fwd")
-        split_dev = self._split_to_device(split, dev)
-        hs = ctypes.c_void_p(split.numpy().ctypes.data)
-        if train:
-            _lib.check(lib.mmmot_pointnet_train_fwd(wts.ptr, _vp(points), _vp(split_dev), hs, pairs, L, _vp(hmask), _vp(feats),
-                                                    wsp, wsn, st), "mmmot_pointnet_train_fwd")
-        else:
-            _lib.check(lib.mmmot_pointnet_fwd(wts.ptr, _vp(points), _vp(split_dev), hs, pairs, L, _vp(feats), wsp, wsn, st),
-                       "mmmot_pointnet_fwd")
+        if stack != 0:                      # the image stack alone needs no PointNet
+            split_dev = self._split_to_device(split, dev)
+            hs = ctypes.c_void_p(split.numpy().ctypes.data)
+            if train:
+                _lib.check(lib.mmmot_pointnet_train_fwd(wts.ptr, _vp(points), _vp(split_dev), hs, pairs, L, _vp(hmask),
+                                                        _vp(feats), wsp, wsn, st), "mmmot_pointnet_train_fwd")
+            else:
+                _lib.check(lib.mmmot_pointnet_fwd(wts.ptr, _vp(points), _vp(split_dev), hs, pairs, L, _vp(feats), wsp, wsn, st),
+                           "mmmot_pointnet_fwd")
         flags, thr = (0, 0.0) if train else (self._score_flags(), float(self.neg_threshold))
-        _lib.check(lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[self.score_fusion_arch], flags, thr, pairs, L, _vp(feats),
-                                            _vp(det), wsp, wsn, st), "mmmot_fusion_det_fwd")
+        if stack is None:
+            _lib.check(lib.mmmot_fusion_det_fwd(wts.ptr, _lib.FUSION[self.score_fusion_arch], flags, thr, pairs, L, _vp(feats),
+                                                _vp(det), wsp, wsn, st), "mmmot_fusion_det_fwd")
+        else:
+            _lib.check(lib.mmmot_fusion_det_stack_fwd(wts.ptr, _lib.FUSION[self.score_fusion_arch], flags, thr, pairs, L, stack,
+                                                      _vp(feats), _vp(det), wsp, wsn, st), "mmmot_fusion_det_stack_fwd")
         if not train:
             return None
         _lib.check(lib.mmmot_w_det_train_fwd(wts.ptr, L, _vp(feats), _vp(det), _vp(bn_det), wsp, wsn, st), "mmmot_w_det_train_fwd")
         return bn_vgg, bn_det
 
-    def _associate(self, wts, ws, st, pairs, n, m, feats, link, new, end):
+    def _associate(self, wts, ws, st, pairs, n, m, feats, link, new, end, stack=None):
         """Affinity / start-end / softmax stage on stream `st`: feats pairs x 3 x 512 x (n+m), contiguous ->
-        link pairs x 3 x n x m, new pairs x 3 x m, end pairs x 3 x n."""
-        _lib.check(_lib.load().mmmot_affinity_fwd(wts.ptr, _lib.AFFINITY[self.affinity_op], _lib.SOFTMAX.get(self.softmax_mode, 0),
-                                                  _lib.END_MODE[self.end_mode], pairs, n, m, _vp(feats), _vp(link), _vp(new),
-                                                  _vp(end), _vp(ws), ctypes.c_size_t(ws.numel()), st), "mmmot_affinity_fwd")
+        link pairs x 3 x n x m, new pairs x 3 x m, end pairs x 3 x n; with `stack`, that stack alone (size-1 stack axis)."""
+        lib = _lib.load()
+        mode = (_lib.AFFINITY[self.affinity_op], _lib.SOFTMAX.get(self.softmax_mode, 0), _lib.END_MODE[self.end_mode])
+        tail = (_vp(feats), _vp(link), _vp(new), _vp(end), _vp(ws), ctypes.c_size_t(ws.numel()), st)
+        if stack is None:
+            _lib.check(lib.mmmot_affinity_fwd(wts.ptr, *mode, pairs, n, m, *tail), "mmmot_affinity_fwd")
+        else:
+            _lib.check(lib.mmmot_affinity_stack_fwd(wts.ptr, *mode, pairs, stack, n, m, *tail), "mmmot_affinity_stack_fwd")
 
     def _score_flags(self):
         """reference tracking_net.py:153-162: sigmoid only when 'cls' is in score_arch; the neg_threshold step is
@@ -272,18 +297,40 @@ class TrackingNet(nn.Module):
         if int(status) & 1:
             _lib.check(-4, "mmmot_b200.TrackingNet forward")
 
-    def _pick_chunk(self, B, n, m, P_per_pair, H, W, dev):
+    def _pick_chunk(self, B, n, m, P_per_pair, H, W, dev, stack=None):
         if self.chunk_pairs:
             return min(B, self.chunk_pairs)
         free, _ = torch.cuda.mem_get_info(dev)
         budget = min(free * 0.5, 48e9)
         c = B
-        while c > 1 and self._workspace_bytes(c, [(n, m)], n + m, int(P_per_pair * c) + 1, H, W) > budget:
+        while c > 1 and self._workspace_bytes(c, [(n, m)], n + m, int(P_per_pair * c) + 1, H, W, stack) > budget:
             c = (c + 1) // 2
         return c
 
+    @staticmethod
+    def _check_stack(stack):
+        if stack is not None and stack not in STACKS:
+            raise ValueError(f"stack must be None or one of {STACKS} (0 image, 1 LiDAR, 2 fused), got {stack!r}")
+
+    @staticmethod
+    def _missing_sensor(stack, have_image, have_points):
+        """The sensor whose input the stack `stack` (None: every stack) needs and lacks, or None."""
+        if stack != 1 and not have_image:
+            return SENSORS[0]
+        if stack != 0 and not have_points:
+            return SENSORS[1]
+        return None
+
+    def _require(self, stack, have_image, have_points):
+        """Eval-mode single-stack calls: the stack's inputs must be given (MmmotError names the missing sensor)."""
+        if self.training:
+            raise NotImplementedError("mmmot_b200.TrackingNet: the single-stack forward is eval mode only")
+        missing = self._missing_sensor(stack, have_image, have_points)
+        if missing is not None:
+            raise _lib.MmmotError(f"stack {stack} needs the {missing} input, which was not given")
+
     @torch.no_grad()
-    def forward_batch(self, crops, points, points_split, n, m=None, keep_feats=False, check=True):
+    def forward_batch(self, crops, points, points_split, n, m=None, keep_feats=False, check=True, stack=None):
         """B independent frame-pairs, each with n previous and m next detections.
 
         crops         (B*(n+m)) x 3 x H x W  fp32, CUDA
@@ -297,53 +344,67 @@ class TrackingNet(nn.Module):
                       status word (int32 device tensor; bit 0 = an activation left FP16's range, MMMOT_E_RANGE).
         check=True (default) reads the status word back (one host sync) and raises MmmotError when it is set;
         pipelined callers pass check=False and test ``out["status"]`` together with the results they copy back.
+
+        stack (None: every stack): 0, 1 or 2 computes that stack alone, bit-identical to forward_batch()[:, stack:stack+1]:
+        the appearance trunk is skipped for 1 (LiDAR) and PointNet for 0 (image), and the input the stack does not need
+        may be None (crops for 1; points and points_split for 0).  The returned tensors keep a stack axis of size 1.
         """
+        self._check_stack(stack)
         if self.training:
             raise NotImplementedError("mmmot_b200.TrackingNet implements the eval-mode forward only (SURVEY §8f N4)")
         m = n if m is None else m
         L = n + m
-        self._check_points(points)
+        use_img, use_pts = stack != 1, stack != 0
+        if stack is not None:
+            self._require(stack, crops is not None, points is not None and points_split is not None)
+        if use_pts:
+            self._check_points(points)
         lib = _lib.load()
         wts = self.prepared()
         dev = wts.flat.device
-        if crops.device != dev or points.device != dev:
+        if (use_img and crops.device != dev) or (use_pts and points.device != dev):
             raise _lib.MmmotError("inputs must live on the module's CUDA device")
-        crops = crops.contiguous().float()
-        points = _aligned_rows(points.contiguous().float())
-        split = points_split.detach().to("cpu", torch.int32).contiguous()
-        if crops.shape[0] % L or split.numel() != crops.shape[0] + 1:
+        crops = crops.contiguous().float() if use_img else None
+        points = _aligned_rows(points.contiguous().float()) if use_pts else None
+        split = points_split.detach().to("cpu", torch.int32).contiguous() if use_pts else None
+        rows = crops.shape[0] if use_img else split.numel() - 1
+        if rows % L or (use_pts and split.numel() != rows + 1):
             raise _lib.MmmotError("crops / points_split do not match n, m")
-        B = crops.shape[0] // L
-        H, W = crops.shape[-2:]
+        B = rows // L
+        H, W = crops.shape[-2:] if use_img else (0, 0)
+        ns = 3 if stack is None else 1
         out = {
             "status": torch.zeros(1, dtype=torch.int32, device=dev),
             "feats": torch.empty(B, 3, 512, L, device=dev),
-            "det": torch.empty(B, 3, L, device=dev),
-            "link": torch.empty(B, 3, n, m, device=dev),
-            "new": torch.empty(B, 3, m, device=dev),
-            "end": torch.empty(B, 3, n, device=dev),
+            "det": torch.empty(B, ns, L, device=dev),
+            "link": torch.empty(B, ns, n, m, device=dev),
+            "new": torch.empty(B, ns, m, device=dev),
+            "end": torch.empty(B, ns, n, device=dev),
         }
         with torch.cuda.device(dev):        # the library works on the CURRENT device
             st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            chunk = self._pick_chunk(B, n, m, int(split[-1]) / B, H, W, dev)
+            chunk = self._pick_chunk(B, n, m, int(split[-1]) / B if use_pts else 0, H, W, dev, stack)
             for p0 in range(0, B, chunk):
                 pc = min(chunk, B - p0)
-                s_host = split[p0 * L:(p0 + pc) * L + 1]
-                off = int(s_host[0])
-                s_host = (s_host - off).contiguous()
-                P = int(s_host[-1])
-                ws = self._workspace(self._workspace_bytes(pc, [(n, m)], L, P, H, W), dev)
+                s_host, pts = None, None
+                if use_pts:
+                    s_host = split[p0 * L:(p0 + pc) * L + 1]
+                    off = int(s_host[0])
+                    s_host = (s_host - off).contiguous()
+                    pts = points[off:off + int(s_host[-1])]
+                P = int(s_host[-1]) if use_pts else 0
+                ws = self._workspace(self._workspace_bytes(pc, [(n, m)], L, P, H, W, stack), dev)
                 _lib.check(lib.mmmot_status_reset(_vp(ws), st), "mmmot_status_reset")
                 feats = out["feats"][p0:p0 + pc]
-                self._features(wts, ws, st, crops[p0 * L:(p0 + pc) * L], points[off:off + P], s_host, pc, L, feats,
-                               out["det"][p0:p0 + pc])
+                self._features(wts, ws, st, crops[p0 * L:(p0 + pc) * L] if use_img else None, pts, s_host, pc, L, feats,
+                               out["det"][p0:p0 + pc], stack)
                 self._associate(wts, ws, st, pc, n, m, feats, out["link"][p0:p0 + pc], out["new"][p0:p0 + pc],
-                                out["end"][p0:p0 + pc])
+                                out["end"][p0:p0 + pc], stack)
                 # the status word (FP16 range flag) of this chunk, accumulated into out["status"] in stream order
                 out["status"] |= ws[:4].view(torch.int32)
         out["trans"] = [wts.trans1.unsqueeze(0).clone(), wts.trans2.unsqueeze(0).clone()]
         if keep_feats:
-            out["feats"] = wts.narrow(out["feats"])
+            out["feats"] = wts.narrow(out["feats"] if stack is None else out["feats"][:, stack:stack + 1])
         else:
             del out["feats"]
         if check:
@@ -374,15 +435,17 @@ class TrackingNet(nn.Module):
         return link, new, end
 
     @torch.no_grad()
-    def predict_batch(self, crops, points, points_split, n, m=None, check=True):
+    def predict_batch(self, crops, points, points_split, n, m=None, check=True, stack=None):
         """forward_batch + association programme on the ``test_mode`` stack, all on the device.
-        Returns forward_batch's dict plus assign_{det,link,new,end} and match (B x n int32)."""
+        Returns forward_batch's dict plus assign_{det,link,new,end} and match (B x n int32).
+        stack: computes that stack alone (forward_batch's ``stack``) and solves the programme on it."""
         from .solvers import solve_batch
         m = n if m is None else m
-        out = self.forward_batch(crops, points, points_split, n, m, check=check)
-        B, t = out["det"].shape[0], self.test_mode
-        zn = out["det"].new_zeros(B, 3, n)
-        zm = out["det"].new_zeros(B, 3, m)
+        out = self.forward_batch(crops, points, points_split, n, m, check=check, stack=stack)
+        B, t = out["det"].shape[0], self.test_mode if stack is None else 0
+        ns = out["det"].shape[1]
+        zn = out["det"].new_zeros(B, ns, n)
+        zm = out["det"].new_zeros(B, ns, m)
         new_p = torch.cat([zn, out["new"]], dim=2)      # tracking_net.py:183-189 zero padding
         end_p = torch.cat([out["end"], zm], dim=2)
         out.update(solve_batch(out["det"][:, t], out["link"][:, t], new_p[:, t], end_p[:, t], n, m))
@@ -442,6 +505,23 @@ class TrackingNet(nn.Module):
         (tracking_net.py:183-192; see _features): raw det logits, new_scores 3 x m and end_scores 3 x n not zero-padded,
         and the BatchNorm layers' running averages are updated.  Forward only: no autograd graph is built through the
         CUDA library."""
+        return self._forward_sample(dets, det_info, dets_split, None)
+
+    @torch.no_grad()
+    def forward_stack(self, dets, det_info, dets_split, stack):
+        """``forward`` on one feature stack alone (0 image, 1 LiDAR, 2 fused), eval mode, for a tracker that reads only
+        that stack: the 5-tuple of ``forward`` with every score tensor holding stack ``stack`` only (det 1 x L, link
+        1 x n_k x n_k+1, new / end 1 x L, zero-padded as in ``forward``), bit-identical to ``forward``'s [stack:stack+1].
+        The absent sensor's input may be left out: dets may be None for stack 1; det_info may be None, [] or a dict
+        without 'points' for stack 0 (the reference's 2-D loader passes det_info = []).  The appearance trunk is skipped
+        for stack 1 and PointNet for stack 0."""
+        if stack not in STACKS:
+            raise ValueError(f"stack must be one of {STACKS} (0 image, 1 LiDAR, 2 fused), got {stack!r}")
+        self._require(stack, dets is not None, bool(det_info) and 'points' in det_info)
+        return self._forward_sample(dets, det_info, dets_split, stack)
+
+    def _forward_sample(self, dets, det_info, dets_split, stack):
+        """forward (stack None) and forward_stack."""
         splits = [int(s) for s in dets_split]
         if self.training and self.appear_arch != "vgg":
             raise NotImplementedError("mmmot_b200.TrackingNet: the training-mode forward (batch-statistics BatchNorm) "
@@ -453,37 +533,41 @@ class TrackingNet(nn.Module):
             raise NotImplementedError("mmmot_b200.TrackingNet supports 2-frame samples (sample_max_len: 2)")
         L = sum(splits)
         C = self.point_channels
-        raw = det_info['points']
-        if raw.dim() < 2 or raw.shape[-1] < C:
-            raise _lib.MmmotError(f"det_info['points'] must carry at least {C} columns per point for this net "
-                                  f"(without_reflectivity={C == 3}), got {list(raw.shape)}")
+        use_img, use_pts = stack != 1, stack != 0
+        if use_pts:
+            raw = det_info['points']
+            if raw.dim() < 2 or raw.shape[-1] < C:
+                raise _lib.MmmotError(f"det_info['points'] must carry at least {C} columns per point for this net "
+                                      f"(without_reflectivity={C == 3}), got {list(raw.shape)}")
         lib = _lib.load()
         if self.training:
             self._prepared = None                  # parameters move under an optimizer: re-derive the operands every step
         wts = self.prepared()
         dev = wts.flat.device
-        crops = dets.contiguous().float()
-        points = _aligned_rows(raw.reshape(-1, raw.shape[-1])[:, :C].contiguous().float())
-        split = det_info['points_split'].reshape(-1).detach().to("cpu", torch.int32).contiguous()
-        if (crops.device != dev or points.device != dev or crops.shape[0] != L or split.numel() != L + 1
+        crops = dets.contiguous().float() if use_img else None
+        points = _aligned_rows(raw.reshape(-1, raw.shape[-1])[:, :C].contiguous().float()) if use_pts else None
+        split = det_info['points_split'].reshape(-1).detach().to("cpu", torch.int32).contiguous() if use_pts else None
+        if ((use_img and (crops.device != dev or crops.shape[0] != L))
+                or (use_pts and (points.device != dev or split.numel() != L + 1))
                 or len(splits) < 2 or min(splits) <= 0):
             raise _lib.MmmotError("inputs do not match the module's device / dets_split")
-        H, W = crops.shape[-2:]
+        H, W = crops.shape[-2:] if use_img else (0, 0)
+        ns = 3 if stack is None else 1
         transitions = list(zip(splits[:-1], splits[1:]))
         feats = torch.empty(1, 3, 512, L, device=dev)
-        det = torch.empty(1, 3, L, device=dev)
+        det = torch.empty(1, ns, L, device=dev)
         links, news, ends = [], [], []
         with torch.cuda.device(dev):
             st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            ws = self._workspace(self._workspace_bytes(1, transitions, L, int(split[-1]), H, W), dev)
+            ws = self._workspace(self._workspace_bytes(1, transitions, L, int(split[-1]) if use_pts else 0, H, W, stack), dev)
             _lib.check(lib.mmmot_status_reset(_vp(ws), st), "mmmot_status_reset")
-            bn = self._features(wts, ws, st, crops, points, split, 1, L, feats, det)
+            bn = self._features(wts, ws, st, crops, points, split, 1, L, feats, det, stack)
             start = 0
             for a, b in transitions:
-                link = torch.empty(1, 3, a, b, device=dev)
-                new = torch.empty(1, 3, b, device=dev)
-                end = torch.empty(1, 3, a, device=dev)
-                self._associate(wts, ws, st, 1, a, b, feats[:, :, :, start:start + a + b].contiguous(), link, new, end)
+                link = torch.empty(1, ns, a, b, device=dev)
+                new = torch.empty(1, ns, b, device=dev)
+                end = torch.empty(1, ns, a, device=dev)
+                self._associate(wts, ws, st, 1, a, b, feats[:, :, :, start:start + a + b].contiguous(), link, new, end, stack)
                 links.append(link[0]); news.append(new[0]); ends.append(end[0])
                 start += a
             _lib.check(lib.mmmot_status_check(_vp(ws), st),
@@ -500,6 +584,6 @@ class TrackingNet(nn.Module):
             self._update_running("w_det.1", bn_det[0, 0, :512], bn_det[0, 1, :512], 3.0 * L)
             self._update_running("w_det.4", bn_det[1, 0, :256], bn_det[1, 1, :256], 3.0 * L)
             return det[0], links, news[0], ends[0], trans
-        new_scores = torch.cat([det.new_zeros(3, splits[0])] + news, dim=1)        # tracking_net.py:183-189
-        end_scores = torch.cat(ends + [det.new_zeros(3, splits[-1])], dim=1)
+        new_scores = torch.cat([det.new_zeros(ns, splits[0])] + news, dim=1)       # tracking_net.py:183-189
+        end_scores = torch.cat(ends + [det.new_zeros(ns, splits[-1])], dim=1)
         return det[0], links, new_scores, end_scores, trans
