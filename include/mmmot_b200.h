@@ -467,6 +467,8 @@ int mmmot_set_kseg(int chunks);
  *   bit 9 (512)  no fused max-pool in the conv epilogues (separate max-pool kernel)
  *   bit 10 (1024) generated-operand engine (csrc/gemm_gen.cuh): producers without the software pipeline, every GEN
  *                 (GEN_NORM: plain producers instead of TMA-staged source rows)
+ *   bit 11 (2048) channel-major conv epilogue through the accumulator image in shared memory instead of from the
+ *                 registers (mmmot_debug_conv_epilogue)
  *   bit 12 (4096) generated-operand engine: GEN_NORM producers with the software pipeline (prefetching variant)
  *                 instead of TMA-staged source rows
  *   bit 13 (8192) PointNet layers 3, 4 through norm_split + the TMA-fed kernel instead of GEN_NORM producers
@@ -582,7 +584,11 @@ int mmmot_debug_linear_planar(const void* Wp, float wp_scale, const float* bias,
  *   conv_layer (Wp1, its compact tiles Wpx1); kseg_scratch as conv_layer.  fused (host, or NULL) receives 1 if the single
  *   fused launch ran (it needs both compact tiles; debug bit 15 forces the two launches), 0 for the two launches.
  * vgg_conv01_plan: *fused (host) = whether vgg_conv01 of that shape takes the fused launch (given both compact tiles),
- *   computed on the host without any CUDA call under the current mmmot_set_debug / mmmot_set_kseg state. */
+ *   computed on the host without any CUDA call under the current mmmot_set_debug / mmmot_set_kseg state.
+ * conv_epilogue: the epilogue the channel-major kernel runs under that launch plan (same arguments as conv_plan): 1 =
+ *   from the wgmma accumulators in registers, stored by TMA; 0 = through the accumulator image in shared memory (debug
+ *   bit 11, K segments, M < 64) or the pixel-major kernel; computed on the host. */
+int mmmot_debug_conv_epilogue(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg);
 int mmmot_debug_conv_plan(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg, int* plan);
 int mmmot_debug_conv_layer(const void* Wp, const void* Wpx, float wp_scale, const float* bias, const void* Xhi, long x_plane,
                            int n_img, int H, int W, int C, int M, void* Yhi, long y_plane, long y_plane_pooled,

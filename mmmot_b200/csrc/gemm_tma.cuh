@@ -37,6 +37,12 @@ constexpr int T_STAGE_BYTES = A_SUB + 2 * B_HALF;
 constexpr size_t T_SMEM_BYTES = (size_t)T_STAGES * T_STAGE_BYTES + 1024 + 256 + T_EPI_WARPS * T_EPI_SCRATCH;
 static_assert(T_SMEM_BYTES <= 227 * 1024, "gemm_tma_kernel exceeds the 227 KB of shared memory per block");
 static_assert(T_STAGES * T_STAGE_BYTES >= 128 * BN * 4, "the accumulator image must fit in the ring it overlays");
+// Conv kernel with the epilogue from the accumulators (gemm_tma_kernel<true>): no accumulator image and no per-warp
+// scratch, but two staging buffers per consumer warpgroup, each [64-channel half of the m128 tile][32 pixels][128 B]
+// (FP16 hi in one, lo in the other, SWIZZLE_128B) that the TMA stores to the NHWC output planes.
+constexpr int T_STG_BUF = 2 * 32 * 128;
+constexpr size_t T_CONV_SMEM_BYTES = (size_t)T_STAGES * T_STAGE_BYTES + 2 * 2 * T_STG_BUF + 1024 + 256;
+static_assert(T_CONV_SMEM_BYTES <= 227 * 1024, "gemm_tma_kernel<true> exceeds the 227 KB of shared memory per block");
 
 enum { OUT_PLANAR = 3 };   // two FP16 planes Y_hi[row][y_ms], Y_lo = Y_hi + plane_elems (channels-last)
 
@@ -98,6 +104,26 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(mbar)
       : "memory");
 }
+// shared -> global box store (bulk async-group of the issuing thread); OOB elements of the box are not written
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// this thread's committed bulk stores have read their shared-memory source (read) / are complete
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// four 8x8 b16 matrices in mma fragment layout (thread (g, t) holds row g, columns 2t, 2t+1), stored transposed:
+// lane l gives the address of row l % 8 of matrix l / 8, which receives column l % 8 of the fragment
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void st_shared_u16(uint32_t addr, unsigned short v) {
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
+}
 // K-major SWIZZLE_64B operand: rows of 64 bytes (32 fp16), 8-row groups 512 B apart (SBO), layout type 2.
 __device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t saddr) {
   return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
@@ -137,14 +163,264 @@ __device__ __forceinline__ void pool_chunk(const float (&x)[32], float (&o)[8]) 
     }
 }
 
+// ---- main loop: one K segment (chunks [kc_lo, kc_hi)) of this warpgroup's 128 rows x 128 columns (column half `half`),
+// two m64n128 wgmma chains.  On return the accumulators are final and every ring stage they read has been released.
+__device__ __forceinline__ void mma_segment(float (&acc)[2][64], const TmaP& P, uint32_t base, uint32_t bar0, int half,
+                                            int lane, int kc_lo, int kc_hi, uint32_t& it) {
+  auto full_bar = [&](int s) { return bar0 + 8u * s; };
+  auto empty_bar = [&](int s) { return bar0 + 8u * (T_STAGES + s); };
+  // The first wgmma of each chain ignores the accumulators (scale_d = 0); clearing them here rather than once per
+  // CTA leaves them dead from the epilogue to the next item, so the epilogue has their registers (no spills).
+#pragma unroll
+  for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[mb][i] = 0.f;
+  for (int kc = kc_lo; kc < kc_hi; kc++, it++) {
+    const int s = it % T_STAGES;
+    mbar_wait(full_bar(s), (it / T_STAGES) & 1);
+    const uint32_t sa = base + s * T_STAGE_BYTES, sb = sa + A_SUB + half * (128 / 8) * 512;
+    if (!(P.t.dbg & 8)) {
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 2; ks++) {
+        const uint64_t b_hi = smem_desc_sw64(sb + ks * 32), b_lo = smem_desc_sw64(sb + B_HALF + ks * 32);
+#pragma unroll
+        for (int mb = 0; mb < 2; mb++) {
+          const uint32_t a = sa + mb * 8 * SBO + ks * 2 * A_LBO;
+          const uint64_t a_hi = smem_desc(a, A_LBO, SBO), a_lo = smem_desc(a + A_HALF, A_LBO, SBO);
+          wgmma_n128(acc[mb], a_hi, b_hi, ((kc - kc_lo) | ks) ? 1u : 0u);
+          wgmma_n128(acc[mb], a_hi, b_lo, 1u);
+          wgmma_n128(acc[mb], a_lo, b_hi, 1u);
+        }
+      }
+      wgmma_commit();
+    }
+    wgmma_wait<1>();   // the previous chunk's wgmmas are done: release its stage
+    if (kc > kc_lo) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar((it - 1) % T_STAGES)); }
+  }
+  wgmma_wait<0>();
+  fence_acc(acc[0]);
+  fence_acc(acc[1]);
+  __syncwarp();
+  if (lane == 0) mbar_arrive(empty_bar((it - 1) % T_STAGES));
+}
+
+__device__ __forceinline__ int opaque(int v) { asm volatile("" : "+r"(v)); return v; }
+
+// Origin (dx, dy, di) inside a box (BX, BY, BI) (powers of two, lbx / lby their logs) of the 32 consecutive columns
+// from column c0 (a multiple of 32), columns numbered (ii*BY + yy)*BX + xx.  Those 32 columns are themselves the box
+// (min(BX, 32), min(BY, 32 / min(BX, 32)), ...) that store_box_dims gives the output tensor maps.
+__device__ __forceinline__ void box_origin32(int c0, int BX, int BY, int lbx, int lby, int& dx, int& dy, int& di) {
+  const int r = c0 >> lbx;
+  dx = c0 & (BX - 1); dy = r & (BY - 1); di = r >> lby;
+}
+
+// Channel-major conv consumers of gemm_tma_kernel<true>: the epilogue runs on the wgmma fragments in registers.
+// Thread (warp w of warpgroup `half`, lane = 4g + t) holds, for m64 block mb and n8 block j, channels
+// mg*128 + mb*64 + 16w + {g, g+8} at columns half*128 + 8j + {2t, 2t+1}: acc[mb][4j + {0, 1}] and acc[mb][4j + {2, 3}].
+// Output: per 32 columns (or the 32 pooled pixels of a half) the FP16 hi and lo values go pixel-major into the
+// warpgroup's two staging buffers (stmatrix.trans, 128-byte swizzle) and one thread stores them by TMA through the
+// NHWC maps out_hi / out_lo, which clip partial boxes.  Only the warpgroup synchronises; the ring is never waited on.
+// Single-pass K only (conv_plan): K-segmented launches keep the accumulator-image epilogue of gemm_tma_kernel<false>.
+template <int BX>
+__device__ __forceinline__ void conv_pool_epi(const TmaP& P, const float (&x)[2][64], int half, int w, int lane, int mg,
+                                              int i0, int y0, int x0, int lby, float& amax, uint32_t buf) {
+  const GemmP& p = P.t.g;
+  const int g = lane >> 2, t = lane & 3;
+  constexpr int NS = BX >= 8 ? 8 : 16;   // pooled values per channel row of the thread
+  constexpr int BX8 = BX >= 8 ? BX / 8 : 1;
+  const int PBY = P.by >> 1, lpby = lby - 1;          // pooled box rows
+  const int Hp = P.H >> 1, Wp = P.W >> 1;
+  float run[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+  int cur = -1;                                        // image of the running sums
+  auto flush = [&]() {
+    // BX >= 4: the quad's four lanes hold the same channel and the same image, so they reduce to one atomic
+#pragma unroll
+    for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        float s = run[mb][h];
+        if (BX >= 4) { s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2); }
+        const int co = mg * 128 + mb * 64 + 16 * w + 8 * h + g;
+        if ((BX >= 4 ? t == 0 : !(t & 1)) && cur >= 0 && cur < P.n_img && co < p.M)
+          atomicAdd(P.pool_sum + (long)cur * p.M + co, __float2ull_rn(s * 4294967296.f));
+        run[mb][h] = 0.f;
+      }
+  };
+#pragma unroll
+  for (int J = 0; J < NS; J++) {
+    // pooled column pc (0..31 in the half, numbered like the columns in the pooled box (BX/2, by/2, bi)) and the
+    // window's maximum for the thread's four channel rows
+    float v[2][2];
+    int pc;
+    bool own = true;
+#pragma unroll
+    for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        if (BX >= 8) {   // vertical partner: the same thread's n8 block BX/8 further on
+          const int j = (J / BX8) * (BX / 4) + J % BX8, jp = j + BX8;
+          v[mb][h] = fmaxf(fmaxf(x[mb][4 * j + 2 * h], x[mb][4 * j + 2 * h + 1]),
+                           fmaxf(x[mb][4 * jp + 2 * h], x[mb][4 * jp + 2 * h + 1]));
+        } else {         // vertical partner: lane ^ 2 (BX = 4) or lane ^ 1 (BX = 2) of the same n8 block
+          const float hm = fmaxf(x[mb][4 * J + 2 * h], x[mb][4 * J + 2 * h + 1]);
+          v[mb][h] = fmaxf(hm, __shfl_xor_sync(0xffffffffu, hm, BX == 4 ? 2 : 1));
+        }
+      }
+    if (BX >= 8) pc = 4 * J + t;
+    else if (BX == 4) { pc = 2 * J + (t & 1); own = t < 2; }
+    else { pc = 2 * J + (t >> 1); own = !(t & 1); }
+    // pooled pixel -> (image, y, x) of the pooled map
+    const int c = half * 32 + pc;
+    const int r = c / (BX / 2);
+    const int pimg = i0 + (r >> lpby), py = (y0 >> 1) + (r & (PBY - 1)), px = (x0 >> 1) + c % (BX / 2);
+    const bool ok = own && pimg < P.n_img && py < Hp && px < Wp;
+#pragma unroll
+    for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int ch = 16 * w + 8 * h + g;
+        if (mg * 128 + mb * 64 + ch < p.M) amax = fmaxf(amax, fabsf(v[mb][h]));
+        if (own) {
+          __half hi, lo;
+          split_f16(v[mb][h], hi, lo);
+          const uint32_t a = buf + mb * 4096 + pc * 128 + ((((ch >> 3) ^ (pc & 7)) << 4) | ((ch & 7) << 1));
+          st_shared_u16(a, __half_as_ushort(hi));
+          st_shared_u16(a + T_STG_BUF, __half_as_ushort(lo));
+        }
+      }
+    if (P.pool_sum) {
+      if (pimg != cur) {   // warp-uniform for BX >= 4 (one image per quad and J); BX = 2 flushes without shuffles
+        flush();
+        cur = pimg;
+      }
+#pragma unroll
+      for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+        for (int h = 0; h < 2; h++) run[mb][h] += ok ? v[mb][h] : 0.f;
+    }
+  }
+  if (P.pool_sum) flush();
+}
+
+__device__ __forceinline__ void conv_acc_consumer(const TmaP& P, uint32_t base, uint32_t bar0, const CUtensorMap* out_hi,
+                                                  const CUtensorMap* out_lo) {
+  const GemmP& p = P.t.g;
+  const int tid = threadIdx.x, half = tid >> 7;
+  const bool elected = (tid & 127) == 0;
+  const uint32_t stg = base + T_STAGES * T_STAGE_BYTES + half * 2 * T_STG_BUF;   // hi buffer; lo = hi + T_STG_BUF
+  const int KC = P.t.k_chunks, mgroups = P.t.m_tiles;
+  const long total_tiles = (long)p.num_tiles * mgroups;
+  const int lbx = 31 - __clz(P.bx), lby = 31 - __clz(P.by);
+  const float s = P.t.out_scale;
+  uint32_t it = 0;
+  float acc[2][64];
+  float amax = 0.f;
+  // write the staging buffers (fill), then store them: [mb] boxes of 64 channels at (x, y, img) of the output map
+  auto stage = [&](auto&& fill, int mg, int cx, int cy, int ci) {
+    if (elected) bulk_wait_read0();   // the previous stores have read the buffers
+    bar_sync(8 + half, 128);
+    fill();
+    fence_async_smem();
+    bar_sync(8 + half, 128);
+    if (elected) {
+#pragma unroll
+      for (int mb = 0; mb < 2; mb++)
+        if (mg * 128 + mb * 64 < p.M) {
+          tma_store_4d(out_hi, stg + mb * 4096, mg * 128 + mb * 64, cx, cy, ci);
+          tma_store_4d(out_lo, stg + T_STG_BUF + mb * 4096, mg * 128 + mb * 64, cx, cy, ci);
+        }
+      bulk_commit();
+    }
+  };
+
+  for (long tl = blockIdx.x; tl < total_tiles; tl += gridDim.x) {
+    const int mg_ = (int)(tl % mgroups);
+    const int nt = (int)(tl / mgroups);
+    const int tx = nt % P.tiles_x, rr = nt / P.tiles_x;
+    const int i0_ = (rr / P.tiles_y) * P.bi, y0_ = (rr % P.tiles_y) * P.by, x0_ = tx * P.bx;
+    {
+      mma_segment(acc, P, base, bar0, half, tid & 31, 0, KC, it);
+      if (P.t.dbg & 1) continue;
+      // Everything below derives from values laundered here, so the compiler cannot hoist the epilogue's lane and tile
+      // arithmetic above the main loop, where it would be live next to the 128 accumulators.
+      const int lane = opaque(threadIdx.x) & 31, w = (threadIdx.x >> 5) & 3, g = lane >> 2;
+      const int mg = opaque(mg_), i0 = opaque(i0_), y0 = opaque(y0_), x0 = opaque(x0_);
+      // bias (+ ReLU) in place: fmaf(v, s, b) as one pass, S + b after K segments
+#pragma unroll
+      for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const int co = mg * 128 + mb * 64 + 16 * w + 8 * h + g;
+          const float bv = (co < p.M && p.bias) ? __ldg(p.bias + co) : 0.f;
+#pragma unroll
+          for (int j = 0; j < 16; j++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+              float& v = acc[mb][4 * j + 2 * h + e];
+              const float a = fmaf(v, s, bv);
+              v = p.relu ? fmaxf(a, 0.f) : a;
+            }
+        }
+      if (P.pool) {
+        int dx, dy, di;
+        box_origin32(half * 32, P.bx >> 1, P.by >> 1, lbx - 1, lby - 1, dx, dy, di);
+        stage([&]() {
+          switch (P.bx) {
+            case 32: conv_pool_epi<32>(P, acc, half, w, lane, mg, i0, y0, x0, lby, amax, stg); break;
+            case 16: conv_pool_epi<16>(P, acc, half, w, lane, mg, i0, y0, x0, lby, amax, stg); break;
+            case 8: conv_pool_epi<8>(P, acc, half, w, lane, mg, i0, y0, x0, lby, amax, stg); break;
+            case 4: conv_pool_epi<4>(P, acc, half, w, lane, mg, i0, y0, x0, lby, amax, stg); break;
+            default: conv_pool_epi<2>(P, acc, half, w, lane, mg, i0, y0, x0, lby, amax, stg); break;
+          }
+        }, mg, (x0 >> 1) + dx, (y0 >> 1) + dy, i0 + di);
+        continue;
+      }
+#pragma unroll
+      for (int cc = 0; cc < 4; cc++) {
+        uint32_t hv[2][8], lv[2][8];   // [mb][2 jj + h]: n8 block 4cc + jj, channel row g + 8h
+#pragma unroll
+        for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+          for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+              const float a0 = acc[mb][4 * (4 * cc + jj) + 2 * h], a1 = acc[mb][4 * (4 * cc + jj) + 2 * h + 1];
+              if (mg * 128 + mb * 64 + 16 * w + 8 * h + g < p.M) amax = fmaxf(amax, fmaxf(fabsf(a0), fabsf(a1)));
+              split_f16x2(a0, a1, hv[mb][2 * jj + h], lv[mb][2 * jj + h]);
+            }
+        int dx, dy, di;
+        box_origin32(half * 128 + cc * 32, P.bx, P.by, lbx, lby, dx, dy, di);
+        stage([&]() {
+          // matrix q = lane / 8 of an x4: n8 block 2pr + q / 2, channels 16w + 8 (q & 1) ..; lane gives pixel row lane % 8
+          const int q = lane >> 3, k = lane & 7;
+#pragma unroll
+          for (int mb = 0; mb < 2; mb++)
+#pragma unroll
+            for (int pr = 0; pr < 2; pr++) {
+              const int px = 8 * (2 * pr + (q >> 1)) + k, c16 = 2 * w + (q & 1);
+              const uint32_t a = stg + mb * 4096 + px * 128 + ((c16 ^ k) << 4);
+              stmatrix_x4_trans(a, hv[mb][4 * pr], hv[mb][4 * pr + 1], hv[mb][4 * pr + 2], hv[mb][4 * pr + 3]);
+              stmatrix_x4_trans(a + T_STG_BUF, lv[mb][4 * pr], lv[mb][4 * pr + 1], lv[mb][4 * pr + 2], lv[mb][4 * pr + 3]);
+            }
+        }, mg, x0 + dx, y0 + dy, i0 + di);
+      }
+    }
+  }
+  if (elected) bulk_wait0();
+  mm_range_flag(P.status, amax);
+}
+
+template <bool ACC_EPI>
 static __global__ void __launch_bounds__(T_THREADS, 1)
-gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo) {
+gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
+                const __grid_constant__ CUtensorMap out_hi, const __grid_constant__ CUtensorMap out_lo) {
   const GemmP& p = P.t.g;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t bar0 = base + T_STAGES * T_STAGE_BYTES;
+  const uint32_t bar0 = base + T_STAGES * T_STAGE_BYTES + (ACC_EPI ? 2 * 2 * T_STG_BUF : 0);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (T_STAGES + s); };
   const uint32_t free_bar = bar0 + 8u * (2 * T_STAGES);   // the epilogue has read the accumulator image
@@ -183,6 +459,10 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
   if (warp < T_EPI_WARPS) {
     // =============================== EPILOGUE ===============================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T_CONS_REGS));
+    if constexpr (ACC_EPI) {
+      conv_acc_consumer(P, base, bar0, &out_hi, &out_lo);
+      return;
+    }
     const int q = warp & 3, half = warp >> 2;
     const int lbx = 31 - __clz(max(P.bx, 1)), lby = 31 - __clz(max(P.by, 1));
     uint32_t wcount = 0;   // (tile, segment) work items processed by this CTA
@@ -295,42 +575,8 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
       int g = 0, c0 = 0, len = BN, i0 = 0, y0 = 0, x0 = 0;
       if (P.conv) conv_origin(nt, i0, y0, x0); else tile_cols(nt, g, c0, len);
       for (int seg = 0; seg < P.ksegs; seg++, wcount++) {
-      // ---- main loop: this warpgroup's 128 rows x 128 columns (column half `half`), two m64n128 wgmma chains ----
-      // The first wgmma of each chain ignores the accumulators (scale_d = 0); clearing them here rather than once per
-      // CTA leaves them dead from the image dump to the next item, so the epilogue has their registers (no spills).
-#pragma unroll
-      for (int mb = 0; mb < 2; mb++)
-#pragma unroll
-        for (int i = 0; i < 64; i++) acc[mb][i] = 0.f;
       const int kc_lo = seg * P.kc_per_seg, kc_hi = min(KC, kc_lo + P.kc_per_seg);
-      for (int kc = kc_lo; kc < kc_hi; kc++, it++) {
-        const int s = it % T_STAGES;
-        mbar_wait(full_bar(s), (it / T_STAGES) & 1);
-        const uint32_t sa = base + s * T_STAGE_BYTES, sb = sa + A_SUB + half * (128 / 8) * 512;
-        if (!(P.t.dbg & 8)) {
-          wgmma_fence();
-#pragma unroll
-          for (int ks = 0; ks < 2; ks++) {
-            const uint64_t b_hi = smem_desc_sw64(sb + ks * 32), b_lo = smem_desc_sw64(sb + B_HALF + ks * 32);
-#pragma unroll
-            for (int mb = 0; mb < 2; mb++) {
-              const uint32_t a = sa + mb * 8 * SBO + ks * 2 * A_LBO;
-              const uint64_t a_hi = smem_desc(a, A_LBO, SBO), a_lo = smem_desc(a + A_HALF, A_LBO, SBO);
-              wgmma_n128(acc[mb], a_hi, b_hi, ((kc - kc_lo) | ks) ? 1u : 0u);
-              wgmma_n128(acc[mb], a_hi, b_lo, 1u);
-              wgmma_n128(acc[mb], a_lo, b_hi, 1u);
-            }
-          }
-          wgmma_commit();
-        }
-        wgmma_wait<1>();   // the previous chunk's wgmmas are done: release its stage
-        if (kc > kc_lo) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar((it - 1) % T_STAGES)); }
-      }
-      wgmma_wait<0>();
-      fence_acc(acc[0]);
-      fence_acc(acc[1]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar((it - 1) % T_STAGES));
+      mma_segment(acc, P, base, bar0, half, lane, kc_lo, kc_hi, it);
       bar_sync(7, T_EPI_WARPS * 32);   // both warpgroups are past their wgmmas: the image may overwrite the ring
       acc_dump(acc[0], img, BN, 0, half * 128);
       acc_dump(acc[1], img, BN, 64, half * 128);
@@ -545,7 +791,7 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
         const int row0 = (int)((long)g * p.x_gs + c0);
         for (int kc = 0; kc < KC; kc++, it++) {
           if (kc % P.kc_per_seg == 0) {   // a new (tile, segment): the previous one's accumulator image has been read
-            if (wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);
+            if (!ACC_EPI && wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);
             wcount++;
           }
           const int s = it % T_STAGES;
@@ -625,6 +871,23 @@ static inline int make_map_4d(CUtensorMap* m, const void* basep, int n_img, int 
   cuuint32_t box[4] = {32, (cuuint32_t)bx, (cuuint32_t)by, (cuuint32_t)bi}, es[4] = {1, 1, 1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(basep), dims, strides, box, es,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
+}
+
+// Output map of gemm_tma_kernel<true>: fp16 NHWC [n_img][H][W][M], box = 64 channels x the 32 consecutive columns of
+// a (bx, by, bi) box (box_origin32), 128-byte swizzle (the staging buffers' layout)
+static inline int make_map_4d_store(CUtensorMap* m, const void* basep, int n_img, int H, int W, int M, int bx, int by,
+                                    int bi) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return MMMOT_E_ARG;
+  const int sx = bx < 32 ? bx : 32, sy = by < 32 / sx ? by : 32 / sx, si = 32 / (sx * sy);
+  if (bx * by * bi < 64 || si > bi) return MMMOT_E_SHAPE;
+  cuuint64_t dims[4] = {(cuuint64_t)M, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n_img};
+  cuuint64_t strides[3] = {(cuuint64_t)M * 2, (cuuint64_t)W * M * 2, (cuuint64_t)H * W * M * 2};
+  cuuint32_t box[4] = {64, (cuuint32_t)sx, (cuuint32_t)sy, (cuuint32_t)si}, es[4] = {1, 1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(basep), dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
 }
@@ -713,7 +976,7 @@ static int gemm_tma_launch_mat(const GemmP& g, const uint4* Wp, float out_scale,
   int sms = 0;
   MM_TRY(mm_sm_count(&sms));
   static std::atomic<unsigned long long> attr{0};
-  MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel, tma::T_SMEM_BYTES, attr));
+  MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<false>, tma::T_SMEM_BYTES, attr));
   tma::TmaP P;
   memset(&P, 0, sizeof(P));
   P.t.g = g;
@@ -743,7 +1006,7 @@ static int gemm_tma_launch_mat(const GemmP& g, const uint4* Wp, float out_scale,
   }
   const long total = (long)g.num_tiles * P.t.m_tiles;
   const int grid = (int)(total < sms ? total : sms);
-  tma::gemm_tma_kernel<<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml);
+  tma::gemm_tma_kernel<false><<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml, mh, ml);
   MM_LAUNCH_CHECK();
   return 0;
 }
@@ -762,6 +1025,7 @@ struct ConvPlan {
   int bx, by, bi;          // box of 256 pixels (powers of two)
   int ksegs, kc_per_seg;   // K accumulated in ksegs passes of kc_per_seg 32-wide chunks
   int tiles_x, tiles_y, num_tiles;   // column tiles (boxes); the channel-major kernel runs ceil(M/128) row tiles of each
+  int acc_epi;             // channel-major: epilogue from the wgmma accumulators, TMA stores (gemm_tma_kernel<true>)
 };
 // want_pool: the caller takes a fused pooled map; use_kseg: the caller provides K-segment scratch.
 // dbg / seg_chunks: mmmot_set_debug / mmmot_set_kseg state.
@@ -798,6 +1062,10 @@ static inline ConvPlan conv_plan(int M, bool part, int n_img, int H, int W, int 
   }
   c.tiles_x = mm_cdiv(W, c.bx); c.tiles_y = mm_cdiv(H, c.by);
   c.num_tiles = c.tiles_x * c.tiles_y * mm_cdiv(n_img, c.bi);
+  // The accumulator epilogue stores 64-channel boxes and runs single-pass K only: combining K segments' partial sums
+  // from the registers through L2 measured slower than the accumulator image on the H100 (DESIGN §4.2).  Debug bit 11
+  // keeps the accumulator-image epilogue (A/B runs).
+  c.acc_epi = !c.px && !part && !(dbg & 2048) && M >= 64 && c.ksegs == 1;
   return c;
 }
 
@@ -818,8 +1086,6 @@ static int gemm_tma_launch_conv(const GemmP& g0, const uint4* Wp, float out_scal
   if (plan) *plan = c;
   int sms = 0;
   MM_TRY(mm_sm_count(&sms));
-  static std::atomic<unsigned long long> attr{0};
-  MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel, tma::T_SMEM_BYTES, attr));
   tma::TmaP P;
   memset(&P, 0, sizeof(P));
   GemmP g = g0;
@@ -856,7 +1122,19 @@ static int gemm_tma_launch_conv(const GemmP& g0, const uint4* Wp, float out_scal
   }
   const long total = (long)g.num_tiles * P.t.m_tiles;
   const int grid = (int)(total < sms ? total : sms);
-  tma::gemm_tma_kernel<<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml);
+  if (c.acc_epi) {
+    static std::atomic<unsigned long long> attr{0};
+    MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<true>, tma::T_CONV_SMEM_BYTES, attr));
+    const int sh = c.pool ? 1 : 0;
+    alignas(64) CUtensorMap oh, ol;
+    MM_TRY(tma::make_map_4d_store(&oh, Yhi, n_img, H >> sh, W >> sh, g.M, c.bx >> sh, c.by >> sh, c.bi));
+    MM_TRY(tma::make_map_4d_store(&ol, Yhi + P.plane_elems, n_img, H >> sh, W >> sh, g.M, c.bx >> sh, c.by >> sh, c.bi));
+    tma::gemm_tma_kernel<true><<<grid, tma::T_THREADS, tma::T_CONV_SMEM_BYTES, st>>>(P, mh, ml, oh, ol);
+  } else {
+    static std::atomic<unsigned long long> attr{0};
+    MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<false>, tma::T_SMEM_BYTES, attr));
+    tma::gemm_tma_kernel<false><<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml, mh, ml);
+  }
   MM_LAUNCH_CHECK();
   return 0;
 }

@@ -4,9 +4,15 @@ forward, under three mmmot_set_debug settings:
     dbg 8  MMA issue skipped: loader (weights + operand boxes from L2) + epilogue
     dbg 6  weight and operand loads skipped: MMA + epilogue without L2 traffic
 next to the ideal MMA time 3 * algorithmic FLOPs / (132 SMs * 4096 FLOP/clk * median SM clock of the run).
+Each setting runs once per conv epilogue: the extra debug bits of --epi-bits are OR'd into it (default "0,2048": the
+epilogue from the accumulators, then debug bit 11's accumulator-image epilogue), and the epilogues alternate in
+--rounds rounds in one process, so both see the same clocks; a table per epilogue (times averaged over the rounds)
+and the per-tag dbg-0 ratio follow.
 Bits 2-8 give wrong results by design: this is timing only, so the forward stops before the assignment LP and neither
 the status word nor the outputs are looked at.
-Run on a GPU box:  python tools/tma_overlap_times.py [pairs] [steps]"""
+Run on a GPU box:  python tools/tma_overlap_times.py [pairs] [steps] [--epi-bits 0,2048] [--rounds 2] [--json out]"""
+import argparse
+import json
 import os
 import subprocess
 import sys
@@ -36,8 +42,15 @@ def card():
 
 
 def main():
-    pairs = int(sys.argv[1]) if len(sys.argv) > 1 else bench.CFG["pairs"]
-    steps = int(sys.argv[2]) if len(sys.argv) > 2 else 2
+    ap = argparse.ArgumentParser()
+    ap.add_argument("pairs", nargs="?", type=int, default=bench.CFG["pairs"])
+    ap.add_argument("steps", nargs="?", type=int, default=2)
+    ap.add_argument("--epi-bits", default="0,2048", help="comma-separated debug bits OR'd into every setting, one epilogue each")
+    ap.add_argument("--rounds", type=int, default=2, help="rounds over the epilogues, alternating")
+    ap.add_argument("--json", default=None, help="also write the tables as JSON here")
+    args = ap.parse_args()
+    pairs, steps = args.pairs, args.steps
+    epis = [int(b) for b in args.epi_bits.split(",")]
     dev = torch.device("cuda:0")
     c = bench.CFG
     n, pts, hw = c["n"], c["pts"], c["hw"]
@@ -55,34 +68,57 @@ def main():
     lib = _lib.load()
     sampler = bench.ClockSampler(0)
     sampler.start()
-    times = {}
-    for dbg in DBG:
-        lib.mmmot_set_debug(dbg)
-        net.forward_batch(crops, points, split, n, check=False)      # warm-up
-        torch.cuda.synchronize(dev)
-        lib.mmmot_timing_enable(1)
-        for _ in range(steps):
-            net.forward_batch(crops, points, split, n, check=False)
-        torch.cuda.synchronize(dev)
-        lib.mmmot_timing_enable(0)
-        times[dbg] = bench.collect_tags(lib)
+    times = {e: {d: {} for d in DBG} for e in epis}       # epi -> dbg -> tag -> [ms, flop] summed over rounds
+    for _ in range(args.rounds):
+        for e in epis:
+            for dbg in DBG:
+                lib.mmmot_set_debug(dbg | e)
+                net.forward_batch(crops, points, split, n, check=False)      # warm-up
+                torch.cuda.synchronize(dev)
+                lib.mmmot_timing_enable(1)
+                for _ in range(steps):
+                    net.forward_batch(crops, points, split, n, check=False)
+                torch.cuda.synchronize(dev)
+                lib.mmmot_timing_enable(0)
+                for t, v in bench.collect_tags(lib).items():
+                    acc = times[e][dbg].setdefault(t, [0.0, 0.0])
+                    acc[0] += v[0]
+                    acc[1] += v[1]
     lib.mmmot_set_debug(0)
     clk = sampler.summary()
     mhz = clk["sm_mhz"]
+    nsteps = steps * args.rounds
     print(f"card: {card()}   SM clock median {mhz} MHz (max {clk['sm_max_mhz']}, throttle {clk['reasons']}, "
-          f"power {clk['power_w']} W)   cfg4, {pairs} pairs, ms per step over {steps} steps")
-    print(f"{'tag':32s} {'dbg0':>8s} {'dbg8':>8s} {'dbg6':>8s} {'mma':>8s}  {'dbg0-mma':>8s}  {'dbg8/dbg0':>9s}")
-    tot = [0.0] * 5
-    for t in TAGS:
-        if t not in times[0]:
-            continue
-        ms = [times[d][t][0] / steps if t in times[d] else float("nan") for d in DBG]
-        flop = times[0][t][1] / steps
-        ideal = 3 * flop / (SM_COUNT * FLOP_PER_CLK * mhz * 1e6) * 1e3 if mhz else float("nan")
-        row = ms + [ideal, ms[0] - ideal]
-        tot = [a + b for a, b in zip(tot, row)]
-        print(f"{t:32s} {row[0]:8.2f} {row[1]:8.2f} {row[2]:8.2f} {row[3]:8.2f}  {row[4]:8.2f}  {ms[1] / ms[0]:9.2f}")
-    print(f"{'total':32s} {tot[0]:8.2f} {tot[1]:8.2f} {tot[2]:8.2f} {tot[3]:8.2f}  {tot[4]:8.2f}  {tot[1] / tot[0]:9.2f}")
+          f"power {clk['power_w']} W)   cfg4, {pairs} pairs, ms per step over {steps} steps x {args.rounds} rounds")
+    out = {"card": card(), "clocks": clk, "pairs": pairs, "steps": steps, "rounds": args.rounds, "epilogues": {}}
+    for e in epis:
+        print(f"\nextra debug bits {e}")
+        print(f"{'tag':32s} {'dbg0':>8s} {'dbg8':>8s} {'dbg6':>8s} {'mma':>8s}  {'dbg0-mma':>8s}  {'dbg8/dbg0':>9s}")
+        tot = [0.0] * 5
+        rows = {}
+        for t in TAGS:
+            if t not in times[e][0]:
+                continue
+            ms = [times[e][d][t][0] / nsteps if t in times[e][d] else float("nan") for d in DBG]
+            flop = times[e][0][t][1] / nsteps
+            ideal = 3 * flop / (SM_COUNT * FLOP_PER_CLK * mhz * 1e6) * 1e3 if mhz else float("nan")
+            row = ms + [ideal, ms[0] - ideal]
+            rows[t] = [round(x, 3) for x in row]
+            tot = [a + b for a, b in zip(tot, row)]
+            print(f"{t:32s} {row[0]:8.2f} {row[1]:8.2f} {row[2]:8.2f} {row[3]:8.2f}  {row[4]:8.2f}  {ms[1] / ms[0]:9.2f}")
+        print(f"{'total':32s} {tot[0]:8.2f} {tot[1]:8.2f} {tot[2]:8.2f} {tot[3]:8.2f}  {tot[4]:8.2f}  {tot[1] / tot[0]:9.2f}")
+        rows["total"] = [round(x, 3) for x in tot]
+        out["epilogues"][str(e)] = rows
+    if len(epis) > 1:
+        e0, e1 = epis[0], epis[1]
+        print(f"\ndbg 0 time, extra bits {e0} / extra bits {e1}")
+        for t in TAGS + ["total"]:
+            if t in out["epilogues"][str(e0)] and t in out["epilogues"][str(e1)]:
+                a, b = out["epilogues"][str(e0)][t][0], out["epilogues"][str(e1)][t][0]
+                print(f"{t:32s} {a:8.2f} {b:8.2f}  {a / b:6.3f}")
+    if args.json:
+        with open(args.json, "w") as f:
+            json.dump(out, f)
 
 
 if __name__ == "__main__":
