@@ -293,12 +293,12 @@ static int vgg_conv0_launch(const float* crops, int n_img, int H, int W, const f
                             int* variant, cudaStream_t st) {
   const long n_pix = (long)n_img * H * W;
   const int dbg = mm_debug_flags();
-  if (dbg & 32) {   // A/B: direct FP32 FFMA first layer
+  if (dbg & MM_DBG_VGG0_FFMA) {   // A/B: direct FP32 FFMA first layer
     if (variant) *variant = 2;
     if (!wt || (W & 1)) return MMMOT_E_ARG;
     conv0_packed_kernel<<<mm_cdiv(n_pix / 2, 64), 256, 0, st>>>(crops, wt, bias, n_pix / 2, H, W, Y, y_plane, status);
     MM_LAUNCH_CHECK();
-  } else if (Wpx && !(dbg & 16384) && ((long)H * W) % 256 == 0 && W <= 512) {
+  } else if (Wpx && !(dbg & MM_DBG_VGG0_IM2COL) && ((long)H * W) % 256 == 0 && W <= 512) {
     // taps generated inside the contraction kernel (no im2col matrix in HBM)
     if (variant) *variant = 0;
     MM_TRY(gemm_tma_px_launch_gen27(crops, n_img, H, W, Wpx, wp_scale, bias, Y, y_plane, status, st));

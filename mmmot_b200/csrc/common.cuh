@@ -27,6 +27,27 @@
 
 void mm_count_launch();
 int mm_debug_flags();
+// mmmot_set_debug bits (include/mmmot_b200.h).  0-3 are profiling experiments whose results are wrong; the others
+// select an alternative implementation of the same arithmetic.
+enum {
+  MM_DBG_SKIP_EPI = 1 << 0,             // skip epilogue work
+  MM_DBG_SKIP_WEIGHTS = 1 << 1,         // skip weight loads
+  MM_DBG_SKIP_OPERANDS = 1 << 2,        // skip operand loads / generation
+  MM_DBG_SKIP_MMA = 1 << 3,             // skip MMA issue
+  MM_DBG_PN_STATS_PASS = 1 << 4,        // PointNet layer-5 / head statistics by a statistics-only contraction pass
+  MM_DBG_VGG0_FFMA = 1 << 5,            // first VGG layer as the direct FP32 FFMA kernel
+  MM_DBG_CM64 = 1 << 6,                 // 64-channel layers on the channel-major kernel instead of the pixel-major one
+  MM_DBG_PX_ST16 = 1 << 7,              // pixel-major epilogue with 16-byte stores
+  MM_DBG_PX_NO_HALO = 1 << 8,           // pixel-major kernel without halo boxes
+  MM_DBG_NO_FUSED_POOL = 1 << 9,        // no fused max-pool in the conv epilogues
+  MM_DBG_GEN_PLAIN = 1 << 10,           // generated-operand engine: producers without the software pipeline
+  MM_DBG_CONV_IMAGE = 1 << 11,          // channel-major conv epilogue through the accumulator image
+  MM_DBG_GEN_NORM_PREFETCH = 1 << 12,   // GEN_NORM producers with the software pipeline instead of TMA-staged rows
+  MM_DBG_PN_NORM_SPLIT = 1 << 13,       // PointNet layers 3, 4 through norm_split + the TMA-fed kernel
+  MM_DBG_VGG0_IM2COL = 1 << 14,         // first VGG layer with a separate im2col pre-pass
+  MM_DBG_VGG01_UNFUSED = 1 << 15,       // first VGG block as two launches instead of the fused kernel
+  MM_DBG_SEGSUM_GENERAL = 1 << 16,      // PointNet's per-detection-sum passes on the general TMA-fed kernel
+};
 int mm_kseg_chunks();  // K-segment length (in 32-wide chunks) of the tensor-core conv engine, 0 = off (mmmot_set_kseg)
 int mm_engine();  // 0 auto, 1 FP32 FFMA engine, 2 tensor-core (wgmma) engine (mmmot_set_engine)
 // Per-launch timing hook (mmmot_timing_*): every hot kernel of the path is bracketed by CUDA events on the launching

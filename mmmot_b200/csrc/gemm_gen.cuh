@@ -128,15 +128,6 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
   }
   __syncthreads();
 
-  // column tile -> group / first column / valid length
-  // (table tiling: {group, first ABSOLUTE row, length}; x_gs and y_gs are 0 then)
-  auto tile_cols = [&](int nt, int& g, int& c0, int& len) {
-    if (p.tile_tab) { const int4 tt = p.tile_tab[nt]; g = tt.x; c0 = tt.y; len = tt.z; return; }
-    g = nt / p.tiles_per_group;
-    c0 = (nt - g * p.tiles_per_group) * BN;
-    len = min(BN, p.S - c0);
-  };
-
   if (warp < G_EPI_WARPS) {
     // =============================== CONSUMERS: wgmma + epilogue ===============================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(G_CONS_REGS));
@@ -155,7 +146,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
       const int mg = (int)(t % mgroups);
       const int nt = (int)(t / mgroups);
       int g, c0, len;
-      tile_cols(nt, g, c0, len);
+      tile_cols(p, nt, g, c0, len);
       // The first wgmma of each chain ignores the accumulators (scale_d = 0).  Staged variants: clearing them here
       // rather than once per CTA leaves them dead from the image dump to the next tile, so the epilogue has their
       // registers (no spills).
@@ -164,7 +155,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
         const int s = it % STAGES;
         mbar_wait(full_bar(s), (it / STAGES) & 1);
         const uint32_t sa = base + s * SB, sb = sa + B_OFF + half * (128 / 8) * 128;
-        if (!(P.t.dbg & 8)) {
+        if (!(P.t.dbg & MM_DBG_SKIP_MMA)) {
           wgmma_fence();
 #pragma unroll
           for (int ks = 0; ks < 2; ks++) {
@@ -189,10 +180,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
       fence_acc(acc[1]);
       __syncwarp();
       if (lane == 0) mbar_arrive(empty_bar((it - 1) % STAGES));
-      bar_sync(7, G_EPI_WARPS * 32);   // both warpgroups are past their wgmmas: stages 0-1 may be overwritten
-      acc_dump(acc[0], img, BN, 0, half * 128);
-      acc_dump(acc[1], img, BN, 64, half * 128);
-      bar_sync(7, G_EPI_WARPS * 32);
+      acc_to_image(acc, img, half);
       {
         const int co = mg * 128 + q * 32 + lane;
         const bool rowok = co < p.M;
@@ -206,43 +194,18 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
           if (col0 >= len) break;   // warp-uniform
           uint32_t v[32];
           acc_ld32(img, BN, q * 32 + lane, col0, v);
-          if (P.t.dbg & 1) continue;
+          if (P.t.dbg & MM_DBG_SKIP_EPI) continue;
           float s1 = 0.f, s2 = 0.f, pv = 0.f;
           if (col0 + 32 <= len) {
             if (p.relu) epi_fast<true>(v, P.t.out_scale, bv, pv, s1, s2);
             else epi_fast<false>(v, P.t.out_scale, bv, pv, s1, s2);
-          } else {
-            float t = 0.f;
-#pragma unroll
-            for (int j = 0; j < 32; j++) {
-              float x = fmaf(__uint_as_float(v[j]), P.t.out_scale, bv);
-              if (p.relu) x = fmaxf(x, 0.f);
-              v[j] = __float_as_uint(x);
-              if (col0 + j < len) t += x;            // columns beyond the group are not counted (and not stored)
-            }
-            pv = t / (float)(len - col0);
-#pragma unroll
-            for (int j = 0; j < 32; j++)
-              if (col0 + j < len) { const float d = __uint_as_float(v[j]) - pv; s1 += d; s2 = fmaf(d, d, s2); }
-          }
+          } else epi_part(v, P.t.out_scale, bv, p.relu, col0, len, pv, s1, s2);
           stat_fold(f1, f2, min(32, len - col0), pv, s1, s2);
-          if (p.Y && rowok) {
-            float* d = dst + (long)cc * 32 * p.y_ms;
-            if (col0 + 32 <= len) {
-#pragma unroll
-              for (int j = 0; j < 32; j++) { *d = __uint_as_float(v[j]); d += p.y_ms; }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; j++)
-                if (col0 + j < len) d[(long)j * p.y_ms] = __uint_as_float(v[j]);
-            }
-          }
+          if (p.Y && rowok) store_cl(dst + (long)cc * 32 * p.y_ms, v, col0, len, p.y_ms);
         }
         if (p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2(f1, f2);
       }
-      fence_async_smem();   // the image's generic-proxy reads precede the next tile's operand and weight writes
-      __syncwarp();
-      if (lane == 0) mbar_arrive(free_bar);
+      image_release(free_bar, lane);   // the next tile's operand and weight writes may overwrite the image
     }
   } else {
     // =============================== OPERAND PRODUCERS (+ weight loads) ===============================
@@ -269,7 +232,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
     struct Raw { float a[NA][8]; float b[NB ? NB : 1][8]; };
     // ROW_TMA: sit counts the source boxes this thread has taken; the first producer thread issues box is_pos = chunk
     // is_kc of tile is_t, G_NSRC boxes ahead of sit, across tile boundaries
-    const bool gen_ops = !(P.t.dbg & 4);
+    const bool gen_ops = !(P.t.dbg & MM_DBG_SKIP_OPERANDS);
     uint32_t sit = 0, is_pos = 0;
     long is_t = blockIdx.x;
     int is_kc = 0;
@@ -278,7 +241,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
       const int ss = is_pos % G_NSRC;
       mbar_wait(src_empty(ss), ((is_pos / G_NSRC) & 1) ^ 1u);
       int g, c0, len;
-      tile_cols((int)(is_t / mgroups), g, c0, len);
+      tile_cols(p, (int)(is_t / mgroups), g, c0, len);
       mbar_expect_tx(src_full(ss), G_SRC_BYTES);   // rows past the tensor are zero-filled and counted
       tma::tma_load_2d(src0 + ss * G_SRC_BYTES, &map_det, is_kc * BK, (int)(g * p.x_gs + c0), src_full(ss));
       is_pos++;
@@ -295,7 +258,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
       const int mg = (int)(t % mgroups);
       const int nt = (int)(t / mgroups);
       int g, c0, len;
-      tile_cols(nt, g, c0, len);
+      tile_cols(p, nt, g, c0, len);
       unsigned okmask = 0;
       // 32-bit element offsets of the items' rows (this thread's k group) relative to the tile's / group's base
       const float* tbase = ROWS ? P.src + ((long)g * p.x_gs + c0) * P.ld_src : P.src + (long)g * P.Lf * p.K;
@@ -332,7 +295,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
       if (wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);   // the previous tile's accumulator image has been read
       wcount++;
       auto load = [&](Raw& R, int kc) {
-        if (P.t.dbg & 4) return;
+        if (P.t.dbg & MM_DBG_SKIP_OPERANDS) return;
 #pragma unroll
         for (int r = 0; r < NA; r++) ld_global_256(tbase + oa[r] + kc * BK, R.a[r]);
 #pragma unroll
@@ -343,7 +306,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
         const int s = it % STAGES;
         mbar_wait(empty_bar(s), ((it / STAGES) & 1) ^ 1u);
         if (pt == 0) {   // the chunk's weight block
-          if (P.t.dbg & 2) {
+          if (P.t.dbg & MM_DBG_SKIP_WEIGHTS) {
             mbar_arrive(full_bar(s));
           } else {
             mbar_expect_tx(full_bar(s), A_SUB);
@@ -352,7 +315,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
           }
         }
         uint8_t* bh = sm + s * SB + B_OFF + off0;
-        if (!(P.t.dbg & 4)) {
+        if (!(P.t.dbg & MM_DBG_SKIP_OPERANDS)) {
           const uint32_t sca = smem_u32(s_gsc + kc * BK + kg * 8), sha = smem_u32(s_gsh + kc * BK + kg * 8);
           float4 sc0, sc1, sh0, sh1;
 #pragma unroll
@@ -422,7 +385,7 @@ gemm_gen_kernel(const GenP P, const __grid_constant__ CUtensorMap map_det, const
           const int s = it % STAGES;
           mbar_wait(empty_bar(s), ((it / STAGES) & 1) ^ 1u);
           if (pt == 0) {   // the chunk's weight block
-            if (P.t.dbg & 2) {
+            if (P.t.dbg & MM_DBG_SKIP_WEIGHTS) {
               mbar_arrive(full_bar(s));
             } else {
               mbar_expect_tx(full_bar(s), A_SUB);
@@ -560,11 +523,11 @@ static int gemm_gen_launch_t(const GemmP& g, const uint4* Wp, float out_scale, c
 
 // Producer variant gemm_gen_launch takes: the software-pipelined (prefetching, PAIRED) producers or the plain ones.
 // Pure host logic, no CUDA call, so that tests can query it without a GPU (mmmot_debug_gen_prefetch).
-// dbg: mmmot_set_debug state; bit 10 (1024) producers without the software pipeline (A/B runs), bit 12 (4096) GEN_NORM
-// with it.  GEN_PAIR_* pipeline only at m == 128 (two whole rows per tile, see gemm_gen_kernel).
+// dbg: mmmot_set_debug state; MM_DBG_GEN_PLAIN producers without the software pipeline (A/B runs), GEN_NORM with
+// it under MM_DBG_GEN_NORM_PREFETCH.  GEN_PAIR_* pipeline only at m == 128 (two whole rows per tile, see gemm_gen_kernel).
 static inline bool gen_prefetch(int GEN, int m, int dbg) {
-  if (dbg & 1024) return false;
-  if (GEN == gen::GEN_NORM) return (dbg & 4096) != 0;
+  if (dbg & MM_DBG_GEN_PLAIN) return false;
+  if (GEN == gen::GEN_NORM) return (dbg & MM_DBG_GEN_NORM_PREFETCH) != 0;
   if (GEN == gen::GEN_COPY) return true;
   return m == 128;
 }
@@ -578,7 +541,7 @@ static inline bool gen_staged(int GEN, int m, int dbg) {
 // Whether a GEN_NORM launch stages its source rows by TMA (gemm_gen_kernel<GEN_NORM, false, true>): the default; bit 10
 // keeps the plain producers (the bit-for-bit reference), bit 12 the prefetching ones.  Pure host logic, like gen_prefetch
 // (mmmot_debug_gen_norm_staged).
-static inline bool gen_norm_staged(int dbg) { return !(dbg & (1024 | 4096)); }
+static inline bool gen_norm_staged(int dbg) { return !(dbg & (MM_DBG_GEN_PLAIN | MM_DBG_GEN_NORM_PREFETCH)); }
 
 // prefetched (host, or NULL) receives the variant taken (gen_prefetch)
 template <int GEN>

@@ -9,11 +9,13 @@
 //     same box at shifted (x, y) coordinates and the zero padding is TMA's out-of-bounds fill — no im2col,
 //     no boundary code, no index arithmetic on the SMs.
 // CTA (384 threads, persistent, one per SM): warps 0-7 are two consumer warpgroups (warpgroup h issues the wgmma
-// chains of the tile's 128 rows x column half h, then runs the epilogue of that half: warp q of it owns rows
-// 32q..32q+31), warp 8 is the loader (weights by cp.async.bulk, operand boxes by TMA; warps 9-11 only complete its
-// warpgroup).  Ring of 4 x 48 KB stages; the accumulator image of a finished tile (128 x 256 fp32) overlays the
-// first 128 KB of it, so the loader starts the next tile once the epilogue has read it.  Conv outputs are transposed through a per-warp smem scratch so each lane stores 64
-// contiguous bytes (32 channels of one pixel) per plane.
+// chains of the tile's 128 rows x column half h, then runs the epilogue of that half), warp 8 is the loader (weights
+// by cp.async.bulk, operand boxes by TMA; warps 9-11 only complete its warpgroup).  Ring of 4 x 48 KB stages.
+// gemm_tma_kernel<EPI> is instantiated once per consumer: EPI_MAT (mat_consumer, 1x1 contractions), EPI_CONV_IMAGE
+// (conv_image_consumer: K-segmented convs, or with GroupNorm partials) and EPI_CONV_ACC (conv_acc_consumer: single-pass
+// convs from the wgmma fragments).  The first two hand each tile over as an accumulator image (128 x 256 fp32) over the
+// ring's first 128 KB, so the loader starts the next tile once the epilogue has read it; their FP16 outputs are
+// transposed through a per-warp smem scratch (store_rows) so each lane stores 64 contiguous bytes per plane.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -37,21 +39,22 @@ constexpr int T_STAGE_BYTES = A_SUB + 2 * B_HALF;
 constexpr size_t T_SMEM_BYTES = (size_t)T_STAGES * T_STAGE_BYTES + 1024 + 256 + T_EPI_WARPS * T_EPI_SCRATCH;
 static_assert(T_SMEM_BYTES <= 227 * 1024, "gemm_tma_kernel exceeds the 227 KB of shared memory per block");
 static_assert(T_STAGES * T_STAGE_BYTES >= 128 * BN * 4, "the accumulator image must fit in the ring it overlays");
-// Conv kernel with the epilogue from the accumulators (gemm_tma_kernel<true>): no accumulator image and no per-warp
-// scratch, but two staging buffers per consumer warpgroup, each [64-channel half of the m128 tile][32 pixels][128 B]
-// (FP16 hi in one, lo in the other, SWIZZLE_128B) that the TMA stores to the NHWC output planes.
+// Conv kernel with the epilogue from the accumulators (gemm_tma_kernel<EPI_CONV_ACC>): no accumulator image and no
+// per-warp scratch, but two staging buffers per consumer warpgroup, each [64-channel half of the m128 tile][32 pixels]
+// [128 B] (FP16 hi in one, lo in the other, SWIZZLE_128B) that the TMA stores to the NHWC output planes.
 constexpr int T_STG_BUF = 2 * 32 * 128;
 constexpr size_t T_CONV_SMEM_BYTES = (size_t)T_STAGES * T_STAGE_BYTES + 2 * 2 * T_STG_BUF + 1024 + 256;
-static_assert(T_CONV_SMEM_BYTES <= 227 * 1024, "gemm_tma_kernel<true> exceeds the 227 KB of shared memory per block");
+static_assert(T_CONV_SMEM_BYTES <= 227 * 1024, "EPI_CONV_ACC exceeds the 227 KB of shared memory per block");
 
 enum { OUT_PLANAR = 3 };   // two FP16 planes Y_hi[row][y_ms], Y_lo = Y_hi + plane_elems (channels-last)
+// gemm_tma_kernel's consumers: rows x C matrix; 3x3 conv through the accumulator image, or from the accumulators
+enum { EPI_MAT = 0, EPI_CONV_IMAGE = 1, EPI_CONV_ACC = 2 };
 
 struct TmaP {
   TcP t;                    // .g: M, K, bias, relu, part, Y, y_ms, y_gs, S/tiles ...
-  int conv;                 // 0: rows x C matrix ; 1: 3x3 conv on [img][H][W][C]
   int bx, by, bi;           // conv box (pixels): columns of a tile = (ii*by + yy)*bx + xx
   int tiles_x, tiles_y;     // conv tile grid per image group
-  int n_img, H, W, C;       // conv geometry (C = input channels)
+  int n_img, H, W, C;       // conv geometry (C = input channels; 0 in a matrix launch)
   long plane_elems;         // output: distance (in fp16 elements) between the hi and lo planes
   int ksegs, kc_per_seg;    // conv: K is accumulated in `ksegs` passes of kc_per_seg chunks whose fp32
   float* acc_scratch;       // partial sums are combined in fp32 RN through acc_scratch[pixel][M] (see launcher)
@@ -179,7 +182,7 @@ __device__ __forceinline__ void mma_segment(float (&acc)[2][64], const TmaP& P, 
     const int s = it % T_STAGES;
     mbar_wait(full_bar(s), (it / T_STAGES) & 1);
     const uint32_t sa = base + s * T_STAGE_BYTES, sb = sa + A_SUB + half * (128 / 8) * 512;
-    if (!(P.t.dbg & 8)) {
+    if (!(P.t.dbg & MM_DBG_SKIP_MMA)) {
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < 2; ks++) {
@@ -215,13 +218,47 @@ __device__ __forceinline__ void box_origin32(int c0, int BX, int BY, int lbx, in
   dx = c0 & (BX - 1); dy = r & (BY - 1); di = r >> lby;
 }
 
-// Channel-major conv consumers of gemm_tma_kernel<true>: the epilogue runs on the wgmma fragments in registers.
+// column tile of a conv launch -> box origin (first image, y, x)
+__device__ __forceinline__ void conv_origin(const TmaP& P, int nt, int& i0, int& y0, int& x0) {
+  const int tx = nt % P.tiles_x;
+  const int r = nt / P.tiles_x;
+  const int ty = r % P.tiles_y;
+  i0 = (r / P.tiles_y) * P.bi; y0 = ty * P.by; x0 = tx * P.bx;
+}
+
+// x[j] = (row j of the warp's 32, channel `lane`) -> FP16 hi / lo planes at dst, dst + plane_elems: the 32x32 block is
+// transposed through the warp's smem scratch so that lane p stores the 32 channels (64 contiguous bytes per plane) of
+// row p at dst (the lane's own row, if ok); amax tracks the magnitudes converted.
+__device__ __forceinline__ void store_rows(const float (&x)[32], bool ok, __half* dst, long plane_elems, __half* scr,
+                                           int lane, float& amax) {
+  __half h[32], l[32];
+#pragma unroll
+  for (int j = 0; j < 32; j++) { split_f16(x[j], h[j], l[j]); amax = fmaxf(amax, fabsf(x[j])); }
+#pragma unroll
+  for (int pl = 0; pl < 2; pl++) {
+#pragma unroll
+    for (int j = 0; j < 32; j++) scr[j * 40 + lane] = pl ? l[j] : h[j];
+    __syncwarp();
+    if (ok) {
+      // 256-bit stores: each instruction writes whole 32-byte sectors (16-byte pieces cost a partial-sector
+      // write each and ran the first layers' epilogues at ~1.8 TB/s)
+      const uint4* src = reinterpret_cast<const uint4*>(scr + lane * 40);
+      __half* d = dst + (pl ? plane_elems : 0);
+      const uint4 a = src[0], b = src[1], c = src[2], e = src[3];
+      st_global_256(d, a, b);
+      st_global_256(d + 16, c, e);
+    }
+    __syncwarp();
+  }
+}
+
+// Channel-major conv consumers of gemm_tma_kernel<EPI_CONV_ACC>: the epilogue runs on the wgmma fragments in registers.
 // Thread (warp w of warpgroup `half`, lane = 4g + t) holds, for m64 block mb and n8 block j, channels
 // mg*128 + mb*64 + 16w + {g, g+8} at columns half*128 + 8j + {2t, 2t+1}: acc[mb][4j + {0, 1}] and acc[mb][4j + {2, 3}].
 // Output: per 32 columns (or the 32 pooled pixels of a half) the FP16 hi and lo values go pixel-major into the
 // warpgroup's two staging buffers (stmatrix.trans, 128-byte swizzle) and one thread stores them by TMA through the
 // NHWC maps out_hi / out_lo, which clip partial boxes.  Only the warpgroup synchronises; the ring is never waited on.
-// Single-pass K only (conv_plan): K-segmented launches keep the accumulator-image epilogue of gemm_tma_kernel<false>.
+// Single-pass K only (conv_plan): K-segmented launches take conv_image_consumer.
 template <int BX>
 __device__ __forceinline__ void conv_pool_epi(const TmaP& P, const float (&x)[2][64], int half, int w, int lane, int mg,
                                               int i0, int y0, int x0, int lby, float& amax, uint32_t buf) {
@@ -337,11 +374,11 @@ __device__ __forceinline__ void conv_acc_consumer(const TmaP& P, uint32_t base, 
   for (long tl = blockIdx.x; tl < total_tiles; tl += gridDim.x) {
     const int mg_ = (int)(tl % mgroups);
     const int nt = (int)(tl / mgroups);
-    const int tx = nt % P.tiles_x, rr = nt / P.tiles_x;
-    const int i0_ = (rr / P.tiles_y) * P.bi, y0_ = (rr % P.tiles_y) * P.by, x0_ = tx * P.bx;
+    int i0_, y0_, x0_;
+    conv_origin(P, nt, i0_, y0_, x0_);
     {
       mma_segment(acc, P, base, bar0, half, tid & 31, 0, KC, it);
-      if (P.t.dbg & 1) continue;
+      if (P.t.dbg & MM_DBG_SKIP_EPI) continue;
       // Everything below derives from values laundered here, so the compiler cannot hoist the epilogue's lane and tile
       // arithmetic above the main loop, where it would be live next to the 128 accumulators.
       const int lane = opaque(threadIdx.x) & 31, w = (threadIdx.x >> 5) & 3, g = lane >> 2;
@@ -411,7 +448,308 @@ __device__ __forceinline__ void conv_acc_consumer(const TmaP& P, uint32_t base, 
   mm_range_flag(P.status, amax);
 }
 
-template <bool ACC_EPI>
+// Matrix consumers of gemm_tma_kernel<EPI_MAT>, thread = one output channel of 128 image columns: bias, per-detection
+// addend, ReLU, GroupNorm partials, then the per-detection sums (segsum) or the fp32 channels-last / planar FP16 store.
+__device__ __forceinline__ void mat_consumer(const TmaP& P, uint8_t* sm, uint32_t base, uint32_t bar0) {
+  const GemmP& p = P.t.g;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = warp & 3, half = warp >> 2;
+  const uint32_t free_bar = bar0 + 8u * (2 * T_STAGES);
+  float* img = reinterpret_cast<float*>(sm);
+  __half* scr = reinterpret_cast<__half*>(sm + T_STAGES * T_STAGE_BYTES + 256 + warp * T_EPI_SCRATCH);
+  __half* yh = reinterpret_cast<__half*>(p.Y);
+  const int KC = P.t.k_chunks, mgroups = P.t.m_tiles;
+  const long total_tiles = (long)p.num_tiles * mgroups;
+  uint32_t it = 0;       // k chunks consumed (ring position)
+  float acc[2][64];      // rows 64 mb + fragment row, columns 128 half + fragment column
+  float amax = 0.f;      // largest magnitude converted to FP16 by this thread (range guard)
+  for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    const int mg = (int)(t % mgroups);
+    const int nt = (int)(t / mgroups);
+    int g, c0, len;
+    tile_cols(p, nt, g, c0, len);
+    mma_segment(acc, P, base, bar0, half, lane, 0, KC, it);
+    acc_to_image(acc, img, half);
+    const int co = mg * 128 + q * 32 + lane;
+    const bool rowok = co < p.M;
+    const float bv = (rowok && p.bias) ? __ldg(p.bias + co) : 0.f;
+    double f1 = 0.0, f2 = 0.0;   // this thread's (sum, sum of squares) over its 128 columns: four shifted chunk sums
+    const bool pass2 = P.segsum && !p.part && !p.Y && !p.relu;
+    // Everything the four 32-column chunks need from global memory is fetched up front, so its latency is paid once
+    // per subtile instead of once (or twice, seg -> addend) per chunk: the detection index at both ends of every
+    // chunk (one load: lane 2c / 2c+1 holds chunk c's first / last column), the per-detection addend row of every
+    // single-detection chunk, and the GroupNorm affine of the recomputing pass.
+    const bool use_seg = p.seg && (p.addend || P.segsum);
+    int4 ct = make_int4(0, 0, 0, 0);
+    if (use_seg) ct = __ldg(P.chunk_tab + (long)nt * 2 + half);   // same address in every lane: one transaction
+    const int cdesc[4] = {ct.x, ct.y, ct.z, ct.w};
+    float adv[4] = {0.f, 0.f, 0.f, 0.f};
+    unsigned one_det = 0;   // bit c: chunk c is complete and lies inside one detection
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+      if (cdesc[c] & 1) {
+        one_det |= 1u << c;
+        if (p.addend && rowok) adv[c] = __ldg(p.addend + (long)(cdesc[c] >> 1) * p.ld_add + co);
+      }
+    }
+    float na = 0.f, nb = 0.f;
+    if (P.segsum && rowok) { na = __ldg(p.sc + (long)g * p.M + co); nb = __ldg(p.sh + (long)g * p.M + co); }
+#pragma unroll 1
+    for (int cc = 0; cc < 4; cc++) {
+      const int col0 = half * 128 + cc * 32;
+      if (col0 >= len) break;   // warp-uniform
+      const int da = (cc == 0 ? ct.x : cc == 1 ? ct.y : cc == 2 ? ct.z : ct.w) >> 1;
+      const float adc = cc == 0 ? adv[0] : cc == 1 ? adv[1] : cc == 2 ? adv[2] : adv[3];
+      const bool single = (one_det >> cc) & 1u;
+      const int nvalid = min(32, len - col0);
+      uint32_t v[32];
+      acc_ld32(img, BN, q * 32 + lane, col0, v);
+      if (P.t.dbg & MM_DBG_SKIP_EPI) continue;
+      float s1 = 0.f, s2 = 0.f, pv = 0.f;
+      bool fast = col0 + 32 <= len;
+      if (pass2 && fast) {
+        // second (recomputing) pass, whole chunk inside one detection: bias, addend and the GroupNorm affine
+        // fold into one fma per element; no statistics, nothing stored
+        if (single) {
+          if (rowok) {
+            const float bva = bv + adc;
+            const float a2 = P.t.out_scale * na, b2 = fmaf(bva, na, nb);
+            float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+            for (int j = 0; j < 32; j += 2) {
+              r0 += fmaxf(fmaf(__uint_as_float(v[j]), a2, b2), 0.f);
+              r1 += fmaxf(fmaf(__uint_as_float(v[j + 1]), a2, b2), 0.f);
+            }
+            atomicAdd(P.segsum + (long)da * p.M + co, __float2ull_rn((r0 + r1) * 4294967296.f));
+          }
+          continue;
+        }
+      }
+      float bva = bv;
+      if (fast && p.addend) {
+        if (single) bva += adc;
+        else fast = false;
+      }
+      if (fast) {
+        if (p.relu) epi_fast<true>(v, P.t.out_scale, bva, pv, s1, s2);
+        else epi_fast<false>(v, P.t.out_scale, bva, pv, s1, s2);
+      } else if (p.addend) {   // per column: the chunk spans detections, or is partial
+        float t = 0.f;
+#pragma unroll
+        for (int j = 0; j < 32; j++) {
+          float x = fmaf(__uint_as_float(v[j]), P.t.out_scale, bv);
+          const int col = col0 + j;
+          if (rowok && col < len) x += __ldg(p.addend + (long)__ldg(p.seg + c0 + col) * p.ld_add + co);
+          if (p.relu) x = fmaxf(x, 0.f);
+          v[j] = __float_as_uint(x);
+          if (col < len) t += x;
+        }
+        pv = t / (float)nvalid;
+#pragma unroll
+        for (int j = 0; j < 32; j++)
+          if (j < nvalid) { const float d = __uint_as_float(v[j]) - pv; s1 += d; s2 = fmaf(d, d, s2); }
+      } else epi_part(v, P.t.out_scale, bv, p.relu, col0, len, pv, s1, s2);
+      stat_fold(f1, f2, nvalid, pv, s1, s2);
+      if (P.segsum && rowok) {
+        // GroupNorm + ReLU + per-detection sum fused into the (recomputing) second pass: the activation never
+        // reaches HBM.  Run sums are fp32 in column order; runs are merged with integer atomics, so the result
+        // does not depend on the order in which tiles finish.
+        int dcur = da;
+        float run = 0.f;
+        if (single) {
+          // common case: the whole 32-column chunk belongs to one detection
+#pragma unroll
+          for (int j = 0; j < 32; j++) run += fmaxf(fmaf(__uint_as_float(v[j]), na, nb), 0.f);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 32; j++) {
+            if (j < nvalid) {
+              const int d = __ldg(p.seg + c0 + col0 + j);
+              if (d != dcur) {
+                atomicAdd(P.segsum + (long)dcur * p.M + co, __float2ull_rn(run * 4294967296.f));
+                run = 0.f; dcur = d;
+              }
+              run += fmaxf(fmaf(__uint_as_float(v[j]), na, nb), 0.f);
+            }
+          }
+        }
+        atomicAdd(P.segsum + (long)dcur * p.M + co, __float2ull_rn(run * 4294967296.f));
+      }
+      if (!p.Y || !rowok) continue;
+      const long row0 = (long)g * p.y_gs + c0 + col0;
+      if (P.t.out_mode == OUT_PLANAR && !(p.y_ms & 31)) {
+        float xv[32];
+#pragma unroll
+        for (int j = 0; j < 32; j++) xv[j] = __uint_as_float(v[j]);
+        store_rows(xv, lane < nvalid, yh + (row0 + lane) * p.y_ms + (co - lane), P.plane_elems, scr, lane, amax);
+      } else if (P.t.out_mode == OUT_PLANAR) {
+        __half* dst = yh + row0 * p.y_ms + co;
+#pragma unroll
+        for (int j = 0; j < 32; j++)
+          if (j < nvalid) {
+            __half h, l;
+            split_f16(__uint_as_float(v[j]), h, l);
+            amax = fmaxf(amax, fabsf(__uint_as_float(v[j])));
+            dst[(long)j * p.y_ms] = h;
+            dst[(long)j * p.y_ms + P.plane_elems] = l;
+          }
+      } else {   // OUT_CL fp32 channels-last
+        store_cl(p.Y + row0 * p.y_ms + co, v, col0, len, p.y_ms);
+      }
+    }
+    if (p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2(f1, f2);
+    image_release(free_bar, lane);
+  }
+  mm_range_flag(P.status, amax);
+}
+
+// Conv consumers of gemm_tma_kernel<EPI_CONV_IMAGE>, thread = one output channel of 128 image pixels: K segments
+// combined through acc_scratch, or one pass with GroupNorm partials; planar FP16 NHWC, optionally 2x2 max-pooled.
+__device__ __forceinline__ void conv_image_consumer(const TmaP& P, uint8_t* sm, uint32_t base, uint32_t bar0) {
+  const GemmP& p = P.t.g;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = warp & 3, half = warp >> 2;
+  const uint32_t free_bar = bar0 + 8u * (2 * T_STAGES);
+  float* img = reinterpret_cast<float*>(sm);
+  __half* scr = reinterpret_cast<__half*>(sm + T_STAGES * T_STAGE_BYTES + 256 + warp * T_EPI_SCRATCH);
+  __half* yh = reinterpret_cast<__half*>(p.Y);
+  const int KC = P.t.k_chunks, mgroups = P.t.m_tiles;
+  const long total_tiles = (long)p.num_tiles * mgroups;
+  const int lbx = 31 - __clz(P.bx), lby = 31 - __clz(P.by);
+  uint32_t it = 0;       // k chunks consumed (ring position)
+  float acc[2][64], amax = 0.f;
+  // ---- fused 2x2 max-pool (P.pool): the thread owns one channel of the tile's columns, so every pooling window of
+  // its chunks is in its own registers.  NP pooled pixels per emission (8 for bx <= 16; 16 for bx == 32, where a
+  // chunk is one box row and the previous chunk's horizontal maxima are kept); lane q < NP stores pooled pixel q's
+  // 32 channels.  The pooled values are also summed per (image, channel) for SkipPool's global average.
+  const int Hp = P.H >> 1, Wp = P.W >> 1;
+  float hprev[16];            // bx == 32: horizontal maxima of the even row
+  float psum = 0.f;           // running sum of this thread's pooled values of image psum_img
+  int psum_img = -1;
+  auto pool_flush = [&](int co_) {
+    if (P.pool_sum && psum_img >= 0 && psum_img < P.n_img)
+      atomicAdd(P.pool_sum + (long)psum_img * p.M + co_, __float2ull_rn(psum * 4294967296.f));
+    psum = 0.f; psum_img = -1;
+  };
+  // o[q], q < np: pooled pixels of box rows (r0, r0 + 1), columns 2q', in box-row units r = ii*by + yy
+  auto pool_emit = [&](const float (&o)[16], int np, int r0, int wq, int cb, int co_, int i0, int y0, int x0) {
+    // pooled pixel q: box row r0 + 2*(q / wq), box column 2*(q % wq)      (wq = windows per row pair)
+    float xs[32];
+#pragma unroll
+    for (int j = 0; j < 32; j++) xs[j] = j < 16 ? o[j] : 0.f;
+    const int q = lane < np ? lane : 0;
+    const int r = r0 + 2 * (q / wq), xx = 2 * (q - (q / wq) * wq);
+    const int yy = r & (P.by - 1), ii = r >> lby;
+    const int img = i0 + ii, y = y0 + yy, xg = x0 + xx;
+    const bool ok = lane < np && img < P.n_img && y < P.H && xg < P.W;
+    store_rows(xs, ok, yh + (((long)img * Hp + (y >> 1)) * Wp + (xg >> 1)) * p.y_ms + cb, P.plane_elems, scr, lane,
+               amax);
+    if (P.pool_sum) {
+#pragma unroll
+      for (int j = 0; j < 16; j++) {
+        if (j < np) {
+          const int rj = r0 + 2 * (j / wq), xj = 2 * (j - (j / wq) * wq);
+          const int imj = i0 + (rj >> lby);
+          const bool okj = imj < P.n_img && y0 + (rj & (P.by - 1)) < P.H && x0 + xj < P.W;
+          if (imj != psum_img) { pool_flush(co_); psum_img = imj; }
+          if (okj) psum += o[j];
+        }
+      }
+    }
+  };
+  // one finished 32-column chunk (bias + ReLU applied) of channel co_: store it (x[j] = pixel column col0 + j, lane p
+  // stores pixel col0 + p), or pool it and store the pooled map
+  auto emit_conv = [&](const float (&x)[32], int cc, int col0, int co_, int i0, int y0, int x0) {
+    if (!P.pool) {
+      const int col = col0 + lane, r = col >> lbx;
+      const int img = i0 + (r >> lby), y = y0 + (r & (P.by - 1)), xg = x0 + (col & (P.bx - 1));
+      store_rows(x, img < P.n_img && y < P.H && xg < P.W, yh + (((long)img * P.H + y) * P.W + xg) * p.y_ms + co_ - lane,
+                 P.plane_elems, scr, lane, amax);
+      return;
+    }
+    float o[16];
+    const int r0 = col0 >> lbx;
+    if (P.bx == 32) {
+      if (!(cc & 1)) {
+#pragma unroll
+        for (int b = 0; b < 16; b++) hprev[b] = fmaxf(x[2 * b], x[2 * b + 1]);
+        return;
+      }
+#pragma unroll
+      for (int b = 0; b < 16; b++) o[b] = fmaxf(hprev[b], fmaxf(x[2 * b], x[2 * b + 1]));
+      pool_emit(o, 16, r0 - 1, 16, co_ - lane, co_, i0, y0, x0);
+      return;
+    }
+    float o8[8];
+    if (P.bx == 16) pool_chunk<16>(x, o8);
+    else if (P.bx == 8) pool_chunk<8>(x, o8);
+    else if (P.bx == 4) pool_chunk<4>(x, o8);
+    else pool_chunk<2>(x, o8);
+#pragma unroll
+    for (int j = 0; j < 16; j++) o[j] = j < 8 ? o8[j] : 0.f;
+    pool_emit(o, 8, r0, P.bx >> 1, co_ - lane, co_, i0, y0, x0);
+  };
+  for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    const int mg = (int)(t % mgroups);
+    const int nt = (int)(t / mgroups);
+    int i0, y0, x0;
+    conv_origin(P, nt, i0, y0, x0);
+    for (int seg = 0; seg < P.ksegs; seg++) {
+      const int kc_lo = seg * P.kc_per_seg, kc_hi = min(KC, kc_lo + P.kc_per_seg);
+      mma_segment(acc, P, base, bar0, half, lane, kc_lo, kc_hi, it);
+      acc_to_image(acc, img, half);
+      const int co = mg * 128 + q * 32 + lane;
+      const bool rowok = co < p.M;
+      const float bv = (rowok && p.bias) ? __ldg(p.bias + co) : 0.f;
+      double f1 = 0.0, f2 = 0.0;   // single pass: GroupNorm partials over the tile's (always complete) chunks
+#pragma unroll 1
+      for (int cc = 0; cc < 4; cc++) {
+        const int col0 = half * 128 + cc * 32;
+        uint32_t v[32];
+        acc_ld32(img, BN, q * 32 + lane, col0, v);
+        float x[32];
+        if (P.ksegs > 1) {
+          // K segments: S = the segments' fmaf(v, s, S) in fp32 RN, then S + bv.  Partial sums live in TILE order,
+          // scratch[(tile*256 + column)][M]: no pixel arithmetic, and a warp's 32 channels of one column are one
+          // 128-byte access
+          if (!rowok) continue;
+          float* sp = P.acc_scratch + ((long)nt * BN + col0) * p.M + co;
+          if (seg == 0 && seg < P.ksegs - 1) {
+#pragma unroll
+            for (int j = 0; j < 32; j++) __stcg(sp + (long)j * p.M, __uint_as_float(v[j]) * P.t.out_scale);
+            continue;
+          }
+#pragma unroll
+          for (int j = 0; j < 32; j++) x[j] = __ldcg(sp + (long)j * p.M);
+          if (seg < P.ksegs - 1) {
+#pragma unroll
+            for (int j = 0; j < 32; j++) __stcg(sp + (long)j * p.M, fmaf(__uint_as_float(v[j]), P.t.out_scale, x[j]));
+            continue;
+          }
+#pragma unroll
+          for (int j = 0; j < 32; j++) {
+            const float a = fmaf(__uint_as_float(v[j]), P.t.out_scale, x[j]) + bv;
+            x[j] = p.relu ? fmaxf(a, 0.f) : a;
+          }
+        } else {
+          if (P.t.dbg & MM_DBG_SKIP_EPI) continue;
+          float s1 = 0.f, s2 = 0.f, pv = 0.f;
+          if (p.relu) epi_fast<true>(v, P.t.out_scale, bv, pv, s1, s2);
+          else epi_fast<false>(v, P.t.out_scale, bv, pv, s1, s2);
+          stat_fold(f1, f2, 32, pv, s1, s2);
+          if (!rowok) continue;
+#pragma unroll
+          for (int j = 0; j < 32; j++) x[j] = __uint_as_float(v[j]);
+        }
+        emit_conv(x, cc, col0, co, i0, y0, x0);
+      }
+      if (P.ksegs == 1 && p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2(f1, f2);
+      if (P.pool && seg == P.ksegs - 1 && rowok) pool_flush(co);
+      image_release(free_bar, lane);
+    }
+  }
+  mm_range_flag(P.status, amax);
+}
+
+template <int EPI>
 static __global__ void __launch_bounds__(T_THREADS, 1)
 gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                 const __grid_constant__ CUtensorMap out_hi, const __grid_constant__ CUtensorMap out_lo) {
@@ -420,19 +758,16 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t bar0 = base + T_STAGES * T_STAGE_BYTES + (ACC_EPI ? 2 * 2 * T_STG_BUF : 0);
+  const uint32_t bar0 = base + T_STAGES * T_STAGE_BYTES + (EPI == EPI_CONV_ACC ? 2 * 2 * T_STG_BUF : 0);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (T_STAGES + s); };
   const uint32_t free_bar = bar0 + 8u * (2 * T_STAGES);   // the epilogue has read the accumulator image
-  float* img = reinterpret_cast<float*>(sm);              // accumulator image [128][BN] fp32 over the ring's first 128 KB
-  uint8_t* epi_scratch = sm + T_STAGES * T_STAGE_BYTES + 256;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int mgroups = P.t.m_tiles;
   const long total_tiles = (long)p.num_tiles * mgroups;
   // K chunks: conv = 9 taps x (C / 32) channel chunks, K order k = tap*C + ci ; matrix = K / 32
   const int KC = P.t.k_chunks;
-  const int cchunks = P.conv ? P.C / BK : KC;
 
   if (tid == 0) {
     for (int s = 0; s < T_STAGES; s++) {
@@ -444,339 +779,11 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
   }
   __syncthreads();
 
-  // tile -> (m group, column tile) ; column tile -> group / first column (matrix) or box origin (conv)
-  auto tile_cols = [&](int nt, int& g, int& c0, int& len) {
-    if (p.tile_tab) { int4 tt = p.tile_tab[nt]; g = tt.x; c0 = tt.y; len = tt.z; }
-    else { g = nt / p.tiles_per_group; c0 = (nt - g * p.tiles_per_group) * BN; len = min(BN, p.S - c0); }
-  };
-  auto conv_origin = [&](int nt, int& i0, int& y0, int& x0) {
-    const int tx = nt % P.tiles_x;
-    const int r = nt / P.tiles_x;
-    const int ty = r % P.tiles_y;
-    i0 = (r / P.tiles_y) * P.bi; y0 = ty * P.by; x0 = tx * P.bx;
-  };
-
   if (warp < T_EPI_WARPS) {
-    // =============================== EPILOGUE ===============================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T_CONS_REGS));
-    if constexpr (ACC_EPI) {
-      conv_acc_consumer(P, base, bar0, &out_hi, &out_lo);
-      return;
-    }
-    const int q = warp & 3, half = warp >> 2;
-    const int lbx = 31 - __clz(max(P.bx, 1)), lby = 31 - __clz(max(P.by, 1));
-    uint32_t wcount = 0;   // (tile, segment) work items processed by this CTA
-    uint32_t it = 0;       // k chunks consumed (ring position)
-    float acc[2][64];      // rows 64 mb + fragment row, columns 128 half + fragment column
-    float amax = 0.f;     // largest magnitude converted to FP16 by this thread (range guard)
-    __half* yh = reinterpret_cast<__half*>(p.Y);
-    __half* scr = reinterpret_cast<__half*>(epi_scratch + warp * T_EPI_SCRATCH);
-    // final conv values x[j] (pixel column col0+j, channel cb+lane) -> FP16 hi/lo NHWC planes.  The 32x32 block is
-    // transposed through smem so that lane p stores the 32 channels (64 contiguous bytes) of pixel col0+p.
-    // lane p stores the 32 channels (64 contiguous bytes per plane) of "its" row: x[j] is (row col0+j, channel cb+lane),
-    // the 32x32 block is transposed through the warp's smem scratch; o = element offset of this lane's row at channel cb
-    auto store_rows = [&](const float (&x)[32], bool ok, long o) {
-      __half h[32], l[32];
-#pragma unroll
-      for (int j = 0; j < 32; j++) { split_f16(x[j], h[j], l[j]); amax = fmaxf(amax, fabsf(x[j])); }
-#pragma unroll
-      for (int pl = 0; pl < 2; pl++) {
-#pragma unroll
-        for (int j = 0; j < 32; j++) scr[j * 40 + lane] = pl ? l[j] : h[j];
-        __syncwarp();
-        if (ok) {
-          // 256-bit stores: each instruction writes whole 32-byte sectors (16-byte pieces cost a partial-sector
-          // write each and ran the first layers' epilogues at ~1.8 TB/s)
-          const uint4* src = reinterpret_cast<const uint4*>(scr + lane * 40);
-          __half* dst = yh + o + (pl ? P.plane_elems : 0);
-          const uint4 a = src[0], b = src[1], c = src[2], d = src[3];
-          st_global_256(dst, a, b);
-          st_global_256(dst + 16, c, d);
-        }
-        __syncwarp();
-      }
-    };
-    // conv tiles: column -> (image, y, x) of the box, NHWC output
-    auto store_planar_block = [&](const float (&x)[32], int col0, int cb, int i0, int y0, int x0) {
-      const int col = col0 + lane;
-      const int xx = col & (P.bx - 1), r = col >> lbx;
-      const int yy = r & (P.by - 1), ii = r >> lby;
-      const int img = i0 + ii, y = y0 + yy, xg = x0 + xx;
-      store_rows(x, img < P.n_img && y < P.H && xg < P.W, (((long)img * P.H + y) * P.W + xg) * p.y_ms + cb);
-    };
-    // ---- fused 2x2 max-pool (P.pool): the thread owns one channel of the tile's columns, so every pooling window of
-    // its chunks is in its own registers.  NP pooled pixels per emission (8 for bx <= 16; 16 for bx == 32, where a
-    // chunk is one box row and the previous chunk's horizontal maxima are kept); lane q < NP stores pooled pixel q's
-    // 32 channels.  The pooled values are also summed per (image, channel) for SkipPool's global average.
-    const int Hp = P.H >> 1, Wp = P.W >> 1;
-    float hprev[16];            // bx == 32: horizontal maxima of the even row
-    float psum = 0.f;           // running sum of this thread's pooled values of image psum_img
-    int psum_img = -1;
-    auto pool_flush = [&](int co_) {
-      if (P.pool_sum && psum_img >= 0 && psum_img < P.n_img)
-        atomicAdd(P.pool_sum + (long)psum_img * p.M + co_, __float2ull_rn(psum * 4294967296.f));
-      psum = 0.f; psum_img = -1;
-    };
-    // o[q], q < NP: pooled pixels of box rows (r0, r0 + 1), columns 2q', in box-row units r = ii*by + yy
-    auto pool_emit = [&](const float (&o)[16], int np, int r0, int rstep_q, int wq, int cb, int co_, int i0, int y0, int x0) {
-      // pooled pixel q: box row r0 + 2*(q / wq), box column 2*(q % wq)      (wq = windows per row pair)
-      float xs[32];
-#pragma unroll
-      for (int j = 0; j < 32; j++) xs[j] = j < 16 ? o[j] : 0.f;
-      const int q = lane < np ? lane : 0;
-      const int r = r0 + 2 * (q / wq), xx = 2 * (q - (q / wq) * wq);
-      const int yy = r & (P.by - 1), ii = r >> lby;
-      const int img = i0 + ii, y = y0 + yy, xg = x0 + xx;
-      const bool ok = lane < np && img < P.n_img && y < P.H && xg < P.W;
-      store_rows(xs, ok, (((long)img * Hp + (y >> 1)) * Wp + (xg >> 1)) * p.y_ms + cb);
-      if (P.pool_sum) {
-        (void)rstep_q;
-#pragma unroll
-        for (int j = 0; j < 16; j++) {
-          if (j < np) {
-            const int rj = r0 + 2 * (j / wq), xj = 2 * (j - (j / wq) * wq);
-            const int imj = i0 + (rj >> lby);
-            const bool okj = imj < P.n_img && y0 + (rj & (P.by - 1)) < P.H && x0 + xj < P.W;
-            if (imj != psum_img) { pool_flush(co_); psum_img = imj; }
-            if (okj) psum += o[j];
-          }
-        }
-      }
-    };
-    // one finished 32-column chunk (bias + ReLU applied) of channel co_: store it, or pool it and store the pooled map
-    auto emit_conv = [&](const float (&x)[32], int cc, int col0, int co_, int i0, int y0, int x0) {
-      if (!P.pool) { store_planar_block(x, col0, co_ - lane, i0, y0, x0); return; }
-      float o[16];
-      const int r0 = col0 >> lbx;
-      if (P.bx == 32) {
-        if (!(cc & 1)) {
-#pragma unroll
-          for (int b = 0; b < 16; b++) hprev[b] = fmaxf(x[2 * b], x[2 * b + 1]);
-          return;
-        }
-#pragma unroll
-        for (int b = 0; b < 16; b++) o[b] = fmaxf(hprev[b], fmaxf(x[2 * b], x[2 * b + 1]));
-        pool_emit(o, 16, r0 - 1, 0, 16, co_ - lane, co_, i0, y0, x0);
-        return;
-      }
-      float o8[8];
-      if (P.bx == 16) pool_chunk<16>(x, o8);
-      else if (P.bx == 8) pool_chunk<8>(x, o8);
-      else if (P.bx == 4) pool_chunk<4>(x, o8);
-      else pool_chunk<2>(x, o8);
-#pragma unroll
-      for (int j = 0; j < 16; j++) o[j] = j < 8 ? o8[j] : 0.f;
-      pool_emit(o, 8, r0, 0, P.bx >> 1, co_ - lane, co_, i0, y0, x0);
-    };
-
-    for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      const int mg = (int)(t % mgroups);
-      const int nt = (int)(t / mgroups);
-      int g = 0, c0 = 0, len = BN, i0 = 0, y0 = 0, x0 = 0;
-      if (P.conv) conv_origin(nt, i0, y0, x0); else tile_cols(nt, g, c0, len);
-      for (int seg = 0; seg < P.ksegs; seg++, wcount++) {
-      const int kc_lo = seg * P.kc_per_seg, kc_hi = min(KC, kc_lo + P.kc_per_seg);
-      mma_segment(acc, P, base, bar0, half, lane, kc_lo, kc_hi, it);
-      bar_sync(7, T_EPI_WARPS * 32);   // both warpgroups are past their wgmmas: the image may overwrite the ring
-      acc_dump(acc[0], img, BN, 0, half * 128);
-      acc_dump(acc[1], img, BN, 64, half * 128);
-      bar_sync(7, T_EPI_WARPS * 32);
-      if (P.ksegs > 1) {
-        // K-segmented convolution: the tensor core's fp32 accumulator rounds toward zero at every K=16 step,
-        // so long K chains are cut into segments whose partial sums are combined here in fp32 round-to-nearest.
-        {
-          const int co = mg * 128 + q * 32 + lane;
-          const bool rowok = co < p.M;
-          const float bv = (rowok && p.bias) ? __ldg(p.bias + co) : 0.f;
-#pragma unroll 1
-          for (int cc = 0; cc < 4; cc++) {
-            const int col0 = half * 128 + cc * 32;
-            uint32_t v[32];
-            acc_ld32(img, BN, q * 32 + lane, col0, v);
-            if (!rowok) continue;
-            // partial sums live in TILE order, scratch[(tile*256 + column)][M]: no pixel arithmetic, and a
-            // warp's 32 channels of one column are one 128-byte access
-            float* sp = P.acc_scratch + ((long)nt * BN + col0) * p.M + co;
-            if (seg < P.ksegs - 1) {
-              if (seg == 0) {
-#pragma unroll
-                for (int j = 0; j < 32; j++) __stcg(sp + (long)j * p.M, __uint_as_float(v[j]) * P.t.out_scale);
-              } else {
-                float sv[32];
-#pragma unroll
-                for (int j = 0; j < 32; j++) sv[j] = __ldcg(sp + (long)j * p.M);
-#pragma unroll
-                for (int j = 0; j < 32; j++) __stcg(sp + (long)j * p.M, fmaf(__uint_as_float(v[j]), P.t.out_scale, sv[j]));
-              }
-            } else {
-              float sv[32];
-#pragma unroll
-              for (int j = 0; j < 32; j++) sv[j] = __ldcg(sp + (long)j * p.M);
-#pragma unroll
-              for (int j = 0; j < 32; j++) {
-                float a = fmaf(__uint_as_float(v[j]), P.t.out_scale, sv[j]) + bv;
-                sv[j] = p.relu ? fmaxf(a, 0.f) : a;
-              }
-              emit_conv(sv, cc, col0, co, i0, y0, x0);
-            }
-          }
-          if (P.pool && seg == P.ksegs - 1 && rowok) pool_flush(co);
-        }
-      } else
-      {
-        const int co = mg * 128 + q * 32 + lane;
-        const bool rowok = co < p.M;
-        const float bv = (rowok && p.bias) ? __ldg(p.bias + co) : 0.f;
-        double f1 = 0.0, f2 = 0.0;   // this thread's (sum, sum of squares) over its 128 columns: four shifted chunk sums
-        const bool pass2 = P.segsum && !p.part && !p.Y && !p.relu;
-        // Everything the four 32-column chunks need from global memory is fetched up front, so its latency is paid once
-        // per subtile instead of once (or twice, seg -> addend) per chunk: the detection index at both ends of every
-        // chunk (one load: lane 2c / 2c+1 holds chunk c's first / last column), the per-detection addend row of every
-        // single-detection chunk, and the GroupNorm affine of the recomputing pass.
-        const bool use_seg = p.seg && (p.addend || P.segsum);
-        int4 ct = make_int4(0, 0, 0, 0);
-        if (use_seg) ct = __ldg(P.chunk_tab + (long)nt * 2 + half);   // same address in every lane: one transaction
-        const int cdesc[4] = {ct.x, ct.y, ct.z, ct.w};
-        float adv[4] = {0.f, 0.f, 0.f, 0.f};
-        unsigned one_det = 0;   // bit c: chunk c is complete and lies inside one detection
-#pragma unroll
-        for (int c = 0; c < 4; c++) {
-          if (cdesc[c] & 1) {
-            one_det |= 1u << c;
-            if (p.addend && rowok) adv[c] = __ldg(p.addend + (long)(cdesc[c] >> 1) * p.ld_add + co);
-          }
-        }
-        float na = 0.f, nb = 0.f;
-        if (P.segsum && rowok) { na = __ldg(p.sc + (long)g * p.M + co); nb = __ldg(p.sh + (long)g * p.M + co); }
-#pragma unroll 1
-        for (int cc = 0; cc < 4; cc++) {
-          const int col0 = half * 128 + cc * 32;
-          if (col0 >= len) break;   // warp-uniform
-          const int da = (cc == 0 ? ct.x : cc == 1 ? ct.y : cc == 2 ? ct.z : ct.w) >> 1;
-          const float adc = cc == 0 ? adv[0] : cc == 1 ? adv[1] : cc == 2 ? adv[2] : adv[3];
-          const bool single = (one_det >> cc) & 1u;
-          uint32_t v[32];
-          acc_ld32(img, BN, q * 32 + lane, col0, v);
-          if (P.t.dbg & 1) continue;
-          float s1 = 0.f, s2 = 0.f, pv = 0.f;
-          bool fast = col0 + 32 <= len;
-          if (pass2 && fast) {
-            // second (recomputing) pass, whole chunk inside one detection: bias, addend and the GroupNorm affine
-            // fold into one fma per element; no statistics, nothing stored
-            if (single) {
-              if (rowok) {
-                const float bva = bv + adc;
-                const float a2 = P.t.out_scale * na, b2 = fmaf(bva, na, nb);
-                float r0 = 0.f, r1 = 0.f;
-#pragma unroll
-                for (int j = 0; j < 32; j += 2) {
-                  r0 += fmaxf(fmaf(__uint_as_float(v[j]), a2, b2), 0.f);
-                  r1 += fmaxf(fmaf(__uint_as_float(v[j + 1]), a2, b2), 0.f);
-                }
-                atomicAdd(P.segsum + (long)da * p.M + co, __float2ull_rn((r0 + r1) * 4294967296.f));
-              }
-              continue;
-            }
-          }
-          float bva = bv;
-          if (fast && p.addend) {
-            if (single) bva += adc;
-            else fast = false;
-          }
-          if (fast) {
-            if (p.relu) epi_fast<true>(v, P.t.out_scale, bva, pv, s1, s2);
-            else epi_fast<false>(v, P.t.out_scale, bva, pv, s1, s2);
-          } else {
-            float t = 0.f;
-#pragma unroll
-            for (int j = 0; j < 32; j++) {
-              float x = fmaf(__uint_as_float(v[j]), P.t.out_scale, bv);
-              const int col = col0 + j;
-              if (p.addend && rowok && col < len)
-                x += __ldg(p.addend + (long)__ldg(p.seg + c0 + col) * p.ld_add + co);
-              if (p.relu) x = fmaxf(x, 0.f);
-              v[j] = __float_as_uint(x);
-              if (col < len) t += x;
-            }
-            pv = t / (float)min(32, len - col0);
-#pragma unroll
-            for (int j = 0; j < 32; j++)
-              if (col0 + j < len) { const float d = __uint_as_float(v[j]) - pv; s1 += d; s2 = fmaf(d, d, s2); }
-          }
-          stat_fold(f1, f2, min(32, len - col0), pv, s1, s2);
-          if (P.segsum && rowok) {
-            // GroupNorm + ReLU + per-detection sum fused into the (recomputing) second pass: the activation never
-            // reaches HBM.  Run sums are fp32 in column order; runs are merged with integer atomics, so the result
-            // does not depend on the order in which tiles finish.
-            const int nvalid = min(32, len - col0);
-            int dcur = da;
-            float run = 0.f;
-            if (single) {
-              // common case: the whole 32-column chunk belongs to one detection
-#pragma unroll
-              for (int j = 0; j < 32; j++) run += fmaxf(fmaf(__uint_as_float(v[j]), na, nb), 0.f);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; j++) {
-                if (j < nvalid) {
-                  const int d = __ldg(p.seg + c0 + col0 + j);
-                  if (d != dcur) {
-                    atomicAdd(P.segsum + (long)dcur * p.M + co, __float2ull_rn(run * 4294967296.f));
-                    run = 0.f; dcur = d;
-                  }
-                  run += fmaxf(fmaf(__uint_as_float(v[j]), na, nb), 0.f);
-                }
-              }
-            }
-            atomicAdd(P.segsum + (long)dcur * p.M + co, __float2ull_rn(run * 4294967296.f));
-          }
-          if (!p.Y || !rowok) continue;
-          if (P.conv) {
-            float xv[32];
-#pragma unroll
-            for (int j = 0; j < 32; j++) xv[j] = __uint_as_float(v[j]);
-            emit_conv(xv, cc, col0, co, i0, y0, x0);
-          } else {
-            const int nvalid = min(32, len - col0);
-            const long row0 = (long)g * p.y_gs + c0 + col0;
-            if (P.t.out_mode == OUT_PLANAR && !(p.y_ms & 31)) {
-              float xv[32];
-#pragma unroll
-              for (int j = 0; j < 32; j++) xv[j] = __uint_as_float(v[j]);
-              store_rows(xv, lane < nvalid, (row0 + lane) * p.y_ms + (co - lane));
-            } else if (P.t.out_mode == OUT_PLANAR) {
-              __half* dst = yh + row0 * p.y_ms + co;
-#pragma unroll
-              for (int j = 0; j < 32; j++)
-                if (j < nvalid) {
-                  __half h, l;
-                  split_f16(__uint_as_float(v[j]), h, l);
-                  amax = fmaxf(amax, fabsf(__uint_as_float(v[j])));
-                  dst[(long)j * p.y_ms] = h;
-                  dst[(long)j * p.y_ms + P.plane_elems] = l;
-                }
-            } else {   // OUT_CL fp32 channels-last
-              float* dst = p.Y + row0 * p.y_ms + co;
-              if (nvalid == 32) {
-#pragma unroll
-                for (int j = 0; j < 32; j++) { *dst = __uint_as_float(v[j]); dst += p.y_ms; }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 32; j++)
-                  if (j < nvalid) dst[(long)j * p.y_ms] = __uint_as_float(v[j]);
-              }
-            }
-          }
-        }
-        if (p.part && rowok) p.part[((long)nt * 2 + half) * p.M + co] = make_double2(f1, f2);
-        if (P.conv && P.pool && rowok) pool_flush(co);
-      }
-      fence_async_smem();   // the image's generic-proxy reads precede the loader's next TMA writes
-      __syncwarp();
-      if (lane == 0) mbar_arrive(free_bar);
-      }
-    }
-    mm_range_flag(P.status, amax);
+    if constexpr (EPI == EPI_MAT) mat_consumer(P, sm, base, bar0);
+    else if constexpr (EPI == EPI_CONV_IMAGE) conv_image_consumer(P, sm, base, bar0);
+    else conv_acc_consumer(P, base, bar0, &out_hi, &out_lo);
   } else {
     // =============================== LOADER (weights + operand boxes) ===============================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(T_LOAD_REGS));
@@ -785,39 +792,39 @@ gemm_tma_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, const 
       for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         const int mg = (int)(t % mgroups);
         const int nt = (int)(t / mgroups);
-        const int mt0 = mg;
         int g = 0, c0 = 0, len = BN, i0 = 0, y0 = 0, x0 = 0;
-        if (P.conv) conv_origin(nt, i0, y0, x0); else tile_cols(nt, g, c0, len);
+        if constexpr (EPI == EPI_MAT) tile_cols(p, nt, g, c0, len);
+        else conv_origin(P, nt, i0, y0, x0);
         const int row0 = (int)((long)g * p.x_gs + c0);
         for (int kc = 0; kc < KC; kc++, it++) {
           if (kc % P.kc_per_seg == 0) {   // a new (tile, segment): the previous one's accumulator image has been read
-            if (!ACC_EPI && wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);
+            if (EPI != EPI_CONV_ACC && wcount > 0) mbar_wait(free_bar, (wcount - 1) & 1);
             wcount++;
           }
           const int s = it % T_STAGES;
           mbar_wait(empty_bar(s), ((it / T_STAGES) & 1) ^ 1);
           const uint32_t abytes = (uint32_t)A_SUB;
-          const bool skipA = P.t.dbg & 2, skipB = P.t.dbg & 4;     // profiling experiments only
+          const bool skipA = P.t.dbg & MM_DBG_SKIP_WEIGHTS, skipB = P.t.dbg & MM_DBG_SKIP_OPERANDS;
           mbar_expect_tx(full_bar(s), (skipA ? 0u : abytes) + (skipB ? 0u : 2u * B_HALF));
           const uint32_t sa = base + s * T_STAGE_BYTES, sb = sa + A_SUB;
-          const uint8_t* src = reinterpret_cast<const uint8_t*>(P.t.Wp) + ((size_t)kc * P.t.m_tiles + mt0) * A_SUB;
+          const uint8_t* src = reinterpret_cast<const uint8_t*>(P.t.Wp) + ((size_t)kc * P.t.m_tiles + mg) * A_SUB;
           if (!skipA) bulk_g2s(sa, src, abytes, full_bar(s));
           if (skipB) continue;
-          if (P.conv) {
+          if constexpr (EPI == EPI_MAT) {
+            tma_load_2d(sb, &map_hi, kc * BK, row0, full_bar(s));
+            tma_load_2d(sb + B_HALF, &map_lo, kc * BK, row0, full_bar(s));
+          } else {
+            const int cchunks = P.C / BK;
             const int tap = kc / cchunks, cc = kc - tap * cchunks;
             const int dx = tap % 3 - 1, dy = tap / 3 - 1;
             tma_load_4d(sb, &map_hi, cc * BK, x0 + dx, y0 + dy, i0, full_bar(s));
             tma_load_4d(sb + B_HALF, &map_lo, cc * BK, x0 + dx, y0 + dy, i0, full_bar(s));
-          } else {
-            tma_load_2d(sb, &map_hi, kc * BK, row0, full_bar(s));
-            tma_load_2d(sb + B_HALF, &map_lo, kc * BK, row0, full_bar(s));
           }
         }
       }
     }
     __syncwarp();
   }
-
 }
 
 // ---- host side: tensor maps through the driver entry point (no libcuda link dependency) ----
@@ -835,66 +842,76 @@ static inline EncodeTiledFn encode_fn() {
   }
   return fn;
 }
-// fp16 [rows][C] matrix (row stride ld elements), box 32 x 256, 64-byte swizzle
-static inline int make_map_2d(CUtensorMap* m, const void* basep, long rows, int C, long ld) {
+// one tiled tensor map (unit element strides, no interleave, zero OOB fill); 900 + the CUresult on failure
+static inline int encode_map(CUtensorMap* m, CUtensorMapDataType type, cuuint32_t rank, const void* basep,
+                             const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box,
+                             CUtensorMapSwizzle swizzle, CUtensorMapL2promotion promo) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return MMMOT_E_ARG;
-  cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {32, 256}, es[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(basep), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const cuuint32_t es[4] = {1, 1, 1, 1};
+  const CUresult r = fn(m, type, rank, const_cast<void*>(basep), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        swizzle, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
+}
+// fp16 [rows][C] matrix (row stride ld elements), box 32 x 256, 64-byte swizzle
+static inline int make_map_2d(CUtensorMap* m, const void* basep, long rows, int C, long ld) {
+  const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)ld * 2};
+  const cuuint32_t box[2] = {32, 256};
+  return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, basep, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // fp32 [rows][C] matrix (row stride ld >= C elements, ld * 4 a multiple of 16), box 32 x box_rows: 128-byte box rows,
 // so SWIZZLE_128B is allowed
 static inline int make_map_2d_f32(CUtensorMap* m, const void* basep, long rows, int C, long ld, int box_rows,
                                   CUtensorMapSwizzle swizzle) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return MMMOT_E_ARG;
-  cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {32, (cuuint32_t)box_rows}, es[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(basep), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
+  const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)ld * 4};
+  const cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
+  return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, basep, dims, strides, box, swizzle,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // fp16 NHWC [n_img][H][W][C], box (32, bx, by, bi)
 static inline int make_map_4d(CUtensorMap* m, const void* basep, int n_img, int H, int W, int C, int bx, int by,
                               int bi) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return MMMOT_E_ARG;
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n_img};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {32, (cuuint32_t)bx, (cuuint32_t)by, (cuuint32_t)bi}, es[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(basep), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n_img};
+  const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint32_t box[4] = {32, (cuuint32_t)bx, (cuuint32_t)by, (cuuint32_t)bi};
+  return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, basep, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 
-// Output map of gemm_tma_kernel<true>: fp16 NHWC [n_img][H][W][M], box = 64 channels x the 32 consecutive columns of
-// a (bx, by, bi) box (box_origin32), 128-byte swizzle (the staging buffers' layout)
+// Output map of gemm_tma_kernel<EPI_CONV_ACC>: fp16 NHWC [n_img][H][W][M], box = 64 channels x the 32 consecutive
+// columns of a (bx, by, bi) box (box_origin32), 128-byte swizzle (the staging buffers' layout)
 static inline int make_map_4d_store(CUtensorMap* m, const void* basep, int n_img, int H, int W, int M, int bx, int by,
                                     int bi) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return MMMOT_E_ARG;
   const int sx = bx < 32 ? bx : 32, sy = by < 32 / sx ? by : 32 / sx, si = 32 / (sx * sy);
   if (bx * by * bi < 64 || si > bi) return MMMOT_E_SHAPE;
-  cuuint64_t dims[4] = {(cuuint64_t)M, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n_img};
-  cuuint64_t strides[3] = {(cuuint64_t)M * 2, (cuuint64_t)W * M * 2, (cuuint64_t)H * W * M * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)sx, (cuuint32_t)sy, (cuuint32_t)si}, es[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(basep), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 900 + (int)r;
+  const cuuint64_t dims[4] = {(cuuint64_t)M, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n_img};
+  const cuuint64_t strides[3] = {(cuuint64_t)M * 2, (cuuint64_t)W * M * 2, (cuuint64_t)H * W * M * 2};
+  const cuuint32_t box[4] = {64, (cuuint32_t)sx, (cuuint32_t)sy, (cuuint32_t)si};
+  return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, basep, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                    CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
 
 }  // namespace tma
 
 #include "gemm_tma_px.cuh"
+
+// launch parameters every TMA-fed launch sets; the rest of TmaP starts zero
+static inline tma::TmaP tma_params(const GemmP& g, const uint4* Wp, float out_scale, int out_mode, long plane_elems,
+                                   int* status) {
+  tma::TmaP P;
+  memset(&P, 0, sizeof(P));
+  P.t.g = g;
+  P.t.Wp = Wp;
+  P.t.m_tiles = (g.M + 127) / 128;
+  P.t.k_chunks = g.K / tc::BK;
+  P.t.out_scale = out_scale;
+  P.t.out_mode = out_mode;
+  P.t.dbg = mm_debug_flags();
+  P.plane_elems = plane_elems;
+  P.status = status;
+  return P;
+}
 
 // pixel-major kernel for 64-channel planar outputs (see gemm_tma_px.cuh); P fully prepared by the caller
 static int gemm_tma_px_launch(tma::TmaP& P, const CUtensorMap& mh, const CUtensorMap& ml, int sms, cudaStream_t st) {
@@ -920,21 +937,13 @@ static int gemm_tma_px_launch_gen27(const float* crops, int n_img, int H, int W,
   MM_TRY(mm_sm_count(&sms));
   static std::atomic<unsigned long long> attr{0};
   MM_TRY(mm_ensure_smem(tma::gemm_tma_px_kernel<true>, tma::PX_SMEM_BYTES, attr));
-  tma::TmaP P;
-  memset(&P, 0, sizeof(P));
   GemmP g = gemm_defaults();
   g.bias = bias; g.M = 64; g.K = 32; g.relu = 1;
   g.S = (int)n_pix; g.tiles_per_group = mm_cdiv(n_pix, tc::BN); g.num_tiles = g.tiles_per_group;
   g.Y = reinterpret_cast<float*>(Yhi); g.y_ms = 64;
-  P.t.g = g;
-  P.t.Wp = Wpx; P.wcompact = 1;
-  P.t.m_tiles = 1; P.t.k_chunks = 1;
-  P.t.out_scale = out_scale;
-  P.t.out_mode = tma::OUT_PLANAR;
-  P.t.dbg = mm_debug_flags();
-  P.plane_elems = y_plane;
+  tma::TmaP P = tma_params(g, Wpx, out_scale, tma::OUT_PLANAR, y_plane, status);
+  P.wcompact = 1;
   P.ksegs = 1; P.kc_per_seg = 1;
-  P.status = status;
   P.gen_src = crops; P.n_img = n_img; P.H = H; P.W = W;
   alignas(64) CUtensorMap dummy;
   memset(&dummy, 0, sizeof(dummy));
@@ -948,10 +957,10 @@ static int gemm_tma_px_launch_gen27(const float* crops, int n_img, int H, int W,
 #include "gemm_segsum.cuh"
 
 // Whether a matrix-mode launch takes gemm_segsum_kernel (gemm_segsum.cuh): the per-detection-sum pass at K = 64 or 128
-// with nothing stored, no statistics and no ReLU before the affine; debug bit 16 (65536) keeps gemm_tma_kernel (A/B
+// with nothing stored, no statistics and no ReLU before the affine; MM_DBG_SEGSUM_GENERAL keeps gemm_tma_kernel (A/B
 // runs).  Pure host logic, no CUDA call (mmmot_debug_segsum_kernel).
 static inline bool segsum_dedicated(int K, bool segsum, bool y, bool part, bool relu, int dbg) {
-  return segsum && !y && !part && !relu && (K == 64 || K == 128) && !(dbg & 65536);
+  return segsum && !y && !part && !relu && (K == 64 || K == 128) && !(dbg & MM_DBG_SEGSUM_GENERAL);
 }
 
 template <int K>
@@ -976,27 +985,17 @@ static int gemm_tma_launch_mat(const GemmP& g, const uint4* Wp, float out_scale,
   int sms = 0;
   MM_TRY(mm_sm_count(&sms));
   static std::atomic<unsigned long long> attr{0};
-  MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<false>, tma::T_SMEM_BYTES, attr));
-  tma::TmaP P;
-  memset(&P, 0, sizeof(P));
-  P.t.g = g;
-  P.t.Wp = Wp;
-  P.t.m_tiles = (g.M + 127) / 128;
-  P.t.k_chunks = g.K / tc::BK;
-  P.t.out_scale = out_scale;
-  P.t.out_mode = out_mode;
-  P.t.dbg = mm_debug_flags();
-  P.plane_elems = y_plane;
+  MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<tma::EPI_MAT>, tma::T_SMEM_BYTES, attr));
+  tma::TmaP P = tma_params(g, Wp, out_scale, out_mode, y_plane, status);
   P.ksegs = 1; P.kc_per_seg = P.t.k_chunks;
   P.segsum = segsum;
-  P.status = status;
   P.chunk_tab = chunk_tab;
   if (g.seg && (g.addend || segsum) && !chunk_tab) return MMMOT_E_ARG;
   alignas(64) CUtensorMap mh, ml;
   MM_TRY(tma::make_map_2d(&mh, Xhi, rows, g.K, ldx));
   MM_TRY(tma::make_map_2d(&ml, Xhi + x_plane, rows, g.K, ldx));
   if (out_mode == tma::OUT_PLANAR && g.M == 64 && g.y_ms == 64 && !g.part && !segsum && !g.addend && !g.tile_tab &&
-      !(P.t.dbg & 64)) {
+      !(P.t.dbg & MM_DBG_CM64)) {
     if (Wpx) { P.t.Wp = Wpx; P.wcompact = 1; }
     return gemm_tma_px_launch(P, mh, ml, sms, st);
   }
@@ -1006,7 +1005,7 @@ static int gemm_tma_launch_mat(const GemmP& g, const uint4* Wp, float out_scale,
   }
   const long total = (long)g.num_tiles * P.t.m_tiles;
   const int grid = (int)(total < sms ? total : sms);
-  tma::gemm_tma_kernel<false><<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml, mh, ml);
+  tma::gemm_tma_kernel<tma::EPI_MAT><<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml, mh, ml);
   MM_LAUNCH_CHECK();
   return 0;
 }
@@ -1025,7 +1024,7 @@ struct ConvPlan {
   int bx, by, bi;          // box of 256 pixels (powers of two)
   int ksegs, kc_per_seg;   // K accumulated in ksegs passes of kc_per_seg 32-wide chunks
   int tiles_x, tiles_y, num_tiles;   // column tiles (boxes); the channel-major kernel runs ceil(M/128) row tiles of each
-  int acc_epi;             // channel-major: epilogue from the wgmma accumulators, TMA stores (gemm_tma_kernel<true>)
+  int acc_epi;             // channel-major: epilogue from the wgmma accumulators, TMA stores (EPI_CONV_ACC)
 };
 // want_pool: the caller takes a fused pooled map; use_kseg: the caller provides K-segment scratch.
 // dbg / seg_chunks: mmmot_set_debug / mmmot_set_kseg state.
@@ -1045,15 +1044,15 @@ static inline ConvPlan conv_plan(int M, bool part, int n_img, int H, int W, int 
   const int kchunks = 9 * C / tc::BK;
   // 64-channel outputs run on the pixel-major kernel (gemm_tma_px.cuh); it prefers a 16 x 16 single-image box
   // (vertical taps from one halo box, 2x2 pooling windows inside a warp) when that wastes no more than the best box
-  c.px = M == 64 && !part && !(dbg & 64) && !(use_kseg && seg_chunks > 0 && kchunks > seg_chunks);
+  c.px = M == 64 && !part && !(dbg & MM_DBG_CM64) && !(use_kseg && seg_chunks > 0 && kchunks > seg_chunks);
   if (c.px && conv_box_waste(1, H, W, 16, 16, 1) <= best + 1e-9) { c.bx = 16; c.by = 16; c.bi = 1; }
   if (c.px) {
-    c.halo = (c.bi == 1 && c.bx >= 8 && c.bx * (c.by + 2) * 64 <= tma::PX_X_PLANE && !(dbg & 256)) ? 1 : 0;
-    c.pool = want_pool && c.bx >= 2 && c.bx <= 16 && c.by >= 2 && !(H & 1) && !(W & 1) && !(dbg & 512);
+    c.halo = (c.bi == 1 && c.bx >= 8 && c.bx * (c.by + 2) * 64 <= tma::PX_X_PLANE && !(dbg & MM_DBG_PX_NO_HALO)) ? 1 : 0;
+    c.pool = want_pool && c.bx >= 2 && c.bx <= 16 && c.by >= 2 && !(H & 1) && !(W & 1) && !(dbg & MM_DBG_NO_FUSED_POOL);
   } else {
     // channel-major kernel: the 2x2 max-pool (and SkipPool's per-image sums) fused into the epilogue when every pooling
     // window lies inside one thread's chunks: box rows of <= 32 pixels, an even number of box rows per 128-column half
-    c.pool = want_pool && c.bx >= 2 && c.bx <= 32 && c.by >= 2 && !(H & 1) && !(W & 1) && !(dbg & 512);
+    c.pool = want_pool && c.bx >= 2 && c.bx <= 32 && c.by >= 2 && !(H & 1) && !(W & 1) && !(dbg & MM_DBG_NO_FUSED_POOL);
   }
   c.ksegs = 1; c.kc_per_seg = kchunks;
   if (use_kseg && seg_chunks > 0 && kchunks > seg_chunks) {
@@ -1065,7 +1064,7 @@ static inline ConvPlan conv_plan(int M, bool part, int n_img, int H, int W, int 
   // The accumulator epilogue stores 64-channel boxes and runs single-pass K only: combining K segments' partial sums
   // from the registers through L2 measured slower than the accumulator image on the H100 (DESIGN §4.2).  Debug bit 11
   // keeps the accumulator-image epilogue (A/B runs).
-  c.acc_epi = !c.px && !part && !(dbg & 2048) && M >= 64 && c.ksegs == 1;
+  c.acc_epi = !c.px && !part && !(dbg & MM_DBG_CONV_IMAGE) && M >= 64 && c.ksegs == 1;
   return c;
 }
 
@@ -1086,30 +1085,20 @@ static int gemm_tma_launch_conv(const GemmP& g0, const uint4* Wp, float out_scal
   if (plan) *plan = c;
   int sms = 0;
   MM_TRY(mm_sm_count(&sms));
-  tma::TmaP P;
-  memset(&P, 0, sizeof(P));
   GemmP g = g0;
   g.K = 9 * C;
-  P.conv = 1; P.bx = c.bx; P.by = c.by; P.bi = c.bi;
+  g.num_tiles = c.num_tiles;
+  g.tile_tab = nullptr;
+  g.Y = reinterpret_cast<float*>(Yhi);
+  g.y_ms = g.M;
+  tma::TmaP P = tma_params(g, Wp, out_scale, tma::OUT_PLANAR, c.pool ? y_plane_pooled : y_plane, status);
+  P.bx = c.bx; P.by = c.by; P.bi = c.bi;
   P.halo = c.halo;
   P.pool = c.pool;
   if (c.pool) *did_pool = 1;
   if (c.pool && !c.px) P.pool_sum = pool_sum;
   P.tiles_x = c.tiles_x; P.tiles_y = c.tiles_y;
   P.n_img = n_img; P.H = H; P.W = W; P.C = C;
-  g.num_tiles = c.num_tiles;
-  g.tile_tab = nullptr;
-  g.Y = reinterpret_cast<float*>(Yhi);
-  g.y_ms = g.M;
-  P.t.g = g;
-  P.t.Wp = Wp;
-  P.t.m_tiles = (g.M + 127) / 128;
-  P.t.k_chunks = g.K / tc::BK;
-  P.t.out_scale = out_scale;
-  P.t.out_mode = tma::OUT_PLANAR;
-  P.t.dbg = mm_debug_flags();
-  P.plane_elems = P.pool ? y_plane_pooled : y_plane;
-  P.status = status;
   P.ksegs = c.ksegs; P.kc_per_seg = c.kc_per_seg;
   if (c.ksegs > 1) P.acc_scratch = acc_scratch;
   alignas(64) CUtensorMap mh, ml;
@@ -1124,16 +1113,16 @@ static int gemm_tma_launch_conv(const GemmP& g0, const uint4* Wp, float out_scal
   const int grid = (int)(total < sms ? total : sms);
   if (c.acc_epi) {
     static std::atomic<unsigned long long> attr{0};
-    MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<true>, tma::T_CONV_SMEM_BYTES, attr));
+    MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<tma::EPI_CONV_ACC>, tma::T_CONV_SMEM_BYTES, attr));
     const int sh = c.pool ? 1 : 0;
     alignas(64) CUtensorMap oh, ol;
     MM_TRY(tma::make_map_4d_store(&oh, Yhi, n_img, H >> sh, W >> sh, g.M, c.bx >> sh, c.by >> sh, c.bi));
     MM_TRY(tma::make_map_4d_store(&ol, Yhi + P.plane_elems, n_img, H >> sh, W >> sh, g.M, c.bx >> sh, c.by >> sh, c.bi));
-    tma::gemm_tma_kernel<true><<<grid, tma::T_THREADS, tma::T_CONV_SMEM_BYTES, st>>>(P, mh, ml, oh, ol);
+    tma::gemm_tma_kernel<tma::EPI_CONV_ACC><<<grid, tma::T_THREADS, tma::T_CONV_SMEM_BYTES, st>>>(P, mh, ml, oh, ol);
   } else {
     static std::atomic<unsigned long long> attr{0};
-    MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<false>, tma::T_SMEM_BYTES, attr));
-    tma::gemm_tma_kernel<false><<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml, mh, ml);
+    MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<tma::EPI_CONV_IMAGE>, tma::T_SMEM_BYTES, attr));
+    tma::gemm_tma_kernel<tma::EPI_CONV_IMAGE><<<grid, tma::T_THREADS, tma::T_SMEM_BYTES, st>>>(P, mh, ml, mh, ml);
   }
   MM_LAUNCH_CHECK();
   return 0;

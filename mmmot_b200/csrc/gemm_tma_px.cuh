@@ -60,7 +60,8 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const long total_tiles = p.num_tiles;
   const int KC = P.t.k_chunks;
-  const int cchunks = P.conv ? P.C / BK : KC;
+  const bool conv = P.C > 0;                             // matrix launches leave the conv geometry 0
+  const int cchunks = conv ? P.C / BK : KC;
   const int ntap = P.halo ? 3 : 1;                       // vertical taps served by one stage
   const int nstage = P.halo ? 3 * cchunks : KC;          // stages per tile
   const uint32_t xbytes = P.halo ? (uint32_t)(P.bx * (P.by + 2) * 64) : (uint32_t)B_HALF;
@@ -74,13 +75,6 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-
-  auto conv_origin = [&](int nt, int& i0, int& y0, int& x0) {
-    const int tx = nt % P.tiles_x;
-    const int r = nt / P.tiles_x;
-    const int ty = r % P.tiles_y;
-    i0 = (r / P.tiles_y) * P.bi; y0 = ty * P.by; x0 = tx * P.bx;
-  };
 
   if (warp < T_EPI_WARPS) {
     // =============================== CONSUMERS: wgmma + epilogue ===============================
@@ -99,13 +93,13 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
     for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       const int nt = (int)t;
       int i0 = 0, y0 = 0, x0 = 0;
-      if (P.conv) conv_origin(nt, i0, y0, x0);
+      if (conv) conv_origin(P, nt, i0, y0, x0);
       // ---- main loop: pixels 128 wg .. 128 wg + 127 x 64 channels, two m64n64 wgmma chains ----
       for (int si = 0; si < nstage; si++, it++) {
         const int s = it % PX_STAGES;
         mbar_wait(full_bar(s), (it / PX_STAGES) & 1);
         const uint32_t sw = base + s * PX_STAGE, sx = sw + PX_X_OFF;
-        if (!(P.t.dbg & 8)) {
+        if (!(P.t.dbg & MM_DBG_SKIP_MMA)) {
           wgmma_fence();
           for (int ky = 0; ky < ntap; ky++) {
             const uint32_t xo = sx + (uint32_t)(ky * P.bx * 64 + wg * (128 * 64)), wo = sw + (uint32_t)(ky * PX_W_SLOT);
@@ -148,7 +142,7 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
         const int col = sub * 128 + q * 32 + lane;
         bool ok;
         long o;
-        if (P.conv) {
+        if (conv) {
           const int xx = col & (P.bx - 1), r = col >> lbx;
           const int yy = r & (P.by - 1), ii = r >> lby;
           const int img = i0 + ii, y = y0 + yy, xg = x0 + xx;
@@ -161,7 +155,7 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
         }
         uint32_t v[32];
         acc_ld32(img, 64, sub * 128 + q * 32 + lane, cb, v);
-        if (P.t.dbg & 1) continue;
+        if (P.t.dbg & MM_DBG_SKIP_EPI) continue;
         if (P.pool) {
           // 2x2 max over lanes l, l^1 (x) and l^bx (y); bias + ReLU commute with the max and are applied below
 #pragma unroll
@@ -220,7 +214,7 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
             if (row0 + px < p.S) st_global_256(dstp + (long)px * 64 + c * 8, w);
           }
           asm volatile("bar.sync %0, 64;" ::"r"(3 + q) : "memory");   // scratch free for the next subtile
-        } else if (ok && !(P.t.dbg & 128)) {
+        } else if (ok && !(P.t.dbg & MM_DBG_PX_ST16)) {
           // 256-bit stores: every instruction writes whole 32-byte sectors (two per plane per thread)
           st_global_256(yh + o, hi);
           st_global_256(yh + o + 16, hi + 8);
@@ -261,7 +255,7 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
       mbar_wait(empty_bar(s), ((it / PX_STAGES) & 1) ^ 1);
       float* stg = reinterpret_cast<float*>(sm + s * PX_STAGE + PX_W_SLOT);
       const int lin0 = r0 - W - 1;
-      if (P.t.dbg & 4) {                         // A/B: no operand generation (results wrong)
+      if (P.t.dbg & MM_DBG_SKIP_OPERANDS) {      // A/B: no operand generation (results wrong)
         __syncwarp();
         if (lane == 0) mbar_arrive(full_bar(s));
         continue;
@@ -328,7 +322,7 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
       for (long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         const int nt = (int)t;
         int i0 = 0, y0 = 0, x0 = 0;
-        if (P.conv) conv_origin(nt, i0, y0, x0);
+        if (conv) conv_origin(P, nt, i0, y0, x0);
         for (int si = 0; si < nstage; si++, it++) {
           const int s = it % PX_STAGES;
           mbar_wait(empty_bar(s), ((it / PX_STAGES) & 1) ^ 1);
@@ -351,7 +345,7 @@ gemm_tma_px_kernel(const TmaP P, const __grid_constant__ CUtensorMap map_hi, con
           if (P.halo) {
             tma_load_4d(sx, &map_hi, cc * BK, x0 + kx - 1, y0 - 1, i0, full_bar(s));
             tma_load_4d(sx + PX_X_PLANE, &map_lo, cc * BK, x0 + kx - 1, y0 - 1, i0, full_bar(s));
-          } else if (P.conv) {
+          } else if (conv) {
             const int tap = si / cchunks, c2 = si - tap * cchunks;
             const int dx = tap % 3 - 1, dy = tap / 3 - 1;
             tma_load_4d(sx, &map_hi, c2 * BK, x0 + dx, y0 + dy, i0, full_bar(s));

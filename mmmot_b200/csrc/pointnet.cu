@@ -582,7 +582,7 @@ int pn_wide_stats(const PnWs& w, const int* h_det_split, const int* det_split, l
                   const __half* X, int K, const float* Wt, const uint4* Wp, float wps, const float* bias, int M,
                   const float* addend, cudaStream_t st) {
   const bool timed = mm_timing_on();
-  if (mm_debug_flags() & 16) {
+  if (mm_debug_flags() & MM_DBG_PN_STATS_PASS) {
     GemmP p = gemm_defaults();
     p.bias = bias; p.M = M; p.K = K;
     p.tile_tab = w.tiles; p.num_tiles = (int)n_tiles;
@@ -675,7 +675,7 @@ int pointnet_tc(const mmmot_weights* wts, const float* points, const int* det_sp
   MM_LAUNCH_CHECK();
   if (timed) mm_timing_end(st);
   float* const ys[3] = {w.t0, w.t1, w.t0};             // outputs of layers 2, 3, 4
-  const bool gen_mid = !(mm_debug_flags() & 8192);   // debug bit 13: layers 3, 4 through norm_split + the TMA-fed kernel
+  const bool gen_mid = !(mm_debug_flags() & MM_DBG_PN_NORM_SPLIT);   // layers 3, 4 through norm_split + the TMA-fed kernel
   for (int i = 1; i < 4; i++) {
     const float* const* q = &wts->w[MMMOT_W_PN_L1 + 4 * i];
     const int cin = 64, cout = i == 3 ? 128 : 64;
@@ -923,7 +923,7 @@ extern "C" int mmmot_debug_pn_stats(const int* det_split, const int* h_det_split
   if (!det_split || !h_det_split || pairs <= 0 || L <= 0 || !Xhi || !bias || !gamma || !beta || !sc || !sh || !workspace)
     return MMMOT_E_ARG;
   if (!(K == 64 || (K == 128 && !addend)) || M <= 0 || M > 1024 || M % 64) return MMMOT_E_ARG;
-  const bool two_pass = mm_debug_flags() & 16;
+  const bool two_pass = mm_debug_flags() & MM_DBG_PN_STATS_PASS;
   if (two_pass ? !Wp : !Wt) return MMMOT_E_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   const int ndet = pairs * L;

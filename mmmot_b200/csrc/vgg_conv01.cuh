@@ -322,7 +322,7 @@ static __global__ void __launch_bounds__(F01_THREADS, 1) vgg_conv01_kernel(const
 // W <= 512) and layer 1 on the pixel-major kernel with 16 x 16 halo boxes and the fused pool (no K segments) — and
 // the 16 x 16 tiles cover the image (H, W multiples of 16).  Debug bit 15 forces the two launches.
 static inline bool vgg_conv01_fused(int n_img, int H, int W, bool compact_tiles, int dbg, int kseg) {
-  if (!compact_tiles || (dbg & (32 | 16384 | 32768)) || n_img <= 0) return false;
+  if (!compact_tiles || (dbg & (MM_DBG_VGG0_FFMA | MM_DBG_VGG0_IM2COL | MM_DBG_VGG01_UNFUSED)) || n_img <= 0) return false;
   if (H % tma::F01_TILE || W % tma::F01_TILE || W > 512 || (long)n_img * H * W >= (1L << 31)) return false;
   const ConvPlan c = conv_plan(64, false, n_img, H, W, 64, true, true, dbg, kseg);
   return c.px && c.halo && c.pool && c.bx == tma::F01_TILE && c.by == tma::F01_TILE && c.bi == 1 && c.ksegs == 1;

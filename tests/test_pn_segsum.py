@@ -247,3 +247,18 @@ def test_segsum_kernels_do_not_spill():
         found[int(m.group(2))] = (int(spill.group(1)), int(spill.group(2)))
     assert found == {64: (0, 0), 128: (0, 0)}, found
     assert not re.search(r"C75\d\d\).*gemm_segsum_kernel", log)
+
+
+def test_tma_kernels_do_not_spill():
+    """ptxas -v of appearance.cu (written by the Makefile): every gemm_tma_kernel instantiation (matrix, conv through the
+    accumulator image, conv from the accumulators) reports no spill stores or loads."""
+    log_path = os.path.join(os.path.dirname(PTXAS_LOG), "appearance.ptxas.log")
+    if not os.path.exists(log_path):
+        pytest.skip("no ptxas log: the library was not built in this tree")
+    log = open(log_path).read()
+    found = {}
+    for m in re.finditer(r"Compiling entry function '(\w*gemm_tma_kernelILi(\d+)E\w*)'.*?\n(.*?\n.*?)\n", log):
+        spill = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", m.group(3))
+        assert spill, m.group(0)
+        found[int(m.group(2))] = (int(spill.group(1)), int(spill.group(2)))
+    assert found == {0: (0, 0), 1: (0, 0), 2: (0, 0)}, found
