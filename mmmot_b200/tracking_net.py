@@ -10,11 +10,13 @@ module lives on a CUDA device and the shared library loads.
 
 New relative to the reference (which handles one frame-pair per call, SURVEY F12):
 ``forward_batch`` runs B independent frame-pairs in one pass with per-pair semantics identical
-to ``forward``, and ``predict_batch`` also solves the association programme on the device.
+to ``forward``, and ``predict_batch`` also solves the association programme on the device.  With ``counts`` both run
+B windows of K >= 2 frames that share the per-frame detection counts, each identical to ``forward`` on that window.
 ``forward_stack`` and the ``stack`` argument of ``forward_batch`` / ``predict_batch`` compute one
 feature stack alone (image, LiDAR or fused), so a tracker runs without the sensor it does not read.
 """
 import ctypes
+import operator
 
 import torch
 import torch.nn as nn
@@ -297,15 +299,36 @@ class TrackingNet(nn.Module):
         if int(status) & 1:
             _lib.check(-4, "mmmot_b200.TrackingNet forward")
 
-    def _pick_chunk(self, B, n, m, P_per_pair, H, W, dev, stack=None):
+    def _pick_chunk(self, B, counts, P_per_pair, H, W, dev, stack=None):
+        """Samples per chunk: halved from B until the workspace of a chunk (the feature stages on its L = sum(counts)
+        detections and the affinity stage of every pair of consecutive frames) fits half the free device memory."""
         if self.chunk_pairs:
             return min(B, self.chunk_pairs)
         free, _ = torch.cuda.mem_get_info(dev)
         budget = min(free * 0.5, 48e9)
+        transitions = list(zip(counts[:-1], counts[1:]))
         c = B
-        while c > 1 and self._workspace_bytes(c, [(n, m)], n + m, int(P_per_pair * c) + 1, H, W, stack) > budget:
+        while c > 1 and self._workspace_bytes(c, transitions, sum(counts), int(P_per_pair * c) + 1, H, W, stack) > budget:
             c = (c + 1) // 2
         return c
+
+    @staticmethod
+    def _frame_counts(n, m, counts):
+        """The per-frame detection counts of a batched call: [n, m] (m defaults to n) for frame-pairs, else `counts`
+        (K >= 2 positive ints).  Raises ValueError for a call that gives both or neither, or a bad count."""
+        if counts is None:
+            if n is None:
+                raise ValueError("give the detections per frame: n (and m) for frame-pairs, or counts")
+            return [n, n if m is None else m]
+        if n is not None or m is not None:
+            raise ValueError("give either n, m or counts, not both")
+        try:
+            counts = [operator.index(c) for c in counts]
+        except TypeError:
+            raise ValueError(f"counts must be a sequence of ints, got {counts!r}") from None
+        if len(counts) < 2 or min(counts) < 1:
+            raise ValueError(f"counts must hold K >= 2 frames of at least one detection each, got {counts}")
+        return counts
 
     @staticmethod
     def _check_stack(stack):
@@ -330,7 +353,8 @@ class TrackingNet(nn.Module):
             raise _lib.MmmotError(f"stack {stack} needs the {missing} input, which was not given")
 
     @torch.no_grad()
-    def forward_batch(self, crops, points, points_split, n, m=None, keep_feats=False, check=True, stack=None):
+    def forward_batch(self, crops, points, points_split, n=None, m=None, keep_feats=False, check=True, stack=None,
+                      counts=None):
         """B independent frame-pairs, each with n previous and m next detections.
 
         crops         (B*(n+m)) x 3 x H x W  fp32, CUDA
@@ -348,17 +372,30 @@ class TrackingNet(nn.Module):
         stack (None: every stack): 0, 1 or 2 computes that stack alone, bit-identical to forward_batch()[:, stack:stack+1]:
         the appearance trunk is skipped for 1 (LiDAR) and PointNet for 0 (image), and the input the stack does not need
         may be None (crops for 1; points and points_split for 0).  The returned tensors keep a stack axis of size 1.
+
+        counts (n_0, ..., n_{K-1}), K >= 2, in place of n, m: B windows of K frames with these detection counts, L =
+        sum(counts) detections each, packed as above (crops B*L rows, points_split B*L + 1 offsets).  Per sample this is
+        ``forward`` on a K-frame sample, bit for bit: the feature stages run once over the sample's L detections, then
+        the affinity stage on every pair of consecutive frames, for all samples of a chunk at once.  link is then a list
+        of K - 1 tensors B x ns x n_k x n_k+1, new B x ns x (L - n_0) and end B x ns x (L - n_{K-1}) (un-padded, as
+        above; ns = 3, or 1 with ``stack``).  counts = (n, m) gives the tensors of (n, m), link in a one-element list.
         """
         self._check_stack(stack)
+        windowed = counts is not None
+        counts = self._frame_counts(n, m, counts)
         if self.training:
             raise NotImplementedError("mmmot_b200.TrackingNet implements the eval-mode forward only (SURVEY §8f N4)")
-        m = n if m is None else m
-        L = n + m
+        L = sum(counts)
+        transitions = list(zip(counts[:-1], counts[1:]))
         use_img, use_pts = stack != 1, stack != 0
         if stack is not None:
             self._require(stack, crops is not None, points is not None and points_split is not None)
         if use_pts:
             self._check_points(points)
+        split = points_split.detach().to("cpu", torch.int32).contiguous() if use_pts else None
+        rows = crops.shape[0] if use_img else split.numel() - 1
+        if rows % L or (use_pts and split.numel() != rows + 1):
+            raise _lib.MmmotError("crops / points_split do not match " + ("counts" if windowed else "n, m"))
         lib = _lib.load()
         wts = self.prepared()
         dev = wts.flat.device
@@ -366,10 +403,6 @@ class TrackingNet(nn.Module):
             raise _lib.MmmotError("inputs must live on the module's CUDA device")
         crops = crops.contiguous().float() if use_img else None
         points = _aligned_rows(points.contiguous().float()) if use_pts else None
-        split = points_split.detach().to("cpu", torch.int32).contiguous() if use_pts else None
-        rows = crops.shape[0] if use_img else split.numel() - 1
-        if rows % L or (use_pts and split.numel() != rows + 1):
-            raise _lib.MmmotError("crops / points_split do not match n, m")
         B = rows // L
         H, W = crops.shape[-2:] if use_img else (0, 0)
         ns = 3 if stack is None else 1
@@ -377,13 +410,13 @@ class TrackingNet(nn.Module):
             "status": torch.zeros(1, dtype=torch.int32, device=dev),
             "feats": torch.empty(B, 3, 512, L, device=dev),
             "det": torch.empty(B, ns, L, device=dev),
-            "link": torch.empty(B, ns, n, m, device=dev),
-            "new": torch.empty(B, ns, m, device=dev),
-            "end": torch.empty(B, ns, n, device=dev),
+            "link": [torch.empty(B, ns, a, b, device=dev) for a, b in transitions],
+            "new": [torch.empty(B, ns, b, device=dev) for _, b in transitions],
+            "end": [torch.empty(B, ns, a, device=dev) for a, _ in transitions],
         }
         with torch.cuda.device(dev):        # the library works on the CURRENT device
             st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            chunk = self._pick_chunk(B, n, m, int(split[-1]) / B if use_pts else 0, H, W, dev, stack)
+            chunk = self._pick_chunk(B, counts, int(split[-1]) / B if use_pts else 0, H, W, dev, stack)
             for p0 in range(0, B, chunk):
                 pc = min(chunk, B - p0)
                 s_host, pts = None, None
@@ -393,15 +426,24 @@ class TrackingNet(nn.Module):
                     s_host = (s_host - off).contiguous()
                     pts = points[off:off + int(s_host[-1])]
                 P = int(s_host[-1]) if use_pts else 0
-                ws = self._workspace(self._workspace_bytes(pc, [(n, m)], L, P, H, W, stack), dev)
+                ws = self._workspace(self._workspace_bytes(pc, transitions, L, P, H, W, stack), dev)
                 _lib.check(lib.mmmot_status_reset(_vp(ws), st), "mmmot_status_reset")
                 feats = out["feats"][p0:p0 + pc]
                 self._features(wts, ws, st, crops[p0 * L:(p0 + pc) * L] if use_img else None, pts, s_host, pc, L, feats,
                                out["det"][p0:p0 + pc], stack)
-                self._associate(wts, ws, st, pc, n, m, feats, out["link"][p0:p0 + pc], out["new"][p0:p0 + pc],
-                                out["end"][p0:p0 + pc], stack)
+                start = 0
+                for k, (a, b) in enumerate(transitions):
+                    # the two frames' feature columns of every sample as one contiguous slab (no copy for two frames)
+                    self._associate(wts, ws, st, pc, a, b, feats[:, :, :, start:start + a + b].contiguous(),
+                                    out["link"][k][p0:p0 + pc], out["new"][k][p0:p0 + pc], out["end"][k][p0:p0 + pc], stack)
+                    start += a
                 # the status word (FP16 range flag) of this chunk, accumulated into out["status"] in stream order
                 out["status"] |= ws[:4].view(torch.int32)
+        if windowed:
+            out["new"] = out["new"][0] if len(transitions) == 1 else torch.cat(out["new"], 2)
+            out["end"] = out["end"][0] if len(transitions) == 1 else torch.cat(out["end"], 2)
+        else:
+            out["link"], out["new"], out["end"] = out["link"][0], out["new"][0], out["end"][0]
         out["trans"] = [wts.trans1.unsqueeze(0).clone(), wts.trans2.unsqueeze(0).clone()]
         if keep_feats:
             out["feats"] = wts.narrow(out["feats"] if stack is None else out["feats"][:, stack:stack + 1])
@@ -435,20 +477,31 @@ class TrackingNet(nn.Module):
         return link, new, end
 
     @torch.no_grad()
-    def predict_batch(self, crops, points, points_split, n, m=None, check=True, stack=None):
+    def predict_batch(self, crops, points, points_split, n=None, m=None, check=True, stack=None, counts=None):
         """forward_batch + association programme on the ``test_mode`` stack, all on the device.
         Returns forward_batch's dict plus assign_{det,link,new,end} and match (B x n int32).
-        stack: computes that stack alone (forward_batch's ``stack``) and solves the programme on it."""
-        from .solvers import solve_batch
-        m = n if m is None else m
-        out = self.forward_batch(crops, points, points_split, n, m, check=check, stack=stack)
+        stack: computes that stack alone (forward_batch's ``stack``) and solves the programme on it.
+        counts: B windows of K frames (forward_batch's ``counts``), every sample's programme solved in one call:
+        assign_det/new/end B x L, assign_link a list of K - 1 tensors B x n_k x n_k+1, match B x (L - n_{K-1}) int32
+        (each detection's successor in the next frame, -1 = none; B x n_0 for two frames, as without counts)."""
+        from .solvers import solve_batch, solve_frames
+        out = self.forward_batch(crops, points, points_split, n, m, check=check, stack=stack, counts=counts)
+        windowed = counts is not None
+        counts = self._frame_counts(n, m, counts)
         B, t = out["det"].shape[0], self.test_mode if stack is None else 0
         ns = out["det"].shape[1]
-        zn = out["det"].new_zeros(B, ns, n)
-        zm = out["det"].new_zeros(B, ns, m)
+        zn = out["det"].new_zeros(B, ns, counts[0])
+        zm = out["det"].new_zeros(B, ns, counts[-1])
         new_p = torch.cat([zn, out["new"]], dim=2)      # tracking_net.py:183-189 zero padding
         end_p = torch.cat([out["end"], zm], dim=2)
-        out.update(solve_batch(out["det"][:, t], out["link"][:, t], new_p[:, t], end_p[:, t], n, m))
+        links = out["link"] if windowed else [out["link"]]
+        if len(counts) == 2:
+            res = solve_batch(out["det"][:, t], links[0][:, t], new_p[:, t], end_p[:, t], *counts)
+            if windowed:
+                res["assign_link"] = [res["assign_link"]]
+        else:
+            res = solve_frames(out["det"][:, t], [l[:, t] for l in links], new_p[:, t], end_p[:, t], counts)
+        out.update(res)
         return out
 
     # ------------------------------------------------------------------ training-mode forward (SURVEY §8f N4)
