@@ -293,7 +293,7 @@ AfWs carve(MmArena& a, size_t G, int n, int m) {
 
 // engine choice from the per-pair shape only (see appearance.cu); a quarter-filled 256-column tile on the tensor cores
 // still beats the FP32 engine (N = 8: 31k -> see DESIGN §6)
-bool affinity_use_tc(int n, int m) { return mm_engine() == 2 || (mm_engine() == 0 && n * m >= 64); }
+bool affinity_use_tc(int n, int m) { return mm_use_tc(n * m >= 64); }
 
 template <int GEN>
 int launch_gen(const GemmP& p, const mmmot_weights* wts, int wid, const float* src, int src_m, long src_rows,
@@ -330,39 +330,22 @@ int mm_affinity_layout(int pairs, int n, int m, size_t* off, int* tensor_cores) 
 
 namespace {
 
-// The stage on every stack (stack < 0: G = 3*pairs groups, group g reads feature block g) or on one (G = pairs, group g
-// reads block g*3 + stack).  Every plan choice depends on the per-pair shape only, so a group's results do not depend on
-// which of the two it runs in.
-int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs, int stack,
-                       int n, int m, const float* feats, float* link, float* new_s, float* end_s, void* workspace,
-                       size_t workspace_bytes, void* stream) {
-  if (!wts || !feats || !link || !new_s || !end_s || !workspace || pairs <= 0 || n <= 0 || m <= 0 || stack > 2)
-    return MMMOT_E_ARG;
-  if (affinity_op < 0 || affinity_op > MMMOT_AFF_MINUS || softmax_mode < 0 || softmax_mode > MMMOT_SM_DUAL_MAX ||
-      end_mode < MMMOT_END_AVG || end_mode > MMMOT_END_MAX)
-    return MMMOT_E_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  MmArena ar(workspace, workspace_bytes);
-  const int G = stack < 0 ? pairs * 3 : pairs, NM = n * m, L = n + m;
-  AfWs w = carve(ar, (size_t)G, n, m);
-  if (!ar.ok()) return MMMOT_E_WORKSPACE;
-  // group g's feature block [512][L]: fbase + g*fgs
-  const float* fbase = stack < 0 ? feats : feats + (long)stack * 512 * L;
-  const long fgs = (stack < 0 ? 1L : 3L) * 512 * L;
-  const bool use_tc = affinity_use_tc(n, m);
-  const int tpg = mm_cdiv(NM, use_tc ? tc::BN : 128);
+// Tensor-core path: every contraction on the generated-operand engine (gemm_gen.cuh), activations channels-last
+int affinity_tc(const mmmot_weights* wts, int affinity_op, int end_mode, int stack, int G, int n, int m, const float* fbase,
+                long fgs, const AfWs& w, int* status, float* zdst, float* new_s, float* end_s, cudaStream_t st) {
+  const int NM = n * m, L = n + m;
+  const long ldv = (long)G * (n + m);
+  const int tpg = mm_cdiv(NM, tc::BN);
   const float* const* W = wts->w;
   const bool timed = mm_timing_on();
 
-  // layer 1: [conv1.0 ; w_new_end.conv0] 512 -> 1024 on the generated pairwise tensor.
-  // FP32 engine: y01[g][1024][NM].  Tensor-core engine: channels-last y01[g*NM + s][1024].
-  const int pm = use_tc ? 2 : 1;   // GroupNorm partials per column tile
-  if (use_tc) {
-    MM_TRY(transpose_f32(fbase, w.fcl, 512, L, G, fgs, st));
-    // every stack: one contiguous range; one stack: a block per pair
-    feats_range_kernel<<<148, 256, 0, st>>>(fbase, stack < 0 ? (long)G * 512 * L : 512L * L, stack < 0 ? 1 : G, fgs,
-                                           affinity_op == MMMOT_AFF_MULTIPLY ? 255.9f : 65504.f, ar.status());
-    MM_LAUNCH_CHECK();
+  // layer 1: [conv1.0 ; w_new_end.conv0] 512 -> 1024 on the generated pairwise tensor, channels-last y01[g*NM + s][1024]
+  MM_TRY(transpose_f32(fbase, w.fcl, 512, L, G, fgs, st));
+  // every stack: one contiguous range; one stack: a block per pair
+  feats_range_kernel<<<148, 256, 0, st>>>(fbase, stack < 0 ? (long)G * 512 * L : 512L * L, stack < 0 ? 1 : G, fgs,
+                                         affinity_op == MMMOT_AFF_MULTIPLY ? 255.9f : 65504.f, status);
+  MM_LAUNCH_CHECK();
+  {
     GemmP p = gemm_defaults();
     p.bias = W[MMMOT_W_AF_B01]; p.M = 1024; p.K = 512;
     p.S = NM; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
@@ -376,7 +359,80 @@ int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mo
                 : launch_gen<gen::GEN_PAIR_SUB>(p, wts, MMMOT_W_AF_W01P, w.fcl, 0, 0, nullptr, nullptr, n, m, L, st);
     if (r) return r;
     if (timed) mm_timing_end(st);
-  } else {
+  }
+  // statistics are [G][1024]: channels 0..511 = conv1.0 -> GroupNorm(512,512) (per channel over N x M),
+  // 512..1023 = conv0 -> GroupNorm(1,512) (one group over 512 x N x M; new_end.py:50); 2 partials per column tile
+  MM_TRY(stats_reduce(w.part, 1024, G, tpg, nullptr, w.stats, st, 2));
+  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G1W], W[MMMOT_W_AF_G1B], nullptr, NM, G, 512, 1, w.sc1, w.sh1, st, 1024, 0, status));
+  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G0W], W[MMMOT_W_AF_G0B], nullptr, NM, G, 512, 512, w.sc0, w.sh0, st, 1024, 512));
+
+  // ---- new / end indicator on y0 = channels 512..1023 of y01 ----
+  if (timed) mm_timing_begin(st, MM_T_AFF_MEAN, 0.0, 4.0 * 512 * (double)G * NM);
+  newend_mean_cl_kernel<<<G * (n + m), 256, 0, st>>>(w.y01, 1024, 512, w.sc0, w.sh0, n, m, 0, w.v, end_mode);
+  MM_LAUNCH_CHECK();
+  if (timed) mm_timing_end(st);
+  const int tn = mm_cdiv(n, tc::BN), tm_ = mm_cdiv(m, tc::BN), ne_tiles = G * (tn + tm_);
+  ne_tiles_kernel<<<mm_cdiv(max(ne_tiles, 2 * G + 1), 128), 128, 0, st>>>(G, n, m, tn, tm_, tc::BN, w.tiles, w.cnt, w.gstart);
+  MM_LAUNCH_CHECK();
+  {
+    // shared Conv1d MLP on the new / end vectors (new_end.py:53-60): rows = columns of V (channels-last), groups =
+    // (g, new | end) through the tile table
+    GemmP p = gemm_defaults();
+    p.bias = W[MMMOT_W_NE_B1]; p.M = 512; p.K = 512;
+    p.tile_tab = w.tiles; p.num_tiles = ne_tiles;
+    p.Y = w.h1; p.y_ms = 512;
+    p.part = w.npart;
+    MM_TRY(launch_gen<gen::GEN_COPY>(p, wts, MMMOT_W_NE_W1P, w.v, 512, 0, nullptr, nullptr, 0, 0, 0, st));
+    MM_TRY(stats_reduce(w.npart, 512, 2 * G, 0, w.gstart, w.nstats, st, 2));
+    MM_TRY(gn_finalize(w.nstats, W[MMMOT_W_NE_G1W], W[MMMOT_W_NE_G1B], w.cnt, 0, 2 * G, 512, 512, w.nsc1, w.nsh1, st, 0, 0, status));
+    p.bias = W[MMMOT_W_NE_B2]; p.M = 128;
+    p.Y = w.h2; p.y_ms = 128;
+    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_NE_W2P, w.h1, 512, ldv, w.nsc1, w.nsh1, 0, 0, 0, st));
+    MM_TRY(stats_reduce(w.npart, 128, 2 * G, 0, w.gstart, w.nstats, st, 2));
+    MM_TRY(gn_finalize(w.nstats, W[MMMOT_W_NE_G2W], W[MMMOT_W_NE_G2B], w.cnt, 0, 2 * G, 128, 128, w.nsc2, w.nsh2, st));
+  }
+  ne_final_cl_kernel<<<mm_cdiv((long)G * (n + m) * 32, 256), 256, 0, st>>>(w.h2, w.nsc2, w.nsh2, W[MMMOT_W_NE_W3], W[MMMOT_W_NE_B3],
+                                                                          G, n, m, new_s, end_s);
+  MM_LAUNCH_CHECK();
+
+  // ---- affinity MLP layers 2, 3 on y1 = channels 0..511 of y01 ----
+  GemmP p = gemm_defaults();
+  p.bias = W[MMMOT_W_AF_B2]; p.M = 512; p.K = 512;
+  p.S = NM; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
+  p.x_gs = NM;
+  p.Y = w.y2; p.y_gs = NM; p.y_ms = 512;
+  p.part = w.part;
+  if (timed) mm_timing_begin(st, MM_T_AFF_L2, 2.0 * 512 * 512 * (double)G * NM, 4.0 * (512 + 512) * (double)G * NM);
+  MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W2P, w.y01, 1024, (long)G * NM, w.sc1, w.sh1, 0, 0, 0, st));
+  if (timed) mm_timing_end(st);
+  MM_TRY(stats_reduce(w.part, 512, G, tpg, nullptr, w.stats, st, 2));
+  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G2W], W[MMMOT_W_AF_G2B], nullptr, NM, G, 512, 1, w.sc2, w.sh2, st, 0, 0, status));
+  p.bias = W[MMMOT_W_AF_B3]; p.M = 128;
+  p.Y = w.y3; p.y_ms = 128;
+  if (timed) mm_timing_begin(st, MM_T_AFF_L3, 2.0 * 128 * 512 * (double)G * NM, 4.0 * (512 + 128) * (double)G * NM);
+  MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W3P, w.y2, 512, (long)G * NM, w.sc2, w.sh2, 0, 0, 0, st));
+  if (timed) mm_timing_end(st);
+  MM_TRY(stats_reduce(w.part, 128, G, tpg, nullptr, w.stats, st, 2));
+  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G3W], W[MMMOT_W_AF_G3B], nullptr, NM, G, 128, 1, w.sc3, w.sh3, st));
+  if (timed) mm_timing_begin(st, MM_T_AFF_LOGIT, 2.0 * 128 * (double)G * NM, 4.0 * 129 * (double)G * NM);
+  const long lrows = (long)G * NM;
+  link_logit_cl_kernel<<<(int)std::min<long>(148L * 8, (lrows + 31) / 32), 256, 0, st>>>(w.y3, w.sc3, w.sh3, W[MMMOT_W_AF_W4],
+                                                                                    W[MMMOT_W_AF_B4], lrows, NM, zdst);
+  MM_LAUNCH_CHECK();
+  if (timed) mm_timing_end(st);
+  return 0;
+}
+
+// FP32 path: channel-major activations y[g][C][NM], every layer stored
+int affinity_fp32(const mmmot_weights* wts, int affinity_op, int end_mode, int G, int n, int m, const float* fbase, long fgs,
+                  const AfWs& w, int* status, float* zdst, float* new_s, float* end_s, cudaStream_t st) {
+  const int NM = n * m, L = n + m;
+  const long ldv = (long)G * (n + m);
+  const int tpg = mm_cdiv(NM, 128);
+  const float* const* W = wts->w;
+
+  // layer 1: [conv1.0 ; w_new_end.conv0] 512 -> 1024 on the generated pairwise tensor, y01[g][1024][NM]
+  {
     GemmP p = gemm_defaults();
     p.Wt = W[MMMOT_W_AF_W01T]; p.bias = W[MMMOT_W_AF_B01]; p.ldw = 1024; p.M = 1024; p.K = 512;
     p.S = NM; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
@@ -388,48 +444,19 @@ int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mo
                                                  : gemm_simt_launch<XM_PAIR_SUB>(p, st);
     if (r) return r;
   }
-  // statistics are [G][1024]: channels 0..511 = conv1.0 -> GroupNorm(512,512) (per channel over N x M),
-  // 512..1023 = conv0 -> GroupNorm(1,512) (one group over 512 x N x M; new_end.py:50)
-  MM_TRY(stats_reduce(w.part, 1024, G, tpg, nullptr, w.stats, st, pm));
-  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G1W], W[MMMOT_W_AF_G1B], nullptr, NM, G, 512, 1, w.sc1, w.sh1, st, 1024, 0, ar.status()));
+  // statistics as on the tensor-core path, 1 partial per column tile
+  MM_TRY(stats_reduce(w.part, 1024, G, tpg, nullptr, w.stats, st, 1));
+  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G1W], W[MMMOT_W_AF_G1B], nullptr, NM, G, 512, 1, w.sc1, w.sh1, st, 1024, 0, status));
   MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G0W], W[MMMOT_W_AF_G0B], nullptr, NM, G, 512, 512, w.sc0, w.sh0, st, 1024, 512));
 
   // ---- new / end indicator on y0 = channels 512..1023 of y01 ----
-  const long ldv = (long)G * (n + m);
-  if (use_tc) {
-    if (timed) mm_timing_begin(st, MM_T_AFF_MEAN, 0.0, 4.0 * 512 * (double)G * NM);
-    newend_mean_cl_kernel<<<G * (n + m), 256, 0, st>>>(w.y01, 1024, 512, w.sc0, w.sh0, n, m, 0, w.v, end_mode);
-    MM_LAUNCH_CHECK();
-    if (timed) mm_timing_end(st);
-  } else {
-    rowcol_mean_kernel<<<G * 512, 256, 8 * m * sizeof(float), st>>>(w.y01 + 512L * NM, 1024L * NM, w.sc0, w.sh0,
-                                                               n, m, ldv, w.v, end_mode);
-    MM_LAUNCH_CHECK();
-  }
-  const int tw = use_tc ? tc::BN : 128;
-  const int tn = mm_cdiv(n, tw), tm_ = mm_cdiv(m, tw), ne_tiles = G * (tn + tm_);
-  ne_tiles_kernel<<<mm_cdiv(max(ne_tiles, 2 * G + 1), 128), 128, 0, st>>>(G, n, m, tn, tm_, tw, w.tiles, w.cnt, w.gstart);
+  rowcol_mean_kernel<<<G * 512, 256, 8 * m * sizeof(float), st>>>(w.y01 + 512L * NM, 1024L * NM, w.sc0, w.sh0,
+                                                             n, m, ldv, w.v, end_mode);
   MM_LAUNCH_CHECK();
-  if (use_tc) {
-    // shared Conv1d MLP on the new / end vectors (new_end.py:53-60) on the tensor cores: rows = columns of V
-    // (channels-last), groups = (g, new | end) through the tile table
-    GemmP p = gemm_defaults();
-    p.bias = W[MMMOT_W_NE_B1]; p.M = 512; p.K = 512;
-    p.tile_tab = w.tiles; p.num_tiles = ne_tiles;
-    p.Y = w.h1; p.y_ms = 512;
-    p.part = w.npart;
-    MM_TRY(launch_gen<gen::GEN_COPY>(p, wts, MMMOT_W_NE_W1P, w.v, 512, 0, nullptr, nullptr, 0, 0, 0, st));
-    MM_TRY(stats_reduce(w.npart, 512, 2 * G, 0, w.gstart, w.nstats, st, 2));
-    MM_TRY(gn_finalize(w.nstats, W[MMMOT_W_NE_G1W], W[MMMOT_W_NE_G1B], w.cnt, 0, 2 * G, 512, 512, w.nsc1, w.nsh1, st, 0, 0, ar.status()));
-    p.bias = W[MMMOT_W_NE_B2]; p.M = 128;
-    p.Y = w.h2; p.y_ms = 128;
-    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_NE_W2P, w.h1, 512, ldv, w.nsc1, w.nsh1, 0, 0, 0, st));
-    MM_TRY(stats_reduce(w.npart, 128, 2 * G, 0, w.gstart, w.nstats, st, 2));
-    MM_TRY(gn_finalize(w.nstats, W[MMMOT_W_NE_G2W], W[MMMOT_W_NE_G2B], w.cnt, 0, 2 * G, 128, 128, w.nsc2, w.nsh2, st));
-    ne_final_cl_kernel<<<mm_cdiv((long)G * (n + m) * 32, 256), 256, 0, st>>>(w.h2, w.nsc2, w.nsh2, W[MMMOT_W_NE_W3], W[MMMOT_W_NE_B3],
-                                                                            G, n, m, new_s, end_s);
-    MM_LAUNCH_CHECK();
-  } else {
+  const int tn = mm_cdiv(n, 128), tm_ = mm_cdiv(m, 128), ne_tiles = G * (tn + tm_);
+  ne_tiles_kernel<<<mm_cdiv(max(ne_tiles, 2 * G + 1), 128), 128, 0, st>>>(G, n, m, tn, tm_, 128, w.tiles, w.cnt, w.gstart);
+  MM_LAUNCH_CHECK();
+  {
     GemmP p = gemm_defaults();
     p.Wt = W[MMMOT_W_NE_W1T]; p.bias = W[MMMOT_W_NE_B1]; p.ldw = 512; p.M = 512; p.K = 512;
     p.tile_tab = w.tiles; p.num_tiles = ne_tiles;
@@ -445,61 +472,58 @@ int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mo
     MM_TRY(gemm_simt_launch<XM_NORM_RELU>(p, st));
     MM_TRY(stats_reduce(w.npart, 128, 2 * G, 0, w.gstart, w.nstats, st));
     MM_TRY(gn_finalize(w.nstats, W[MMMOT_W_NE_G2W], W[MMMOT_W_NE_G2B], w.cnt, 0, 2 * G, 128, 128, w.nsc2, w.nsh2, st));
-    ne_final_kernel<<<mm_cdiv((long)G * (n + m), 128), 128, 0, st>>>(w.h2, ldv, w.nsc2, w.nsh2, W[MMMOT_W_NE_W3],
-                                                                   W[MMMOT_W_NE_B3], G, n, m, new_s, end_s);
-    MM_LAUNCH_CHECK();
   }
+  ne_final_kernel<<<mm_cdiv((long)G * (n + m), 128), 128, 0, st>>>(w.h2, ldv, w.nsc2, w.nsh2, W[MMMOT_W_NE_W3],
+                                                                 W[MMMOT_W_NE_B3], G, n, m, new_s, end_s);
+  MM_LAUNCH_CHECK();
 
   // ---- affinity MLP layers 2, 3 on y1 = channels 0..511 of y01 ----
-  if (use_tc) {
-    // GroupNorm + ReLU of the previous layer is applied by this layer's operand producers (gemm_gen.cuh, GEN_NORM)
-    GemmP p = gemm_defaults();
-    p.bias = W[MMMOT_W_AF_B2]; p.M = 512; p.K = 512;
-    p.S = NM; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
-    p.x_gs = NM;
-    p.Y = w.y2; p.y_gs = NM; p.y_ms = 512;
-    p.part = w.part;
-    if (timed) mm_timing_begin(st, MM_T_AFF_L2, 2.0 * 512 * 512 * (double)G * NM, 4.0 * (512 + 512) * (double)G * NM);
-    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W2P, w.y01, 1024, (long)G * NM, w.sc1, w.sh1, 0, 0, 0, st));
-    if (timed) mm_timing_end(st);
-    MM_TRY(stats_reduce(w.part, 512, G, tpg, nullptr, w.stats, st, 2));
-    MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G2W], W[MMMOT_W_AF_G2B], nullptr, NM, G, 512, 1, w.sc2, w.sh2, st, 0, 0, ar.status()));
-    p.bias = W[MMMOT_W_AF_B3]; p.M = 128;
-    p.Y = w.y3; p.y_ms = 128;
-    if (timed) mm_timing_begin(st, MM_T_AFF_L3, 2.0 * 128 * 512 * (double)G * NM, 4.0 * (512 + 128) * (double)G * NM);
-    MM_TRY(launch_gen<gen::GEN_NORM>(p, wts, MMMOT_W_AF_W3P, w.y2, 512, (long)G * NM, w.sc2, w.sh2, 0, 0, 0, st));
-    if (timed) mm_timing_end(st);
-    MM_TRY(stats_reduce(w.part, 128, G, tpg, nullptr, w.stats, st, 2));
-    MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G3W], W[MMMOT_W_AF_G3B], nullptr, NM, G, 128, 1, w.sc3, w.sh3, st));
-  } else {
-    GemmP p = gemm_defaults();
-    p.Wt = W[MMMOT_W_AF_W2T]; p.bias = W[MMMOT_W_AF_B2]; p.ldw = 512; p.M = 512; p.K = 512;
-    p.S = NM; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
-    p.X = w.y01; p.x_gs = 1024L * NM; p.x_ks = NM; p.sc = w.sc1; p.sh = w.sh1;
-    p.Y = w.y2; p.y_gs = 512L * NM; p.y_ms = NM;
-    p.part = w.part;
-    MM_TRY(gemm_simt_launch<XM_NORM_RELU>(p, st));
-    MM_TRY(stats_reduce(w.part, 512, G, tpg, nullptr, w.stats, st));
-    MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G2W], W[MMMOT_W_AF_G2B], nullptr, NM, G, 512, 1, w.sc2, w.sh2, st));
-    p.Wt = W[MMMOT_W_AF_W3T]; p.bias = W[MMMOT_W_AF_B3]; p.ldw = 128; p.M = 128;
-    p.X = w.y2; p.x_gs = 512L * NM; p.sc = w.sc2; p.sh = w.sh2;
-    p.Y = w.y3; p.y_gs = 128L * NM;
-    MM_TRY(gemm_simt_launch<XM_NORM_RELU>(p, st));
-    MM_TRY(stats_reduce(w.part, 128, G, tpg, nullptr, w.stats, st));
-    MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G3W], W[MMMOT_W_AF_G3B], nullptr, NM, G, 128, 1, w.sc3, w.sh3, st));
-  }
-  float* zdst = softmax_mode == MMMOT_SM_NONE ? link : w.z;
-  if (use_tc) {
-    if (timed) mm_timing_begin(st, MM_T_AFF_LOGIT, 2.0 * 128 * (double)G * NM, 4.0 * 129 * (double)G * NM);
-    const long lrows = (long)G * NM;
-    link_logit_cl_kernel<<<(int)std::min<long>(148L * 8, (lrows + 31) / 32), 256, 0, st>>>(w.y3, w.sc3, w.sh3, W[MMMOT_W_AF_W4],
-                                                                                      W[MMMOT_W_AF_B4], lrows, NM, zdst);
-  } else {
-    link_logit_kernel<<<mm_cdiv((long)G * NM, 256), 256, 0, st>>>(w.y3, w.sc3, w.sh3, W[MMMOT_W_AF_W4],
-                                                                 W[MMMOT_W_AF_B4], G, NM, zdst);
-  }
+  GemmP p = gemm_defaults();
+  p.Wt = W[MMMOT_W_AF_W2T]; p.bias = W[MMMOT_W_AF_B2]; p.ldw = 512; p.M = 512; p.K = 512;
+  p.S = NM; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
+  p.X = w.y01; p.x_gs = 1024L * NM; p.x_ks = NM; p.sc = w.sc1; p.sh = w.sh1;
+  p.Y = w.y2; p.y_gs = 512L * NM; p.y_ms = NM;
+  p.part = w.part;
+  MM_TRY(gemm_simt_launch<XM_NORM_RELU>(p, st));
+  MM_TRY(stats_reduce(w.part, 512, G, tpg, nullptr, w.stats, st));
+  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G2W], W[MMMOT_W_AF_G2B], nullptr, NM, G, 512, 1, w.sc2, w.sh2, st));
+  p.Wt = W[MMMOT_W_AF_W3T]; p.bias = W[MMMOT_W_AF_B3]; p.ldw = 128; p.M = 128;
+  p.X = w.y2; p.x_gs = 512L * NM; p.sc = w.sc2; p.sh = w.sh2;
+  p.Y = w.y3; p.y_gs = 128L * NM;
+  MM_TRY(gemm_simt_launch<XM_NORM_RELU>(p, st));
+  MM_TRY(stats_reduce(w.part, 128, G, tpg, nullptr, w.stats, st));
+  MM_TRY(gn_finalize(w.stats, W[MMMOT_W_AF_G3W], W[MMMOT_W_AF_G3B], nullptr, NM, G, 128, 1, w.sc3, w.sh3, st));
+  link_logit_kernel<<<mm_cdiv((long)G * NM, 256), 256, 0, st>>>(w.y3, w.sc3, w.sh3, W[MMMOT_W_AF_W4],
+                                                               W[MMMOT_W_AF_B4], G, NM, zdst);
   MM_LAUNCH_CHECK();
-  if (use_tc && timed) mm_timing_end(st);
+  return 0;
+}
+
+// The stage on every stack (stack < 0: G = 3*pairs groups, group g reads feature block g) or on one (G = pairs, group g
+// reads block g*3 + stack).  Every plan choice depends on the per-pair shape only, so a group's results do not depend on
+// which of the two it runs in.
+int affinity_impl(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs, int stack, int n,
+                  int m, const float* feats, float* link, float* new_s, float* end_s, void* workspace,
+                  size_t workspace_bytes, void* stream) {
+  if (!wts || !feats || !link || !new_s || !end_s || !workspace || pairs <= 0 || n <= 0 || m <= 0 || stack > 2)
+    return MMMOT_E_ARG;
+  if (affinity_op < 0 || affinity_op > MMMOT_AFF_MINUS || softmax_mode < 0 || softmax_mode > MMMOT_SM_DUAL_MAX ||
+      end_mode < MMMOT_END_AVG || end_mode > MMMOT_END_MAX)
+    return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  MmArena ar(workspace, workspace_bytes);
+  const int G = stack < 0 ? pairs * 3 : pairs, NM = n * m, L = n + m;
+  const AfWs w = carve(ar, (size_t)G, n, m);
+  if (!ar.ok()) return MMMOT_E_WORKSPACE;
+  // group g's feature block [512][L]: fbase + g*fgs
+  const float* fbase = stack < 0 ? feats : feats + (long)stack * 512 * L;
+  const long fgs = (stack < 0 ? 1L : 3L) * 512 * L;
+  // the link logits go straight to link when no softmax follows
+  float* zdst = softmax_mode == MMMOT_SM_NONE ? link : w.z;
+  if (affinity_use_tc(n, m))
+    MM_TRY(affinity_tc(wts, affinity_op, end_mode, stack, G, n, m, fbase, fgs, w, ar.status(), zdst, new_s, end_s, st));
+  else
+    MM_TRY(affinity_fp32(wts, affinity_op, end_mode, G, n, m, fbase, fgs, w, ar.status(), zdst, new_s, end_s, st));
   if (softmax_mode != MMMOT_SM_NONE) {
     softmax_stats_kernel<<<mm_cdiv((long)G * (n + m) * 32, 256), 256, 0, st>>>(w.z, G, n, m, w.rmax, w.rsum,
                                                                               w.cmax, w.csum);
@@ -513,18 +537,17 @@ int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mo
 
 }  // namespace
 
-extern "C" int
-mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs,
-                                  int n, int m, const float* feats, float* link, float* new_s,
-                                  float* end_s, void* workspace, size_t workspace_bytes, void* stream) {
-  return mmmot_affinity_fwd(wts, affinity_op, softmax_mode, end_mode, pairs, -1, n, m, feats, link, new_s, end_s, workspace,
-                      workspace_bytes, stream);
+extern "C" int mmmot_affinity_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs, int n,
+                                  int m, const float* feats, float* link, float* new_s, float* end_s, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  return affinity_impl(wts, affinity_op, softmax_mode, end_mode, pairs, -1, n, m, feats, link, new_s, end_s, workspace,
+                       workspace_bytes, stream);
 }
 
 extern "C" int mmmot_affinity_stack_fwd(const mmmot_weights* wts, int affinity_op, int softmax_mode, int end_mode, int pairs,
                                         int stack, int n, int m, const float* feats, float* link, float* new_s, float* end_s,
                                         void* workspace, size_t workspace_bytes, void* stream) {
   if (stack < 0 || stack > 2) return MMMOT_E_ARG;
-  return mmmot_affinity_fwd(wts, affinity_op, softmax_mode, end_mode, pairs, stack, n, m, feats, link, new_s, end_s, workspace,
-                      workspace_bytes, stream);
+  return affinity_impl(wts, affinity_op, softmax_mode, end_mode, pairs, stack, n, m, feats, link, new_s, end_s, workspace,
+                       workspace_bytes, stream);
 }

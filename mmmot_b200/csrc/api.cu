@@ -175,6 +175,7 @@ int mm_debug_flags() { return g_dbg; }
 extern "C" int mmmot_set_debug(int flags) { g_dbg = flags; return 0; }
 
 int mm_engine() { return g_engine; }
+bool mm_use_tc(bool auto_tc) { return mm_engine() == 2 || (mm_engine() == 0 && auto_tc); }
 
 extern "C" int mmmot_set_engine(int engine) {
   if (engine < 0 || engine > 2) return MMMOT_E_ARG;

@@ -522,7 +522,7 @@ extern "C" int mmmot_appearance_fwd(const mmmot_weights* wts, const float* crops
   // writes exactly what the next conv's TMA loads read (3x3 taps = shifted boxes, padding = TMA zero fill).
   // engine choice depends on per-pair shapes only (never on the batch size), so batched, looped and sharded runs
   // take the same path and stay bit-identical
-  const bool tc_trunk = mm_engine() == 2 || (mm_engine() == 0 && (long)L * H * W >= 32768);
+  const bool tc_trunk = mm_use_tc((long)L * H * W >= 32768);
   if (tc_trunk) {
     __half* hb[2] = {reinterpret_cast<__half*>(ws.buf[0]), reinterpret_cast<__half*>(ws.buf[1])};
     const bool timed = mm_timing_on();   // roofline hook: every launch tagged (stage, layer)

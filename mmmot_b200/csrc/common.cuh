@@ -50,6 +50,8 @@ enum {
 };
 int mm_kseg_chunks();  // K-segment length (in 32-wide chunks) of the tensor-core conv engine, 0 = off (mmmot_set_kseg)
 int mm_engine();  // 0 auto, 1 FP32 FFMA engine, 2 tensor-core (wgmma) engine (mmmot_set_engine)
+// whether a stage runs on the tensor cores: a forced engine wins, else (auto) the stage's own shape rule auto_tc
+bool mm_use_tc(bool auto_tc);
 // Per-launch timing hook (mmmot_timing_*): every hot kernel of the path is bracketed by CUDA events on the launching
 // stream while timing is enabled, tagged with (stage, layer) and its ALGORITHMIC work (FLOPs, compulsory HBM bytes).
 enum {

@@ -145,7 +145,7 @@ FdWs carve(MmArena& a, int pairs, int L, int ns) {
 }
 
 // engine choice from the per-pair shape only (see appearance.cu)
-bool fusion_det_use_tc(int L) { return mm_engine() == 2 || (mm_engine() == 0 && L >= 64); }
+bool fusion_det_use_tc(int L) { return mm_use_tc(L >= 64); }
 
 }  // namespace
 
@@ -174,77 +174,69 @@ int mm_fusion_det_layout(int pairs, int L, size_t* off, int* tensor_cores) {
 
 namespace {
 
-// stack < 0: fusion, then w_det on all three stacks.  stack 2: fusion, then w_det on stack 2.  stack 0 or 1: w_det on that
-// stack alone (no fusion; nothing else of feats is read or written).  A stack's scores are the same in either case.
-int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold, int pairs, int L,
-                         int stack, float* feats, float* det_scores, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!wts || !feats || !det_scores || !workspace || pairs <= 0 || L <= 0 || stack > 2) return MMMOT_E_ARG;
-  if (fusion_arch < MMMOT_FUSION_A || fusion_arch > MMMOT_FUSION_C) return MMMOT_E_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  MmArena ar(workspace, workspace_bytes);
-  const int ns = stack < 0 ? 3 : 1;   // stacks scored
-  FdWs w = carve(ar, pairs, L, ns);
-  if (!ar.ok()) return MMMOT_E_WORKSPACE;
-  const bool fuse = stack < 0 || stack == 2;
-  const long fs = 3L * 512 * L;  // floats per pair in feats
-
-  if (fusion_det_use_tc(L)) {
-    // ---------------- tensor-core path: every contraction on the generated-operand engine (GEN_COPY) over
-    // detection-major channels-last rows F3[(pair*L + l)*3 + stack][512]
-    const int tpg2 = mm_cdiv(L, tc::BN);
-    const dim3 tb(32, 8);
-    // the stacks read: image and LiDAR for the fusion, else the one scored
-    feats_to_rows_kernel<<<dim3(mm_cdiv(L, 32), 16, pairs * (fuse ? 2 : 1)), tb, 0, st>>>(feats, w.f3, L, fuse ? 0 : stack,
-                                                                                      fuse ? 2 : 1);
-    MM_LAUNCH_CHECK();
-    auto lin_tc = [&](int wp_id, int wb, int K, int sidx, float* Y, bool stats, int gw, int gb, float* sc, float* sh) -> int {
-      GemmP p = gemm_defaults();
-      p.bias = wts->w[wb]; p.M = 512; p.K = K;
-      p.S = L; p.tiles_per_group = tpg2; p.num_tiles = tpg2 * pairs;
-      p.x_gs = L;                                            // rows per group (= per pair) of the source view below
-      p.Y = Y; p.y_gs = L; p.y_ms = 512;
-      p.part = stats ? w.part : nullptr;
-      MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[wp_id], wts->tc_scale[wp_id], w.f3 + (long)sidx * 512, 1536, 0,
-                                             nullptr, nullptr, 0, 0, 0, st)));
-      if (stats) MM_TRY(stats_reduce(w.part, 512, pairs, tpg2, nullptr, w.stats, st, 2));
-      if (stats) MM_TRY(gn_finalize(w.stats, wts->w[gw], wts->w[gb], nullptr, L, pairs, 512, 1, sc, sh, st));
-      return 0;
-    };
-    if (fuse) {
-      if (fusion_arch == MMMOT_FUSION_A) {
-        MM_TRY(lin_tc(MMMOT_W_FU_WPP, MMMOT_W_FU_BP, 1024, 0, w.yp, true, MMMOT_W_FU_GPW, MMMOT_W_FU_GPB, w.scp, w.shp));
-      } else {
-        MM_TRY(lin_tc(MMMOT_W_FU_WPP, MMMOT_W_FU_BP, 512, 0, w.yp, true, MMMOT_W_FU_GPW, MMMOT_W_FU_GPB, w.scp, w.shp));
-        MM_TRY(lin_tc(MMMOT_W_FU_WIP, MMMOT_W_FU_BI, 512, 1, w.yi, true, MMMOT_W_FU_GIW, MMMOT_W_FU_GIB, w.sci, w.shi));
-        if (fusion_arch == MMMOT_FUSION_C) {
-          MM_TRY(lin_tc(MMMOT_W_FU_GATE_PP, MMMOT_W_FU_GATE_PB, 512, 0, w.gp, false, 0, 0, nullptr, nullptr));
-          MM_TRY(lin_tc(MMMOT_W_FU_GATE_IP, MMMOT_W_FU_GATE_IB, 512, 1, w.gi, false, 0, 0, nullptr, nullptr));
-        }
-      }
-      fusion_combine_rows_kernel<<<dim3(mm_cdiv(L, 32), 16, pairs), tb, 0, st>>>(fusion_arch, w.yp, w.yi, w.gp, w.gi, w.scp, w.shp,
-                                                                                w.sci, w.shi, L, feats, w.f3);
-      MM_LAUNCH_CHECK();
-    }
-    // w_det on all three stacks = one matrix of pairs*L*3 rows x 512 channels, or on one stack = the pairs*L rows of that
-    // stack in F3 (row stride 1536); BN(eval) folded, ReLU in the epilogue
-    const long rows = (long)pairs * L * ns;
+// Tensor-core path: every contraction on the generated-operand engine (GEN_COPY) over detection-major channels-last rows
+// F3[(pair*L + l)*3 + stack][512]
+int fusion_det_tc(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold, int pairs, int L, int stack,
+                  int ns, bool fuse, float* feats, float* det_scores, const FdWs& w, cudaStream_t st) {
+  const int tpg2 = mm_cdiv(L, tc::BN);
+  const dim3 tb(32, 8);
+  // the stacks read: image and LiDAR for the fusion, else the one scored
+  feats_to_rows_kernel<<<dim3(mm_cdiv(L, 32), 16, pairs * (fuse ? 2 : 1)), tb, 0, st>>>(feats, w.f3, L, fuse ? 0 : stack,
+                                                                                    fuse ? 2 : 1);
+  MM_LAUNCH_CHECK();
+  auto lin_tc = [&](int wp_id, int wb, int K, int sidx, float* Y, bool stats, int gw, int gb, float* sc, float* sh) -> int {
     GemmP p = gemm_defaults();
-    p.bias = wts->w[MMMOT_W_WD_B1]; p.M = 512; p.K = 512; p.relu = 1;
-    p.S = (int)rows; p.tiles_per_group = mm_cdiv(rows, tc::BN); p.num_tiles = p.tiles_per_group;
-    p.x_gs = rows;
-    p.Y = w.h1; p.y_gs = rows; p.y_ms = 512;
-    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W1P], wts->tc_scale[MMMOT_W_WD_W1P],
-                                           stack < 0 ? w.f3 : w.f3 + (long)stack * 512, stack < 0 ? 512 : 1536, 0, nullptr,
-                                           nullptr, 0, 0, 0, st)));
-    p.bias = wts->w[MMMOT_W_WD_B2]; p.M = 256;
-    p.Y = w.h2; p.y_ms = 256;
-    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W2P], wts->tc_scale[MMMOT_W_WD_W2P], w.h1, 512, 0, nullptr,
-                                           nullptr, 0, 0, 0, st)));
-    det_score_rows_kernel<<<mm_cdiv(rows * 32, 256), 256, 0, st>>>(w.h2, wts->w[MMMOT_W_WD_W3], wts->w[MMMOT_W_WD_B3], score_flags,
-                                                                  neg_threshold, rows, L, ns, det_scores);
-    MM_LAUNCH_CHECK();
+    p.bias = wts->w[wb]; p.M = 512; p.K = K;
+    p.S = L; p.tiles_per_group = tpg2; p.num_tiles = tpg2 * pairs;
+    p.x_gs = L;                                            // rows per group (= per pair) of the source view below
+    p.Y = Y; p.y_gs = L; p.y_ms = 512;
+    p.part = stats ? w.part : nullptr;
+    MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[wp_id], wts->tc_scale[wp_id], w.f3 + (long)sidx * 512, 1536, 0,
+                                           nullptr, nullptr, 0, 0, 0, st)));
+    if (stats) MM_TRY(stats_reduce(w.part, 512, pairs, tpg2, nullptr, w.stats, st, 2));
+    if (stats) MM_TRY(gn_finalize(w.stats, wts->w[gw], wts->w[gb], nullptr, L, pairs, 512, 1, sc, sh, st));
     return 0;
+  };
+  if (fuse) {
+    if (fusion_arch == MMMOT_FUSION_A) {
+      MM_TRY(lin_tc(MMMOT_W_FU_WPP, MMMOT_W_FU_BP, 1024, 0, w.yp, true, MMMOT_W_FU_GPW, MMMOT_W_FU_GPB, w.scp, w.shp));
+    } else {
+      MM_TRY(lin_tc(MMMOT_W_FU_WPP, MMMOT_W_FU_BP, 512, 0, w.yp, true, MMMOT_W_FU_GPW, MMMOT_W_FU_GPB, w.scp, w.shp));
+      MM_TRY(lin_tc(MMMOT_W_FU_WIP, MMMOT_W_FU_BI, 512, 1, w.yi, true, MMMOT_W_FU_GIW, MMMOT_W_FU_GIB, w.sci, w.shi));
+      if (fusion_arch == MMMOT_FUSION_C) {
+        MM_TRY(lin_tc(MMMOT_W_FU_GATE_PP, MMMOT_W_FU_GATE_PB, 512, 0, w.gp, false, 0, 0, nullptr, nullptr));
+        MM_TRY(lin_tc(MMMOT_W_FU_GATE_IP, MMMOT_W_FU_GATE_IB, 512, 1, w.gi, false, 0, 0, nullptr, nullptr));
+      }
+    }
+    fusion_combine_rows_kernel<<<dim3(mm_cdiv(L, 32), 16, pairs), tb, 0, st>>>(fusion_arch, w.yp, w.yi, w.gp, w.gi, w.scp, w.shp,
+                                                                              w.sci, w.shi, L, feats, w.f3);
+    MM_LAUNCH_CHECK();
   }
+  // w_det on all three stacks = one matrix of pairs*L*3 rows x 512 channels, or on one stack = the pairs*L rows of that
+  // stack in F3 (row stride 1536); BN(eval) folded, ReLU in the epilogue
+  const long rows = (long)pairs * L * ns;
+  GemmP p = gemm_defaults();
+  p.bias = wts->w[MMMOT_W_WD_B1]; p.M = 512; p.K = 512; p.relu = 1;
+  p.S = (int)rows; p.tiles_per_group = mm_cdiv(rows, tc::BN); p.num_tiles = p.tiles_per_group;
+  p.x_gs = rows;
+  p.Y = w.h1; p.y_gs = rows; p.y_ms = 512;
+  MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W1P], wts->tc_scale[MMMOT_W_WD_W1P],
+                                         stack < 0 ? w.f3 : w.f3 + (long)stack * 512, stack < 0 ? 512 : 1536, 0, nullptr,
+                                         nullptr, 0, 0, 0, st)));
+  p.bias = wts->w[MMMOT_W_WD_B2]; p.M = 256;
+  p.Y = w.h2; p.y_ms = 256;
+  MM_TRY((gemm_gen_launch<gen::GEN_COPY>(p, (const uint4*)wts->w[MMMOT_W_WD_W2P], wts->tc_scale[MMMOT_W_WD_W2P], w.h1, 512, 0, nullptr,
+                                         nullptr, 0, 0, 0, st)));
+  det_score_rows_kernel<<<mm_cdiv(rows * 32, 256), 256, 0, st>>>(w.h2, wts->w[MMMOT_W_WD_W3], wts->w[MMMOT_W_WD_B3], score_flags,
+                                                                neg_threshold, rows, L, ns, det_scores);
+  MM_LAUNCH_CHECK();
+  return 0;
+}
+
+// FP32 path: channel-major activations [group][C][L], the layout of feats itself
+int fusion_det_fp32(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold, int pairs, int L,
+                    int stack, int ns, bool fuse, float* feats, float* det_scores, const FdWs& w, cudaStream_t st) {
+  const long fs = 3L * 512 * L;  // floats per pair in feats
   const int tpg = mm_cdiv(L, 128);
 
   // linear (+ optional GroupNorm statistics) on one modality: X = feats[pair][stack]
@@ -283,19 +275,17 @@ int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, int score_fl
   // w_det on all three stacks (groups g = pair*3 + stack) or on one (g = pair, feature block g*3 + stack), BN(eval)
   // folded, ReLU in the epilogue
   const int G = pairs * ns;
-  {
-    GemmP p = gemm_defaults();
-    p.Wt = wts->w[MMMOT_W_WD_W1T]; p.bias = wts->w[MMMOT_W_WD_B1]; p.ldw = 512; p.M = 512; p.K = 512;
-    p.S = L; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
-    p.X = stack < 0 ? feats : feats + (long)stack * 512 * L; p.x_gs = stack < 0 ? 512L * L : fs; p.x_ks = L;
-    p.Y = w.h1; p.y_gs = 512L * L; p.y_ms = L;
-    p.relu = 1;
-    MM_TRY(gemm_simt_launch<XM_DIRECT>(p, st));
-    p.Wt = wts->w[MMMOT_W_WD_W2T]; p.bias = wts->w[MMMOT_W_WD_B2]; p.ldw = 256; p.M = 256;
-    p.X = w.h1; p.x_gs = 512L * L;
-    p.Y = w.h2; p.y_gs = 256L * L;
-    MM_TRY(gemm_simt_launch<XM_DIRECT>(p, st));
-  }
+  GemmP p = gemm_defaults();
+  p.Wt = wts->w[MMMOT_W_WD_W1T]; p.bias = wts->w[MMMOT_W_WD_B1]; p.ldw = 512; p.M = 512; p.K = 512;
+  p.S = L; p.tiles_per_group = tpg; p.num_tiles = tpg * G;
+  p.X = stack < 0 ? feats : feats + (long)stack * 512 * L; p.x_gs = stack < 0 ? 512L * L : fs; p.x_ks = L;
+  p.Y = w.h1; p.y_gs = 512L * L; p.y_ms = L;
+  p.relu = 1;
+  MM_TRY(gemm_simt_launch<XM_DIRECT>(p, st));
+  p.Wt = wts->w[MMMOT_W_WD_W2T]; p.bias = wts->w[MMMOT_W_WD_B2]; p.ldw = 256; p.M = 256;
+  p.X = w.h1; p.x_gs = 512L * L;
+  p.Y = w.h2; p.y_gs = 256L * L;
+  MM_TRY(gemm_simt_launch<XM_DIRECT>(p, st));
   det_score_kernel<<<mm_cdiv((long)G * L, 128), 128, 0, st>>>(w.h2, wts->w[MMMOT_W_WD_W3],
                                                               wts->w[MMMOT_W_WD_B3], score_flags, neg_threshold, G, L,
                                                               det_scores);
@@ -303,20 +293,36 @@ int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, int score_fl
   return 0;
 }
 
+// stack < 0: fusion, then w_det on all three stacks.  stack 2: fusion, then w_det on stack 2.  stack 0 or 1: w_det on that
+// stack alone (no fusion; nothing else of feats is read or written).  A stack's scores are the same in either case.
+int fusion_det_impl(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold, int pairs, int L,
+                    int stack, float* feats, float* det_scores, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!wts || !feats || !det_scores || !workspace || pairs <= 0 || L <= 0 || stack > 2) return MMMOT_E_ARG;
+  if (fusion_arch < MMMOT_FUSION_A || fusion_arch > MMMOT_FUSION_C) return MMMOT_E_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  MmArena ar(workspace, workspace_bytes);
+  const int ns = stack < 0 ? 3 : 1;   // stacks scored
+  const FdWs w = carve(ar, pairs, L, ns);
+  if (!ar.ok()) return MMMOT_E_WORKSPACE;
+  const bool fuse = stack < 0 || stack == 2;
+  if (fusion_det_use_tc(L))
+    return fusion_det_tc(wts, fusion_arch, score_flags, neg_threshold, pairs, L, stack, ns, fuse, feats, det_scores, w, st);
+  return fusion_det_fp32(wts, fusion_arch, score_flags, neg_threshold, pairs, L, stack, ns, fuse, feats, det_scores, w, st);
+}
+
 }  // namespace
 
-extern "C" int
-mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold,
-                                    int pairs, int L, float* feats, float* det_scores, void* workspace,
-                                    size_t workspace_bytes, void* stream) {
-  return mmmot_fusion_det_fwd(wts, fusion_arch, score_flags, neg_threshold, pairs, L, -1, feats, det_scores, workspace,
-                        workspace_bytes, stream);
+extern "C" int mmmot_fusion_det_fwd(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold, int pairs,
+                                    int L, float* feats, float* det_scores, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+  return fusion_det_impl(wts, fusion_arch, score_flags, neg_threshold, pairs, L, -1, feats, det_scores, workspace,
+                         workspace_bytes, stream);
 }
 
 extern "C" int mmmot_fusion_det_stack_fwd(const mmmot_weights* wts, int fusion_arch, int score_flags, float neg_threshold,
                                           int pairs, int L, int stack, float* feats, float* det_scores, void* workspace,
                                           size_t workspace_bytes, void* stream) {
   if (stack < 0 || stack > 2) return MMMOT_E_ARG;
-  return mmmot_fusion_det_fwd(wts, fusion_arch, score_flags, neg_threshold, pairs, L, stack, feats, det_scores, workspace,
-                        workspace_bytes, stream);
+  return fusion_det_impl(wts, fusion_arch, score_flags, neg_threshold, pairs, L, stack, feats, det_scores, workspace,
+                         workspace_bytes, stream);
 }

@@ -821,7 +821,7 @@ int pointnet_fp32(const mmmot_weights* wts, const float* points, const int* det_
 }  // namespace
 
 // engine choice from the per-pair shape only (see appearance.cu)
-static bool pointnet_use_tc(int L) { return mm_engine() == 2 || (mm_engine() == 0 && L >= 16); }
+static bool pointnet_use_tc(int L) { return mm_use_tc(L >= 16); }
 
 extern "C" size_t mmmot_pointnet_workspace(int pairs, int L, long p_total) {
   MmArena a(nullptr, 0);

@@ -598,7 +598,7 @@ Trunk make_trunk(const mmmot_resnet_weights* rw, int n_img, int H, int W, int L,
                  cudaStream_t st) {
   Trunk t;
   t.rw = rw; t.n_img = n_img;
-  t.tc = mm_engine() == 2 || (mm_engine() == 0 && (long)L * H * W >= 32768);
+  t.tc = mm_use_tc((long)L * H * W >= 32768);
   t.timed = mm_timing_on();
   t.cols = ws.cols; t.kseg = ws.kseg; t.status = status; t.st = st;
   return t;

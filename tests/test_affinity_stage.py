@@ -354,40 +354,44 @@ def test_case_coverage():
     assert {c[1] for c in CASES if c[1] == c[2] and path[c[0]] == "tc" and c[4] == "auto"} >= {32, 64, 128, 256}
 
 
-# Every kernel launch and helper call of mmmot_affinity_fwd, in source order (both paths), with the checks that hold
-# its output: this file's CHECKS or tests/test_heads.py's HEAD_CHECKS.  feats_range_kernel's only output is the status
-# word, which every case requires clear.
+# The functions the stage runs and, per function, every kernel launch and helper call in its body, in source order, with
+# the checks that hold its output: this file's CHECKS or tests/test_heads.py's HEAD_CHECKS.  feats_range_kernel's only
+# output is the status word, which every case requires clear.
 AF_HELPERS = ("launch_gen", "gemm_simt_launch", "transpose_f32", "stats_reduce", "gn_finalize")
-LAUNCH_SITES = [
-    ("transpose_f32", ("fcl",)), ("feats_range_kernel", ("y01",)),
-    ("launch_gen", ("y01",)), ("launch_gen", ("y01",)), ("launch_gen", ("y01",)),                    # TC layer 1, per op
-    ("gemm_simt_launch", ("y01",)), ("gemm_simt_launch", ("y01",)), ("gemm_simt_launch", ("y01",)),  # FP32 layer 1
-    ("stats_reduce", ("sc1_sh1", "sc0_sh0")), ("gn_finalize", ("sc1_sh1",)), ("gn_finalize", ("sc0_sh0",)),
-    ("newend_mean_cl_kernel", ("new_end_mean",)), ("rowcol_mean_kernel", ("new_end_mean",)),
-    ("ne_tiles_kernel", ("tables",)),
-    # new / end MLP, tensor cores
-    ("launch_gen", ("h1",)), ("stats_reduce", ("nsc1_nsh1",)), ("gn_finalize", ("nsc1_nsh1",)),
-    ("launch_gen", ("h2",)), ("stats_reduce", ("nstats",)), ("gn_finalize", ("nsc2_nsh2",)),
-    ("ne_final_cl_kernel", ("new_end_sigmoid",)),
-    # new / end MLP, FP32
-    ("gemm_simt_launch", ("h1",)), ("stats_reduce", ("nsc1_nsh1",)), ("gn_finalize", ("nsc1_nsh1",)),
-    ("gemm_simt_launch", ("h2",)), ("stats_reduce", ("nstats",)), ("gn_finalize", ("nsc2_nsh2",)),
-    ("ne_final_kernel", ("new_end_sigmoid",)),
-    # affinity layers 2, 3, tensor cores then FP32
-    ("launch_gen", ("y2",)), ("stats_reduce", ("sc2_sh2",)), ("gn_finalize", ("sc2_sh2",)),
-    ("launch_gen", ("y3",)), ("stats_reduce", ("stats",)), ("gn_finalize", ("sc3_sh3",)),
-    ("gemm_simt_launch", ("y2",)), ("stats_reduce", ("sc2_sh2",)), ("gn_finalize", ("sc2_sh2",)),
-    ("gemm_simt_launch", ("y3",)), ("stats_reduce", ("stats",)), ("gn_finalize", ("sc3_sh3",)),
-    ("link_logit_cl_kernel", ("link_logit",)), ("link_logit_kernel", ("link_logit",)),
-    ("softmax_stats_kernel", ("softmax_sums",)), ("softmax_apply_kernel", ("softmax_link",)),
-]
+LAUNCH_SITES = {
+    "affinity_impl": [("softmax_stats_kernel", ("softmax_sums",)), ("softmax_apply_kernel", ("softmax_link",))],
+    "affinity_tc": [
+        ("transpose_f32", ("fcl",)), ("feats_range_kernel", ("y01",)),
+        ("launch_gen", ("y01",)), ("launch_gen", ("y01",)), ("launch_gen", ("y01",)),          # layer 1, per op
+        ("stats_reduce", ("sc1_sh1", "sc0_sh0")), ("gn_finalize", ("sc1_sh1",)), ("gn_finalize", ("sc0_sh0",)),
+        ("newend_mean_cl_kernel", ("new_end_mean",)), ("ne_tiles_kernel", ("tables",)),
+        ("launch_gen", ("h1",)), ("stats_reduce", ("nsc1_nsh1",)), ("gn_finalize", ("nsc1_nsh1",)),
+        ("launch_gen", ("h2",)), ("stats_reduce", ("nstats",)), ("gn_finalize", ("nsc2_nsh2",)),
+        ("ne_final_cl_kernel", ("new_end_sigmoid",)),
+        ("launch_gen", ("y2",)), ("stats_reduce", ("sc2_sh2",)), ("gn_finalize", ("sc2_sh2",)),
+        ("launch_gen", ("y3",)), ("stats_reduce", ("stats",)), ("gn_finalize", ("sc3_sh3",)),
+        ("link_logit_cl_kernel", ("link_logit",)),
+    ],
+    "affinity_fp32": [
+        ("gemm_simt_launch", ("y01",)), ("gemm_simt_launch", ("y01",)), ("gemm_simt_launch", ("y01",)),  # layer 1, per op
+        ("stats_reduce", ("sc1_sh1", "sc0_sh0")), ("gn_finalize", ("sc1_sh1",)), ("gn_finalize", ("sc0_sh0",)),
+        ("rowcol_mean_kernel", ("new_end_mean",)), ("ne_tiles_kernel", ("tables",)),
+        ("gemm_simt_launch", ("h1",)), ("stats_reduce", ("nsc1_nsh1",)), ("gn_finalize", ("nsc1_nsh1",)),
+        ("gemm_simt_launch", ("h2",)), ("stats_reduce", ("nstats",)), ("gn_finalize", ("nsc2_nsh2",)),
+        ("ne_final_kernel", ("new_end_sigmoid",)),
+        ("gemm_simt_launch", ("y2",)), ("stats_reduce", ("sc2_sh2",)), ("gn_finalize", ("sc2_sh2",)),
+        ("gemm_simt_launch", ("y3",)), ("stats_reduce", ("stats",)), ("gn_finalize", ("sc3_sh3",)),
+        ("link_logit_kernel", ("link_logit",)),
+    ],
+}
 
 
-def test_stage_launch_coverage_guard():
-    """Every launch of mmmot_affinity_fwd maps to a check: a launch added, removed or reordered without its entry in
-    LAUNCH_SITES fails here; every check named there is one the GPU tests fill, and every check is named."""
-    assert impl_launches("affinity.cu", "mmmot_affinity_fwd", AF_HELPERS) == [s[0] for s in LAUNCH_SITES]
-    named = {c for _, cs in LAUNCH_SITES for c in cs}
+def test_stage_functions_launch_coverage_guard():
+    """Every launch in the functions the stage runs maps to a check: a launch added, removed or reordered without its
+    entry in LAUNCH_SITES fails here; every check named there is one the GPU tests fill, and every check is named."""
+    for func, sites in LAUNCH_SITES.items():
+        assert impl_launches("affinity.cu", func, AF_HELPERS) == [s[0] for s in sites], func
+    named = {c for sites in LAUNCH_SITES.values() for _, cs in sites for c in cs}
     assert named == set(CHECKS) | set(HEAD_CHECKS), named ^ (set(CHECKS) | set(HEAD_CHECKS))
     heads = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_heads.py")).read()
     for c in HEAD_CHECKS:

@@ -341,26 +341,31 @@ def test_case_coverage():
     assert all(2 <= c[3] <= 4 for c in CASES if c[0].startswith("cfg"))
 
 
-# Every kernel launch and helper call of mmmot_fusion_det_fwd, in source order (tensor-core path, then FP32), with the
-# checks that hold its output: this file's CHECKS or tests/test_heads.py's HEAD_CHECKS.
+# The functions the stage runs and, per function, every kernel launch and helper call in its body, in source order, with
+# the checks that hold its output: this file's CHECKS or tests/test_heads.py's HEAD_CHECKS.
 FD_HELPERS = ("gemm_gen_launch", "gemm_simt_launch", "stats_reduce", "gn_finalize")
 LINEAR_CHECKS = ("yp", "yi", "gp", "gi")
 NORM_CHECKS = ("scp_shp", "sci_shi", "stats_affine")
-LAUNCH_SITES = [
-    ("feats_to_rows_kernel", ("f3",)), ("gemm_gen_launch", LINEAR_CHECKS), ("stats_reduce", ("stats",)),
-    ("gn_finalize", NORM_CHECKS), ("fusion_combine_rows_kernel", ("combine", "f3")),
-    ("gemm_gen_launch", ("h1",)), ("gemm_gen_launch", ("h2",)), ("det_score_rows_kernel", ("det",)),
-    ("gemm_simt_launch", LINEAR_CHECKS), ("stats_reduce", ("stats",)), ("gn_finalize", NORM_CHECKS),
-    ("fusion_combine_kernel", ("combine",)), ("gemm_simt_launch", ("h1",)), ("gemm_simt_launch", ("h2",)),
-    ("det_score_kernel", ("det",)),
-]
+LAUNCH_SITES = {
+    "fusion_det_tc": [
+        ("feats_to_rows_kernel", ("f3",)), ("gemm_gen_launch", LINEAR_CHECKS), ("stats_reduce", ("stats",)),
+        ("gn_finalize", NORM_CHECKS), ("fusion_combine_rows_kernel", ("combine", "f3")),
+        ("gemm_gen_launch", ("h1",)), ("gemm_gen_launch", ("h2",)), ("det_score_rows_kernel", ("det",)),
+    ],
+    "fusion_det_fp32": [
+        ("gemm_simt_launch", LINEAR_CHECKS), ("stats_reduce", ("stats",)), ("gn_finalize", NORM_CHECKS),
+        ("fusion_combine_kernel", ("combine",)), ("gemm_simt_launch", ("h1",)), ("gemm_simt_launch", ("h2",)),
+        ("det_score_kernel", ("det",)),
+    ],
+}
 
 
-def test_stage_launch_coverage_guard():
-    """Every launch of mmmot_fusion_det_fwd maps to a check: a launch added, removed or reordered without its entry in
-    LAUNCH_SITES fails here; every check named there is one the GPU test fills, and every check is named."""
-    assert impl_launches("fusion_det.cu", "mmmot_fusion_det_fwd", FD_HELPERS) == [s[0] for s in LAUNCH_SITES]
-    named = {c for _, cs in LAUNCH_SITES for c in cs}
+def test_stage_functions_launch_coverage_guard():
+    """Every launch in the functions the stage runs maps to a check: a launch added, removed or reordered without its
+    entry in LAUNCH_SITES fails here; every check named there is one the GPU test fills, and every check is named."""
+    for func, sites in LAUNCH_SITES.items():
+        assert impl_launches("fusion_det.cu", func, FD_HELPERS) == [s[0] for s in sites], func
+    named = {c for sites in LAUNCH_SITES.values() for _, cs in sites for c in cs}
     every = set(CHECKS["C"]) | set(HEAD_CHECKS)
     assert named == every, named ^ every
     heads = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_heads.py")).read()

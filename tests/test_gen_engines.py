@@ -43,7 +43,7 @@ def uniform_lengths(S):
 
 
 # ------------------------------------------------------------------------------------------------ GPU: pairwise layer 1
-# affinity.cu:339-343: [conv1.0 ; new/end conv0] 512 -> 1024 on the generated pairwise tensor, uniform tiling, S = n*m
+# affinity.cu affinity_tc layer 1: [conv1.0 ; new/end conv0] 512 -> 1024 on the generated pairwise tensor, uniform tiling, S = n*m
 PAIR_SHAPES = [(128, 128, 3), (127, 128, 4), (1, 128, 6), (20, 45, 5), (8, 8, 6), (2, 300, 4), (256, 256, 3)]
 PAIR_CASES = [(op, n, m, G) for op in (GEN.MUL, GEN.ABS, GEN.SUB) for n, m, G in PAIR_SHAPES]
 
@@ -83,8 +83,8 @@ def test_pairwise_vs_fp64(op, n, m, G):
 
 
 # ------------------------------------------------------------------------------------------------ GPU: GEN_NORM
-# (M, K, ld_src, S, groups, dbg).  affinity.cu:430 (layer 2: K = 512, M = 512, ld_src = 1024 reads y01's first 512
-# channels), affinity.cu:437 (layer 3: M = 128, ld_src = 512).  Enough groups that persistent CTAs see several groups
+# (M, K, ld_src, S, groups, dbg).  affinity.cu affinity_tc layer 2 (K = 512, M = 512, ld_src = 1024 reads y01's first
+# 512 channels) and layer 3 (M = 128, ld_src = 512).  Enough groups that persistent CTAs see several groups
 # (the per-group affine staging).  The last five are the engine's former single-group linear test (ld_src = K).
 NORM_UNIFORM = [(512, 512, 1024, 300, 48, 0), (512, 512, 1024, 512, 36, 0), (512, 512, 1024, 400, 40, 4096),
                 (512, 512, 512, 300, 48, 4096), (128, 512, 512, 300, 80, 0), (128, 512, 512, 512, 80, 0),
@@ -140,7 +140,7 @@ def _table_with_gaps(tiles, every):
 
 
 # (name, M, K, tiles builder, dbg): pointnet_tc (layers 3, 4: GEN_NORM over ragged per-pair point ranges, K = 64,
-# M = 64 / 128), affinity.cu:393 (new/end layer 2: K = 512, M = 128, groups 2g / 2g+1 of lengths m / n)
+# M = 64 / 128), affinity_tc (new/end layer 2: K = 512, M = 128, groups 2g / 2g+1 of lengths m / n)
 def _pn_table(seed, pairs=40, L=8):
     split = _ragged_split(seed, pairs, L, 1, 200, ones=3)
     tiles = _table_with_gaps(pn_tiles_host(split, pairs, L), 7)
@@ -174,18 +174,18 @@ def test_gen_norm_table_vs_fp64(name, M, K, build, dbg):
 # ------------------------------------------------------------------------------------------------ GPU: GEN_COPY
 # (name, M, K, ld_src, src offset, relu, layout): layout = ("table", builder) or ("uniform", S, groups, x_gs)
 COPY_CASES = [
-    ("ne_l1", 512, 512, 512, 0, 0, ("table", ne_table)),                               # affinity.cu:388
+    ("ne_l1", 512, 512, 512, 0, 0, ("table", ne_table)),                               # affinity_tc new/end layer 1
     ("ne_l1_256", 512, 512, 512, 0, 0, ("table", lambda: ne_table(G=4, n=256, m=200))),
     ("pn_u_120", 512, 1024, 1024, 0, 0, ("uniform", 120, 1, 120)),                       # pointnet_tc U, S = pairs*L
     ("pn_u_400", 512, 1024, 1024, 0, 0, ("uniform", 400, 1, 400)),
     ("pn_conv2_L40", 512, 512, 512, 0, 0, ("uniform", 40, 5, 40)),                       # pointnet_tc conv2, groups = pairs
     ("pn_conv2_L400", 512, 512, 512, 0, 0, ("uniform", 400, 2, 400)),
-    ("fusion_a", 512, 1024, 1536, 0, 0, ("uniform", 64, 3, 64)),                          # fusion_det.cu:179, stacks 0+1
-    ("fusion_bc_img", 512, 512, 1536, 0, 0, ("uniform", 128, 3, 128)),                    # fusion_det.cu:179, stack 0
-    ("fusion_bc_lidar", 512, 512, 1536, 512, 0, ("uniform", 256, 2, 256)),                # fusion_det.cu:179, stack 1
-    ("wdet_1", 512, 512, 512, 0, 1, ("uniform", 420, 1, 420)),                           # fusion_det.cu:205, 3 rows per det
+    ("fusion_a", 512, 1024, 1536, 0, 0, ("uniform", 64, 3, 64)),                          # fusion_det_tc inputs, stacks 0+1
+    ("fusion_bc_img", 512, 512, 1536, 0, 0, ("uniform", 128, 3, 128)),                    # fusion_det_tc inputs, stack 0
+    ("fusion_bc_lidar", 512, 512, 1536, 512, 0, ("uniform", 256, 2, 256)),                # fusion_det_tc inputs, stack 1
+    ("wdet_1", 512, 512, 512, 0, 1, ("uniform", 420, 1, 420)),                           # fusion_det_tc w_det1, 3 rows per det
     ("wdet_1_576", 512, 512, 512, 0, 1, ("uniform", 576, 1, 576)),
-    ("wdet_2", 256, 512, 512, 0, 1, ("uniform", 400, 1, 400)),                           # fusion_det.cu:209
+    ("wdet_2", 256, 512, 512, 0, 1, ("uniform", 400, 1, 400)),                           # fusion_det_tc w_det2
 ]
 
 
@@ -361,12 +361,12 @@ def bench_site_classes(lib):
             if NM < 64:
                 continue
             lengths = uniform_lengths(NM)
-            add(("affinity.cu:339-343", cfg, n), site_classes(lib, op, 1024, 512, 512, "uniform", lengths, m=n))
+            add(("affinity.cu affinity_tc l1", cfg, n), site_classes(lib, op, 1024, 512, 512, "uniform", lengths, m=n))
             ne = [t[2] for t in ne_tiles_host(1, n, n, 0)[0]]
-            add(("affinity.cu:388", cfg, n), site_classes(lib, GEN.COPY, 512, 512, 512, "table", ne))
-            add(("affinity.cu:393", cfg, n), site_classes(lib, GEN.NORM, 128, 512, 512, "table", ne))
-            add(("affinity.cu:430", cfg, n), site_classes(lib, GEN.NORM, 512, 512, 1024, "uniform", lengths))
-            add(("affinity.cu:437", cfg, n), site_classes(lib, GEN.NORM, 128, 512, 512, "uniform", lengths))
+            add(("affinity.cu affinity_tc ne_l1", cfg, n), site_classes(lib, GEN.COPY, 512, 512, 512, "table", ne))
+            add(("affinity.cu affinity_tc ne_l2", cfg, n), site_classes(lib, GEN.NORM, 128, 512, 512, "table", ne))
+            add(("affinity.cu affinity_tc l2", cfg, n), site_classes(lib, GEN.NORM, 512, 512, 1024, "uniform", lengths))
+            add(("affinity.cu affinity_tc l3", cfg, n), site_classes(lib, GEN.NORM, 128, 512, 512, "uniform", lengths))
         if cfg == "cfg5":
             continue
         L = 2 * c["n"]
@@ -384,10 +384,10 @@ def bench_site_classes(lib):
             if L >= 64:
                 Kf = (1024,) if c["fusion"] == "A" else (512,)
                 for K in Kf:
-                    add(("fusion_det.cu:179", cfg, pairs), site_classes(lib, GEN.COPY, 512, K, 1536, "uniform", uniform_lengths(L)))
+                    add(("fusion_det.cu fusion_det_tc inputs", cfg, pairs), site_classes(lib, GEN.COPY, 512, K, 1536, "uniform", uniform_lengths(L)))
                 rows = uniform_lengths(pairs * L * 3)
-                add(("fusion_det.cu:205", cfg, pairs), site_classes(lib, GEN.COPY, 512, 512, 512, "uniform", rows))
-                add(("fusion_det.cu:209", cfg, pairs), site_classes(lib, GEN.COPY, 256, 512, 512, "uniform", rows))
+                add(("fusion_det.cu fusion_det_tc w_det1", cfg, pairs), site_classes(lib, GEN.COPY, 512, 512, 512, "uniform", rows))
+                add(("fusion_det.cu fusion_det_tc w_det2", cfg, pairs), site_classes(lib, GEN.COPY, 256, 512, 512, "uniform", rows))
     return out
 
 
