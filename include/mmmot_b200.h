@@ -468,7 +468,7 @@ int mmmot_set_kseg(int chunks);
  *   bit 10 (1024) generated-operand engine (csrc/gemm_gen.cuh): producers without the software pipeline, every GEN
  *                 (GEN_NORM: plain producers instead of TMA-staged source rows)
  *   bit 11 (2048) channel-major conv epilogue through the accumulator image in shared memory instead of from the
- *                 registers (mmmot_debug_conv_epilogue)
+ *                 registers, K-segmented launches included (mmmot_debug_conv_epilogue, mmmot_debug_conv_seg_epilogue)
  *   bit 12 (4096) generated-operand engine: GEN_NORM producers with the software pipeline (prefetching variant)
  *                 instead of TMA-staged source rows
  *   bit 13 (8192) PointNet layers 3, 4 through norm_split + the TMA-fed kernel instead of GEN_NORM producers
@@ -585,10 +585,16 @@ int mmmot_debug_linear_planar(const void* Wp, float wp_scale, const float* bias,
  *   fused launch ran (it needs both compact tiles; debug bit 15 forces the two launches), 0 for the two launches.
  * vgg_conv01_plan: *fused (host) = whether vgg_conv01 of that shape takes the fused launch (given both compact tiles),
  *   computed on the host without any CUDA call under the current mmmot_set_debug / mmmot_set_kseg state.
- * conv_epilogue: the epilogue the channel-major kernel runs under that launch plan (same arguments as conv_plan): 1 =
- *   from the wgmma accumulators in registers, stored by TMA; 0 = through the accumulator image in shared memory (debug
- *   bit 11, K segments, M < 64) or the pixel-major kernel; computed on the host. */
+ * conv_epilogue: the epilogue the channel-major kernel runs under that launch plan (same arguments as conv_plan), for
+ *   single-pass K only: 1 = from the wgmma accumulators in registers, stored by TMA; 0 = through the accumulator image in
+ *   shared memory (debug bit 11, M < 64), K segments (see conv_seg_epilogue) or the pixel-major kernel; computed on the
+ *   host.
+ * conv_seg_epilogue: 1 if that launch plan runs K segments on the epilogue from the wgmma accumulators, which folds the
+ *   segments' partial sums from the registers through kseg_scratch (M a multiple of 64); 0 otherwise (single pass,
+ *   pixel-major kernel, or the accumulator image: debug bit 11, M not a multiple of 64); same arguments as conv_plan,
+ *   computed on the host. */
 int mmmot_debug_conv_epilogue(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg);
+int mmmot_debug_conv_seg_epilogue(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg);
 int mmmot_debug_conv_plan(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg, int* plan);
 int mmmot_debug_conv_layer(const void* Wp, const void* Wpx, float wp_scale, const float* bias, const void* Xhi, long x_plane,
                            int n_img, int H, int W, int C, int M, void* Yhi, long y_plane, long y_plane_pooled,

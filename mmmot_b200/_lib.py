@@ -78,6 +78,7 @@ SIGNATURES = {
     "mmmot_debug_linear_planar": (_i, [_vp, _f, _vp, _vp, _vp, _i, _i, _l, _vp]),
     "mmmot_debug_conv_plan": (_i, [_i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(_i)]),
     "mmmot_debug_conv_epilogue": (_i, [_i, _i, _i, _i, _i, _i, _i]),
+    "mmmot_debug_conv_seg_epilogue": (_i, [_i, _i, _i, _i, _i, _i, _i]),
     "mmmot_debug_conv_layer": (_i, [_vp, _vp, _f, _vp, _vp, _l, _i, _i, _i, _i, _i, _vp, _l, _l, ctypes.POINTER(_i), _vp, _vp,
                                     _vp, ctypes.POINTER(_i), _vp]),
     "mmmot_debug_vgg_conv0": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _f, _vp, _vp, _l, _vp, _vp, ctypes.POINTER(_i), _vp]),

@@ -323,11 +323,17 @@ extern "C" int mmmot_debug_conv_plan(int n_img, int H, int W, int C, int M, int 
   return 0;
 }
 
-// Which epilogue that launch plan runs: 1 = from the wgmma accumulators, 0 = through the accumulator image (or the
-// pixel-major kernel).
+// Which epilogue that launch plan runs in a single pass: 1 = from the wgmma accumulators, 0 = otherwise (through the
+// accumulator image, K-segmented, or the pixel-major kernel).
 extern "C" int mmmot_debug_conv_epilogue(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg) {
   if (n_img <= 0 || H <= 0 || W <= 0 || C <= 0 || C % tc::BK || M <= 0) return MMMOT_E_ARG;
   return conv_plan(M, false, n_img, H, W, C, want_pool != 0, use_kseg != 0, mm_debug_flags(), mm_kseg_chunks()).acc_epi;
+}
+
+// Whether that launch plan runs K segments with the epilogue from the wgmma accumulators (1) or not (0).
+extern "C" int mmmot_debug_conv_seg_epilogue(int n_img, int H, int W, int C, int M, int want_pool, int use_kseg) {
+  if (n_img <= 0 || H <= 0 || W <= 0 || C <= 0 || C % tc::BK || M <= 0) return MMMOT_E_ARG;
+  return conv_plan(M, false, n_img, H, W, C, want_pool != 0, use_kseg != 0, mm_debug_flags(), mm_kseg_chunks()).seg_acc;
 }
 
 // One VGG conv layer (3x3 pad 1 + bias + ReLU) through gemm_tma_launch_conv with the arguments mmmot_appearance_fwd

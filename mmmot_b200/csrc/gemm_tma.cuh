@@ -12,8 +12,8 @@
 // chains of the tile's 128 rows x column half h, then runs the epilogue of that half), warp 8 is the loader (weights
 // by cp.async.bulk, operand boxes by TMA; warps 9-11 only complete its warpgroup).  Ring of 4 x 48 KB stages.
 // gemm_tma_kernel<EPI> is instantiated once per consumer: EPI_MAT (mat_consumer, 1x1 contractions), EPI_CONV_IMAGE
-// (conv_image_consumer: K-segmented convs, or with GroupNorm partials) and EPI_CONV_ACC (conv_acc_consumer: single-pass
-// convs from the wgmma fragments).  The first two hand each tile over as an accumulator image (128 x 256 fp32) over the
+// (conv_image_consumer: convs with GroupNorm partials, or under debug bit 11) and EPI_CONV_ACC (conv_acc_consumer: convs
+// from the wgmma fragments, K segments included).  The first two hand each tile over as an accumulator image (128 x 256 fp32) over the
 // ring's first 128 KB, so the loader starts the next tile once the epilogue has read it; their FP16 outputs are
 // transposed through a per-warp smem scratch (store_rows) so each lane stores 64 contiguous bytes per plane.
 #pragma once
@@ -57,7 +57,8 @@ struct TmaP {
   int n_img, H, W, C;       // conv geometry (C = input channels; 0 in a matrix launch)
   long plane_elems;         // output: distance (in fp16 elements) between the hi and lo planes
   int ksegs, kc_per_seg;    // conv: K is accumulated in `ksegs` passes of kc_per_seg chunks whose fp32
-  float* acc_scratch;       // partial sums are combined in fp32 RN through acc_scratch[pixel][M] (see launcher)
+  float* acc_scratch;       // partial sums are combined in fp32 RN through acc_scratch: [tile*256 + column][M]
+                            // (conv_image_consumer), or that range's blocks in fragment order (seg_fold)
   int halo, pool;           // halo: pixel-major kernel only (gemm_tma_px.cuh), vertical taps from one halo box
                             // pool: fused 2x2 max-pool in the conv epilogue (both kernels): the pooled map is written
   unsigned long long* pool_sum;   // channel-major conv + pool: if set, the pooled values are also summed per (image, channel)
@@ -258,7 +259,7 @@ __device__ __forceinline__ void store_rows(const float (&x)[32], bool ok, __half
 // Output: per 32 columns (or the 32 pooled pixels of a half) the FP16 hi and lo values go pixel-major into the
 // warpgroup's two staging buffers (stmatrix.trans, 128-byte swizzle) and one thread stores them by TMA through the
 // NHWC maps out_hi / out_lo, which clip partial boxes.  Only the warpgroup synchronises; the ring is never waited on.
-// Single-pass K only (conv_plan): K-segmented launches take conv_image_consumer.
+// K-segmented launches fold their segments' partial sums first (seg_fold).
 template <int BX>
 __device__ __forceinline__ void conv_pool_epi(const TmaP& P, const float (&x)[2][64], int half, int w, int lane, int mg,
                                               int i0, int y0, int x0, int lby, float& amax, uint32_t buf) {
@@ -340,6 +341,55 @@ __device__ __forceinline__ void conv_pool_epi(const TmaP& P, const float (&x)[2]
   if (P.pool_sum) flush();
 }
 
+// K-segmented launches of conv_acc_consumer: fold segment `seg`'s fragments into the tile's running fp32 sums S, the
+// same operations in the same order as conv_image_consumer, so the outputs are byte-identical: after segment 0
+// S = RN(v s), after each later one S = fmaf(v, s, S).  S lives in acc_scratch between segments, one block per (tile,
+// m-group) where the tile-order layout [tile*256 + column][M] puts it (256 x min(128, M - 128 mg) floats), in fragment
+// order: float4 piece pc of m64 block mb of consumer thread tid at [mb][pc][tid], so a warp instruction covers 512
+// contiguous bytes; m64 blocks of rows >= M are neither loaded nor stored (conv_plan takes this path for M % 64 == 0
+// only, so every block is whole).  Every S of a batch is loaded and folded
+// before any store, so no load waits on a store of the same boundary; a thread reads back only what it wrote, so
+// program order suffices (ld.global.cg: the non-coherent path could return stale lines written by this kernel).
+// On return acc holds S; after the last segment nothing is stored.
+constexpr int SEG_BATCH = 8;   // float4 pieces loaded together
+__device__ __forceinline__ void seg_fold(float (&acc)[2][64], const TmaP& P, int nt, int mg, int seg) {
+  const GemmP& p = P.t.g;
+  const float s = P.t.out_scale;
+  float4* blk = reinterpret_cast<float4*>(P.acc_scratch + ((long)nt * BN * p.M + (long)mg * 128 * BN)) +
+                (opaque(threadIdx.x) & 255);
+#pragma unroll
+  for (int mb = 0; mb < 2; mb++) {
+    if (mg * 128 + mb * 64 >= p.M) continue;
+    const float4* sp = blk + mb * 16 * 256;
+    if (seg == 0) {
+#pragma unroll
+      for (int i = 0; i < 64; i++) acc[mb][i] = __fmul_rn(acc[mb][i], s);
+      continue;
+    }
+#pragma unroll
+    for (int b = 0; b < 16; b += SEG_BATCH) {
+      float4 S[SEG_BATCH];
+#pragma unroll
+      for (int i = 0; i < SEG_BATCH; i++) S[i] = __ldcg(sp + (b + i) * 256);
+#pragma unroll
+      for (int i = 0; i < SEG_BATCH; i++) {
+        float* v = &acc[mb][4 * (b + i)];
+        v[0] = fmaf(v[0], s, S[i].x); v[1] = fmaf(v[1], s, S[i].y);
+        v[2] = fmaf(v[2], s, S[i].z); v[3] = fmaf(v[3], s, S[i].w);
+      }
+    }
+  }
+  if (seg == P.ksegs - 1) return;
+#pragma unroll
+  for (int mb = 0; mb < 2; mb++) {
+    if (mg * 128 + mb * 64 >= p.M) continue;
+#pragma unroll
+    for (int pc = 0; pc < 16; pc++)
+      __stcg(blk + (mb * 16 + pc) * 256,
+             make_float4(acc[mb][4 * pc], acc[mb][4 * pc + 1], acc[mb][4 * pc + 2], acc[mb][4 * pc + 3]));
+  }
+}
+
 __device__ __forceinline__ void conv_acc_consumer(const TmaP& P, uint32_t base, uint32_t bar0, const CUtensorMap* out_hi,
                                                   const CUtensorMap* out_lo) {
   const GemmP& p = P.t.g;
@@ -377,13 +427,20 @@ __device__ __forceinline__ void conv_acc_consumer(const TmaP& P, uint32_t base, 
     int i0_, y0_, x0_;
     conv_origin(P, nt, i0_, y0_, x0_);
     {
-      mma_segment(acc, P, base, bar0, half, tid & 31, 0, KC, it);
+      // K segments run back to back: the loader streams through their boundaries, where seg_fold carries the partial
+      // sums through acc_scratch (single-pass launches: one segment of KC chunks)
+      for (int seg = 0; seg < P.ksegs; seg++) {
+        const int kc_lo = seg * P.kc_per_seg;
+        mma_segment(acc, P, base, bar0, half, tid & 31, kc_lo, min(KC, kc_lo + P.kc_per_seg), it);
+        if (P.ksegs > 1 && !(P.t.dbg & MM_DBG_SKIP_EPI)) seg_fold(acc, P, opaque(nt), opaque(mg_), seg);
+      }
       if (P.t.dbg & MM_DBG_SKIP_EPI) continue;
       // Everything below derives from values laundered here, so the compiler cannot hoist the epilogue's lane and tile
       // arithmetic above the main loop, where it would be live next to the 128 accumulators.
       const int lane = opaque(threadIdx.x) & 31, w = (threadIdx.x >> 5) & 3, g = lane >> 2;
       const int mg = opaque(mg_), i0 = opaque(i0_), y0 = opaque(y0_), x0 = opaque(x0_);
-      // bias (+ ReLU) in place: fmaf(v, s, b) as one pass, S + b after K segments
+      // bias (+ ReLU) in place: fmaf(v, s, b) as one pass, S + b after K segments (seg_fold left S in acc)
+      const bool segmented = P.ksegs > 1;
 #pragma unroll
       for (int mb = 0; mb < 2; mb++)
 #pragma unroll
@@ -395,7 +452,7 @@ __device__ __forceinline__ void conv_acc_consumer(const TmaP& P, uint32_t base, 
 #pragma unroll
             for (int e = 0; e < 2; e++) {
               float& v = acc[mb][4 * j + 2 * h + e];
-              const float a = fmaf(v, s, bv);
+              const float a = segmented ? __fadd_rn(v, bv) : fmaf(v, s, bv);
               v = p.relu ? fmaxf(a, 0.f) : a;
             }
         }
@@ -1024,7 +1081,8 @@ struct ConvPlan {
   int bx, by, bi;          // box of 256 pixels (powers of two)
   int ksegs, kc_per_seg;   // K accumulated in ksegs passes of kc_per_seg 32-wide chunks
   int tiles_x, tiles_y, num_tiles;   // column tiles (boxes); the channel-major kernel runs ceil(M/128) row tiles of each
-  int acc_epi;             // channel-major: epilogue from the wgmma accumulators, TMA stores (EPI_CONV_ACC)
+  int acc_epi;             // channel-major, single-pass K: epilogue from the wgmma accumulators, TMA stores (EPI_CONV_ACC)
+  int seg_acc;             // channel-major, K segments: the same kernel, partial sums folded from the fragments (seg_fold)
 };
 // want_pool: the caller takes a fused pooled map; use_kseg: the caller provides K-segment scratch.
 // dbg / seg_chunks: mmmot_set_debug / mmmot_set_kseg state.
@@ -1061,10 +1119,14 @@ static inline ConvPlan conv_plan(int M, bool part, int n_img, int H, int W, int 
   }
   c.tiles_x = mm_cdiv(W, c.bx); c.tiles_y = mm_cdiv(H, c.by);
   c.num_tiles = c.tiles_x * c.tiles_y * mm_cdiv(n_img, c.bi);
-  // The accumulator epilogue stores 64-channel boxes and runs single-pass K only: combining K segments' partial sums
-  // from the registers through L2 measured slower than the accumulator image on the H100 (DESIGN §4.2).  Debug bit 11
-  // keeps the accumulator-image epilogue (A/B runs).
-  c.acc_epi = !c.px && !part && !(dbg & MM_DBG_CONV_IMAGE) && M >= 64 && c.ksegs == 1;
+  // The accumulator epilogue stores 64-channel boxes; with K segments it also carries the partial sums between them
+  // (seg_fold), so no segment boundary waits for an accumulator image.  GroupNorm partials (part) need the image.
+  // seg_fold keeps whole m64 blocks of partial sums, so K segments need M % 64 == 0 (a partial block would not fit its
+  // place in the [tiles*256][M] scratch); other M keep the image.  Debug bit 11 keeps the accumulator-image epilogue
+  // (A/B runs).
+  const bool acc = !c.px && !part && !(dbg & MM_DBG_CONV_IMAGE) && M >= 64;
+  c.acc_epi = acc && c.ksegs == 1;
+  c.seg_acc = acc && c.ksegs > 1 && M % 64 == 0;
   return c;
 }
 
@@ -1111,7 +1173,7 @@ static int gemm_tma_launch_conv(const GemmP& g0, const uint4* Wp, float out_scal
   }
   const long total = (long)g.num_tiles * P.t.m_tiles;
   const int grid = (int)(total < sms ? total : sms);
-  if (c.acc_epi) {
+  if (c.acc_epi || c.seg_acc) {
     static std::atomic<unsigned long long> attr{0};
     MM_TRY(mm_ensure_smem(tma::gemm_tma_kernel<tma::EPI_CONV_ACC>, tma::T_CONV_SMEM_BYTES, attr));
     const int sh = c.pool ? 1 : 0;

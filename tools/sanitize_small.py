@@ -1,6 +1,6 @@
 """Small runs of every device path for compute-sanitizer (memcheck / racecheck): eval forward + LP on both engines
 (N=M=8, 32x32 crops; the tensor-core engine forced so that its kernels, incl. the first layer's in-kernel operand
-producers, are the ones checked), all fusion / softmax / affinity variants, end_mode max, a three-frame sample and its
+producers and VGG conv5-conv12's K-segmented accumulator epilogue with its fused pools, are the ones checked), all fusion / softmax / affinity variants, end_mode max, a three-frame sample and its
 assignment programme, the training-mode forward with DropBlock + Dropout, the pinned-host pipeline, LiDAR cropping in
 both precisions and image crop-and-resize.
   compute-sanitizer --tool memcheck  python tools/sanitize_small.py
